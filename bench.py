@@ -9,8 +9,7 @@ another BASELINE configuration as the bench line.  Each step uses fresh seeds.
   value     rounds/s with the seeds already resident in HBM (kernel only, CUDA events, max over ranks)
   e2e       rounds/s through the public API with HOST buffers: seeds host->device, kernel, summaries device->host
             (commit counts, state keys, rounds, status land in caller-owned arrays), every step
-  roofline  algorithmic bytes (SURVEY §8d formula over the run's own event counters) / kernel time vs the measured
-            HBM copy peak; the measured DRAM traffic (ncu) and its own rate are reported next to it
+  roofline  algorithmic bytes (SURVEY §8d formula over the run's own event counters) / kernel time vs the HBM peak
   parity    EVERY instance of the last timed batch is compared with the CPU oracle (commit counts, state keys,
             event/RNG counters) outside the timed region ("checked N of N"; a bounded sample only where the oracle
             would need more than a minute, and then it says so)
@@ -22,6 +21,7 @@ another BASELINE configuration as the bench line.  Each step uses fresh seeds.
 Multi-GPU: one process per GPU under torchrun through `ShardedBatchSimulator`: instances sharded with no data-path
 collective; one NCCL all-gather of the per-instance summaries at the end of every step.  "scaling": "weak" (the
 configuration's batch per GPU) unless `--scaling strong` (the configuration's batch split over the GPUs).
+`--dump-outputs DIR` writes the results of the last timed step (see dump_outputs) for output-by-output comparison of builds.
 """
 import argparse
 import json
@@ -59,6 +59,7 @@ CONFIGS = {
                  "base seeds swept per step (BASELINE configs[4], SURVEY 8d.5)"),
 }
 ORACLE_PARITY_BUDGET_S = 45.0   # full-batch compare whenever the oracle needs less than this; else a strided sample
+DUMP_LIMIT_BYTES = 60 * 10**6   # --dump-outputs: array bytes in all (< 64 MB with the .npy headers); a fixed, seeded sample beyond
 
 
 def make_sim(seeds, nodes, device=0, **kw):
@@ -96,27 +97,13 @@ def effective_cores():
     return max(1, n)
 
 
-def ncu_traffic_bytes(config_id, per_gpu, kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the event-loop kernel, from the committed ncu
-    --set full capture (profiles/traffic.json: one entry per (config, kernel)); None if there is no matching capture."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            t = json.load(f)
-        for e in t.get("captures", []):
-            if e.get("config") == config_id and e.get("instances") == per_gpu and e.get("kernel") == kernel:
-                return e["dram_bytes_per_launch"], e.get("source")
-    except Exception:
-        pass
-    return None, None
-
-
 def measured_peak_gbs():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     try:
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -274,24 +261,37 @@ def gpu_arrays(res):
     return {"commit_counts": res.commit_counts, "last_states": res.last_committed_states, "counters": res.counters}
 
 
-def roofline_block(cfg_id, cfg, per_gpu, counters, kernel_ms, kernel_name):
+def roofline_block(cfg, counters, kernel_ms, kernel_name):
     peak, peak_src = measured_peak_gbs()
     bytes_launch = algorithmic_bytes(counters, cfg["nodes"])
     achieved = bytes_launch / (kernel_ms * 1e-3) / 1e9
-    traffic, traffic_src = ncu_traffic_bytes(cfg_id, per_gpu, kernel_name)
-    block = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-             "traffic_source": traffic_src, "peak_source": peak_src, "kernel": kernel_name, "kernel_ms": kernel_ms,
-             "algorithmic_bytes_per_launch": bytes_launch,
-             "events_per_s": float(counters[:, 0:4].sum()) / (kernel_ms * 1e-3),
-             "note": "achieved/frac are the ALGORITHMIC (layout-independent) bytes of SURVEY 8d over the kernel time; the kernel is "
-                     "issue/latency-bound, its real DRAM traffic is `traffic` (ncu) = dram_achieved GB/s"}
-    if traffic:
-        block["dram_achieved"] = traffic / (kernel_ms * 1e-3) / 1e9
-        block["dram_frac"] = block["dram_achieved"] / peak
-    return block
+    return {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
+            "peak_source": peak_src, "kernel": kernel_name, "kernel_ms": kernel_ms,
+            "algorithmic_bytes_per_launch": bytes_launch,
+            "events_per_s": float(counters[:, 0:4].sum()) / (kernel_ms * 1e-3),
+            "note": "achieved/frac are the ALGORITHMIC (layout-independent) bytes of SURVEY 8d over the kernel time, not "
+                    "measured DRAM traffic"}
 
 
-def measure_side_config(cfg_id, device, steps=2, warmup=1):
+def dump_outputs(outdir, commit_counts, states, active_rounds, status, counters):
+    """--dump-outputs: what the timed path returned in its last step for the whole job (all ranks' shards, in instance
+    order), one float64 .npy per array.  The 64-bit state keys are split into their two exact 32-bit halves.  instances.npy
+    lists the rows written: every instance, or a fixed, seeded sample when the whole would exceed DUMP_LIMIT_BYTES."""
+    arrays = {"commit_counts": commit_counts, "last_committed_states_hi": states >> np.uint64(32),
+              "last_committed_states_lo": states & np.uint64(0xffffffff), "active_rounds": active_rounds,
+              "status": status, "counters": counters}
+    n = len(status)
+    row_bytes = 8 * (1 + sum(a.size // n for a in arrays.values()))
+    rows = np.arange(n)
+    if row_bytes * n > DUMP_LIMIT_BYTES:
+        rows = np.sort(np.random.default_rng(0).choice(n, DUMP_LIMIT_BYTES // row_bytes, replace=False))
+    os.makedirs(outdir, exist_ok=True)
+    np.save(os.path.join(outdir, "instances.npy"), rows.astype(np.float64))
+    for name, a in arrays.items():
+        np.save(os.path.join(outdir, name + ".npy"), a[rows].astype(np.float64))
+
+
+def measure_side_config(cfg_id, device, steps, warmup):
     """One of the non-headline BASELINE configurations on one GPU: kernel time (CUDA events, seeds resident), e2e time
     (host buffers), full parity and the CPU baseline.  Used for the `configs` block of the default line."""
     import torch
@@ -323,7 +323,7 @@ def measure_side_config(cfg_id, device, steps=2, warmup=1):
     out = {"workload": cfg["text"], "kernel": kernel, "kernel_ms": k_ms, "value": rounds / (sum(kms) * 1e-3), "unit": UNIT,
            "e2e": e2e_rounds / e2e_s, "steps": steps, "warmup": warmup,
            "events_per_s": float(res.counters[:, 0:4].sum()) / (k_ms * 1e-3),
-           "roofline": roofline_block(cfg_id, cfg, I, res.counters, k_ms, kernel),
+           "roofline": roofline_block(cfg, res.counters, k_ms, kernel),
            "flagged_instances": int(((res.status & 0x9E) != 0).sum()),
            "parity": parity, "cpu_baseline": base, "e2e_over_cpu": (e2e_rounds / e2e_s) / base["value"]}
     sim.close()
@@ -362,6 +362,7 @@ def main():
                     help="weak: the configuration's batch per GPU; strong: the configuration's batch split over the GPUs")
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the oracle (no parity check, no cpu_baseline)")
     ap.add_argument("--no-configs", action="store_true", help="skip the per-config block of the default line")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the results of the last timed step as DIR/<name>.npy (float64)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -378,6 +379,7 @@ def main():
     import torch
     import torch.distributed as dist
     from librabft_simulator_b200 import ShardedBatchSimulator
+    from librabft_simulator_b200.distributed import ShardedResult, all_gather_rows
 
     if not torch.cuda.is_available():
         raise SystemExit("bench.py needs a CUDA device (there is no CPU fallback for the product path)")
@@ -435,7 +437,7 @@ def main():
     h2d_bytes, d2h_bytes = int(sim.timing.h2d_bytes), int(sim.timing.d2h_bytes)
 
     # ---------------- value leg: inputs resident in HBM, device-timed kernel ----------------
-    kernel_ms, rounds_dev, last, last_seeds, flagged = [], 0.0, None, None, 0
+    kernel_ms, rounds_dev, last, last_seeds, flagged, block = [], 0.0, None, None, 0, None
     barrier()
     for s in range(args.steps):
         last_seeds = job_seeds(100 + s)[sharded.lo:sharded.hi]
@@ -444,11 +446,22 @@ def main():
         sim.run_device()                                  # CUDA events on the launching stream around the kernel
         kernel_ms.append(float(sim.timing.sim_ms))
         last = sim.download(strict=False)
-        sharded.gather(last)
+        block = sharded.gather(last)
         rounds_dev += float(last.active_rounds.sum())
         flagged += int(((last.status & 0x9E) != 0).sum())  # any LBFT_ST_ERROR_MASK bit (capacity / invariant / epoch)
     barrier()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:  # (every rank takes part in the gathers)
+        job = ShardedResult(last, block, sharded.hi - sharded.lo, nodes, sharded.lo, sharded.hi)
+
+        def job_rows(a):  # a per-instance array of this rank's shard, gathered over the ranks
+            if not distributed:
+                return a
+            return all_gather_rows(torch.as_tensor(a.astype(np.int64), device="cuda"), world, dist).cpu().numpy()
+
+        status, counters = job_rows(last.status), job_rows(last.counters)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, job.commit_counts, job.last_committed_states, job.active_rounds, status, counters)
 
     dev_seconds = sum(kernel_ms) / 1e3
     stats = torch.tensor([dev_seconds, e2e_seconds], dtype=torch.float64, device="cuda")
@@ -469,7 +482,7 @@ def main():
             "config": {"workload": cfg["text"], "baseline_config": args.config,
                        "seeds": "base_seed %d + instance, fresh block per step" % cfg["base_seed"],
                        "instances_total": total, "instances_per_gpu": per_gpu,
-                       "l2": "state working set %.0f MB per GPU (126 MB L2); every step re-initialises it" % (dev_bytes / 1e6),
+                       "l2": "state working set %.0f MB per GPU (50 MB L2); every step re-initialises it" % (dev_bytes / 1e6),
                        "parallelism": "instances sharded over %d GPU(s) (ShardedBatchSimulator); one NCCL all-gather of {commit counts, "
                                       "state keys, rounds} per step" % world},
             "e2e": {"value": e2e_rounds / e2e_seconds, "unit": UNIT, "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": d2h_bytes,
@@ -477,7 +490,7 @@ def main():
                     "returns": "commit counts [I][N], state keys [I][N], rounds [I], status [I] in caller-owned host arrays",
                     "pipeline": "run_stream: one run in flight per GPU (lbft_run_async / lbft_wait, double-buffered pinned staging)"},
             "gpu_launches": args.steps * 2,
-            "roofline": roofline_block(args.config, cfg, per_gpu, last.counters, k_ms, kernel),
+            "roofline": roofline_block(cfg, last.counters, k_ms, kernel),
             "clocks": clocks,
             "state_bytes_per_instance": words_per_inst * 4,
             "flagged_instances": flagged,  # instances (rank 0, value leg) that hit a capacity/invariant flag: expected 0
@@ -491,7 +504,7 @@ def main():
                 sim.close()
                 side = {}
                 for k in (1, 2, 4, 5):
-                    side[str(k)] = measure_side_config(k, local_rank)
+                    side[str(k)] = measure_side_config(k, local_rank, args.steps, args.warmup)
                 me = {"workload": cfg["text"], "kernel": kernel, "kernel_ms": k_ms, "value": value, "unit": UNIT,
                       "e2e": line["e2e"]["value"], "events_per_s": line["roofline"]["events_per_s"], "roofline": line["roofline"],
                       "flagged_instances": flagged, "parity": parity, "cpu_baseline": base,

@@ -1,4 +1,4 @@
-//! `bft-lib-gpu` — the reference's simulator call shape over the B200 library.
+//! `bft-lib-gpu` — the reference's simulator call shape over the H100 library.
 //!
 //! Replaces, for the LibraBFTv2 + `SimulatedContext` instantiation, `bft_lib::simulator::Simulator`
 //! (bft-lib/src/simulator.rs:26-33): `Simulator::new(seed, nodes, RandomDelay::new(mean, variance), context_factory)`
@@ -6,7 +6,7 @@
 //! librabft-v2/src/main.rs:36-53 and librabft-v2/tests/simulated_run.rs:19-43, switch to `GpuSimulator` and keep
 //! reading `committed_history()` / `last_committed_state()` (bft-lib/src/simulated_context.rs:98-100, 194-196).
 //!
-//! `ffi` mirrors include/lbft.h item by item (checked by tests/test_rust_shim.py in the B200 repository).
+//! `ffi` mirrors include/lbft.h item by item (checked by tests/test_rust_shim.py in this repository).
 use std::os::raw::{c_char, c_int};
 
 use bft_lib::base_types::NodeTime;

@@ -1,4 +1,4 @@
-/* lbft.h — C ABI of the B200-native batched LibraBFTv2 discrete-event simulator.
+/* lbft.h — C ABI of the H100-native batched LibraBFTv2 discrete-event simulator.
  *
  * Drop-in boundary for the ONE hot path of novifinancial/librabft_simulator (reference checkout
  * /root/reference @ cc2ec64d): the discrete-event loop `Simulator::new` + `Simulator::loop_until`

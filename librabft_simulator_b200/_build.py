@@ -1,8 +1,8 @@
 """Build recipes for the native pieces (run by ``__graft_entry__.build()``).
 
-* ``csrc/liblbft_b200.so`` — the product: sm_100a CUDA kernels + the C ABI of ``include/lbft.h``.
+* ``csrc/liblbft_b200.so`` — the product: sm_90a (H100) CUDA kernels + the C ABI of ``include/lbft.h``.
 * ``oracle/liblbft_oracle.so`` and ``tests/hostcore/libhostcore.so`` — test infrastructure only.
-All artefacts are built in-tree (git-ignored, but they travel to the GPU box with the snapshot).
+All artefacts are built in-tree and git-ignored.
 """
 import os
 import shutil
@@ -16,7 +16,8 @@ ORACLE_PATH = os.path.join(ORACLE_DIR, "liblbft_oracle.so")
 HOSTCORE_DIR = os.path.join(ROOT, "tests", "hostcore")
 HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore.so")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
+NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # Translation units of the product library: the host runtime (C ABI) and the kernel instantiations, one group per file so
 # that they compile in parallel and the bench kernel (k_fixed.cu) can be rebuilt alone.
 PRODUCT_UNITS = ["lbft_api.cu", "k_fixed.cu", "k_scan.cu", "k_calendar.cu", "k_heap.cu", "k_wide.cu"]
@@ -42,7 +43,7 @@ def nvcc_path():
 
 
 def build_product(force=False, verbose_ptxas=False, extra_flags=(), lib_path=None):
-    """nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo on every unit (objects in csrc/build/, in parallel), then one
+    """nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo on every unit (objects in csrc/build/, in parallel), then one
     shared library.  Only units older than their sources are recompiled."""
     from concurrent.futures import ThreadPoolExecutor
     lib_path = lib_path or LIB_PATH
@@ -64,7 +65,7 @@ def build_product(force=False, verbose_ptxas=False, extra_flags=(), lib_path=Non
         print("\n".join(outs))
     objs = [os.path.join(objdir, u.replace(".cu", ".o")) for u in PRODUCT_UNITS]
     if jobs or not _newer(lib_path, objs):
-        _run([nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", lib_path] + objs, CSRC)
+        _run([nvcc_path()] + GENCODE + ["-shared", "-o", lib_path] + objs, CSRC)
     return lib_path
 
 
@@ -78,23 +79,31 @@ def build_oracle(force=False):
 
 
 def build_oracle_native():
-    """The CPU-baseline build of the oracle (-O3 -march=native), compiled on the machine that times it (the GPU box: same
-    image, g++ present) into a host-specific file name so that a copy built for another CPU is never loaded.  Falls back
-    to the portable build if no compiler is available.  Returns (path, flags description)."""
+    """The CPU-baseline build of the oracle (-O3 -march=native), compiled on the machine that times it under the temporary
+    directory (the source tree may be read-only there).  The file name carries a hash of the CPU and of the oracle's
+    sources and build recipe, so that neither a copy built for another CPU nor one built from another checkout's sources
+    is ever loaded.  Falls back to the portable build if no compiler is available.  Returns (path, flags description)."""
     import hashlib
     import platform
+    import tempfile
     try:
         cpu = [ln for ln in open("/proc/cpuinfo") if ln.startswith(("model name", "flags"))][:2]
     except OSError:
         cpu = [platform.processor()]
-    tag = hashlib.sha1("".join(cpu).encode()).hexdigest()[:10]
-    path = os.path.join(ORACLE_DIR, "liblbft_oracle_native_%s.so" % tag)
-    srcs = [os.path.join(ORACLE_DIR, f) for f in ("oracle_capi.cpp", "oracle_selftest.cpp", "lbft_oracle.hpp")]
-    if _newer(path, srcs):
+    h = hashlib.sha1("".join(cpu).encode())
+    for src in [os.path.join(ORACLE_DIR, f) for f in ("oracle_capi.cpp", "oracle_selftest.cpp", "lbft_oracle.hpp", "Makefile")] + [
+            os.path.join(ROOT, "include", "lbft.h")]:
+        with open(src, "rb") as f:
+            h.update(f.read())
+    outdir = os.path.join(tempfile.gettempdir(), "lbft-oracle-native-%d" % os.getuid())
+    path = os.path.join(outdir, "liblbft_oracle_native_%s.so" % h.hexdigest()[:16])
+    if os.path.exists(path):
         return path, "-O3 -march=native"
     try:
-        _run(["make", "-B", "liblbft_oracle_native.so"], ORACLE_DIR)
-        os.replace(os.path.join(ORACLE_DIR, "liblbft_oracle_native.so"), path)
+        os.makedirs(outdir, exist_ok=True)
+        tmp = "%s.%d.tmp" % (path, os.getpid())
+        _run(["make", "-B", "liblbft_oracle_native.so", "NATIVE_OUT=" + tmp], ORACLE_DIR)
+        os.replace(tmp, path)
         return path, "-O3 -march=native"
     except Exception:
         return build_oracle(), "-O2 (portable build: native build failed)"

@@ -149,11 +149,12 @@ struct HostSetup {
     // (explicit capacities beyond what the scan queue can encode / scan efficiently select the heap.)
     uint32_t qscan = (N <= 5 && c.max_clock < (1 << 24) - 64) ? 1u : 0u;
     if (c.payload_cap > 255 || c.queue_cap > 512) qscan = 0;
-    // Kernel family.  One thread per instance needs tens of thousands of instances to fill a B200 (65 536 x 4 authors is
-    // exactly one wave of warps) and serialises the 32 instances of a warp through every fan-out; one WARP per instance
+    // Kernel family.  One thread per instance needs tens of thousands of instances to fill an H100 (65 536 x 4 authors is
+    // one wave of warps) and serialises the 32 instances of a warp through every fan-out; one WARP per instance
     // (lbft_wide_kernel) has no cross-instance divergence, splits fan-outs, queue scans and per-author vectors over its
-    // lanes, and for committees of <= 16 keeps the whole instance in shared memory.  Measured cross-over (profiles/README.md,
-    // round 2): committees of <= 5 switch below ~4 K instances, larger ones always profit.  Recording / resumable handles
+    // lanes, and for committees of <= 16 keeps the whole instance in shared memory: committees of <= 5 switch below ~4 K
+    // instances, larger ones always profit (H100: 1 024 x 4 takes 2.5 ms wide against 9.2 ms on the thread kernel, 65 536 x 4
+    // 49.5 ms on the thread kernel against 68.4 ms wide).  Recording / resumable handles
     // stay on the thread kernel (the wide one has no save area).  LBFT_FORCE_KERNEL=wide|thread overrides (A/B runs).
     const bool modes = (c.flags & (LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE)) != 0;
     use_wide = !modes && !tds && (N >= 6 || c.num_instances <= 4096);
@@ -163,9 +164,9 @@ struct HostSetup {
     }
     // Sparse warp tiles of the thread kernel (kernels.cuh TILE: 8 or 16 instances per warp, the other lanes retire at once):
     // the instances of a warp serialise through each other's code paths, so as long as the batch does not fill the machine
-    // with full warps (2 048 warps of <= 128 registers = one wave on 148 SMs), fewer instances per warp finish sooner.
-    // Measured on BASELINE configs[4] (16 384 x 7, profiles/r2j_ab_tiles.txt, r2k): 8 per warp 59.3 ms, 16 per warp 72.8, full
-    // tiles 88.9, the wide kernel (8 lanes per instance) 76.2.  So for committees of 6..16 (calendar queue, plain
+    // with full warps (2 112 warps of <= 128 registers = one wave on 132 SMs), fewer instances per warp finish sooner.
+    // Measured on BASELINE configs[4] (16 384 x 7, H100): 8 per warp 42.0 ms, full tiles 77.7, the wide kernel (8 lanes per
+    // instance) 60.4.  So for committees of 6..16 (calendar queue, plain
     // single-epoch handles): about one wave of 8-instance warps -> tile 8, of 16-instance warps -> tile 16, more -> full
     // tiles; below that the wide kernel.  LBFT_THREAD_TILE=8|16 / LBFT_FORCE_KERNEL override (A/B runs); honoured further
     // down, once the queue mode is known.
@@ -181,9 +182,9 @@ struct HostSetup {
     }
     tile_stride = use_wide ? 1u : 32u;
     // lanes per instance: enough for the committee's fan-out, few enough that a warp carries several instances
-    // (measured, profiles/README.md r2e: 8 lanes per instance — four instances per warp — win once the batch fills the machine
-    // with warps, committees of 64 included: 8 192 x 64 takes 1.14 s against 1.63 s with a warp per instance; below ~4 K
-    // instances a whole warp per instance has the lower latency)
+    // (8 lanes per instance — four instances per warp — win once the batch fills the machine with warps, committees of 64
+    // included: on an H100 8 192 x 64 takes 0.86 s against 1.32 s with a warp per instance; below ~4 K instances a whole warp
+    // per instance has the lower latency)
     wide_group = c.num_instances > 4096 ? 8u : 32u;
     if (const char* g = std::getenv("LBFT_WIDE_GROUP")) {
       const int v = atoi(g);
@@ -246,7 +247,7 @@ struct HostSetup {
     }
     p.L = make_layout(N, rcap, qcap, pcap, c.partition_windows, qscan, (uint32_t)c.max_clock, p.record_rs != 0, p.resumable != 0, epochs, tds);
     // (calendar queue: the sparse-tile kernels keep the occupancy words of their instances in shared memory, sim_core.cuh KS —
-    // ((max_clock + 8) / 8) x tile words per warp, 14 warps per SM: horizons up to ~3 500 ms at 8 per warp, ~1 750 at 16)
+    // ((max_clock + 8) / 8) x tile words per warp: horizons up to ~3 500 ms at 8 per warp, ~1 750 at 16)
     const bool ks_fits = (uint64_t)(((uint32_t)c.max_clock + 8) / 8) * want_tile <= 3584;
     if (!use_wide && want_tile != 32 && ((qscan == 3 && ks_fits && (want_tile == 8 || N <= 16)) || (qscan == 2 && want_tile == 8)) && !modes && !tds && epochs == 1)
       tile_stride = want_tile;

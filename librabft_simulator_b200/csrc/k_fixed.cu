@@ -8,11 +8,9 @@ cudaError_t launch_fixed(const KernelSel& k, const Params& P, cudaStream_t strea
   const size_t dyn = (size_t)(T / 32) * 64 * (32 * 4 + 32 * 2);
   if (k.tile == 8) {  // sparse tiles: eight instances per warp (batches too small to fill the GPU with full warps)
     const uint32_t tiles = (P.num_instances + 7) / 8;
-    lbft_event_loop_kernel<16, 2, FX_DEFAULT4, false, false, false, false, 8><<<(tiles * 32 + T - 1) / T, T, dyn, stream>>>(P);
-    return cudaGetLastError();
+    return launch_thread<16, 2, FX_DEFAULT4, false, false, false, false, 8>((tiles * 32 + T - 1) / T, dyn, P, stream);
   }
   if (k.tile != 32) return cudaErrorInvalidValue;
-  lbft_event_loop_kernel<16, 2, FX_DEFAULT4><<<(P.num_instances + T - 1) / T, T, dyn, stream>>>(P);
-  return cudaGetLastError();
+  return launch_thread<16, 2, FX_DEFAULT4>((P.num_instances + T - 1) / T, dyn, P, stream);
 }
 }  // namespace lbft

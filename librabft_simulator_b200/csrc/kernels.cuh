@@ -16,27 +16,27 @@ namespace lbft {
 #ifndef LBFT_NO_KS
 #define LBFT_NO_KS 0  // A/B switch: 1 keeps the calendar's occupancy words in the instance's HBM block everywhere
 #endif
-// The wide kernels keep them in HBM: measured (profiles/r2n_ab_ks.txt) 8 192 x 64 on 8 lanes per instance 879 ms with the words in
-// shared memory against 858 ms without (1 024 x 64 on a warp per instance: 313 vs 317 ms) — the words are L1-resident there
-// anyway; the sparse-tile thread kernel gains 7.7 % (16 384 x 7: 42.4 vs 45.9 ms).
+// The wide kernels keep them in HBM: the words are L1-resident there anyway, and shared memory gains nothing; the sparse-tile
+// thread kernel keeps them in shared memory.
 #ifndef LBFT_WIDE_KS
 #define LBFT_WIDE_KS 0
 #endif
 LBFT_LAYOUT_FN uint32_t calendar_kmask_words(const Layout& L) { return (L.cal_times + 7) / 8; }
 constexpr uint32_t kThrSmem = 256;  // doubles: delay thresholds held in shared memory when they fit
 
-// Launch shapes of the thread-per-instance kernel.  QMODE 0/1/3: one-warp blocks, 14 resident per SM (2 048 tiles of a
-// 65 536-instance batch over 148 SMs; <= 144 registers/thread keeps every tile resident).  QMODE 2: two-warp blocks, 7 per
-// SM, so that the ziggurat/threshold tables (6 KB) are shared by two tiles and the per-tile event queues (queue_cap x 32 x
-// 6 B) fit in the 227 KB of shared memory.
+// Launch shapes of the thread-per-instance kernel: 16 warp tiles per SM, so that the 2 048 tiles of a 65 536-instance batch
+// are resident in one wave on the 132 SMs of an H100 (14 per SM would leave 200 tiles for a second wave).  16 warps are four
+// per SM sub-partition, i.e. <= 128 registers/thread — the bound ptxas already applies at 14.  QMODE 0/1/3: one-warp blocks.
+// QMODE 2: four-warp blocks, 4 per SM, so that the ziggurat/threshold tables (6 KB) are shared by four tiles and the per-tile
+// event queues (queue_cap x 32 x 6 B: 48 KB per block at queue_cap 64) fit in the 228 KB of shared memory of an SM.
 #ifndef LBFT_Q2_WARPS
-#define LBFT_Q2_WARPS 2   // warps per block of the shared-memory-queue kernels (they share the 6 KB of tables)
-#define LBFT_Q2_BLOCKS 7  // ... and blocks per SM: WARPS x BLOCKS = 14 tiles per SM, all 2 048 tiles of the bench batch resident
+#define LBFT_Q2_WARPS 4   // warps per block of the shared-memory-queue kernels (they share the 6 KB of tables)
+#define LBFT_Q2_BLOCKS 4  // ... and blocks per SM: WARPS x BLOCKS = 16 tiles per SM
 #endif
 template <int QMODE>
 struct LaunchShape {
   static constexpr int kThreads = QMODE == 2 ? 32 * LBFT_Q2_WARPS : 32;
-  static constexpr int kBlocksPerSm = QMODE == 2 ? LBFT_Q2_BLOCKS : 14;
+  static constexpr int kBlocksPerSm = QMODE == 2 ? LBFT_Q2_BLOCKS : 16;
 };
 
 // TILE: instances per warp tile.  32 fills every lane; 8 / 4 ("sparse" tiles: the other lanes of the warp retire at once) trade
@@ -48,8 +48,8 @@ template <int NMAX, int QMODE, int FX = FX_NONE, bool REC = false, bool RES = fa
 __global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMODE>::kBlocksPerSm) lbft_event_loop_kernel(const __grid_constant__ Params P) {
   static_assert(TILE == 32 || ((QMODE == 3 || QMODE == 2) && !REC && !RES && !EP && !TDS), "sparse tiles: plain kernels over the calendar / shared-memory queue");
   // The ziggurat layers are indexed by a random byte per lane: a per-block shared-memory copy (4 KB) serves the 32
-  // scattered 8-byte reads of a warp in ~1-2 wavefronts; reading them through L1 from global memory instead was
-  // measured 1.5x slower for the whole kernel (44.1 vs 28.9 ms).
+  // scattered 8-byte reads of a warp in ~1-2 wavefronts; reading them through L1 from global memory instead makes the
+  // whole kernel markedly slower.
   __shared__ double s_zx[257];
   __shared__ double s_zf[257];
   __shared__ double s_thr[kThrSmem];  // delay thresholds (same scattered access pattern), when they fit
@@ -95,9 +95,8 @@ __global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMOD
 // contiguous extent (TileMem<1>: stride 1), tables are read through L1 (every lane of a group reads the same element), the
 // shared-memory queue of QMODE 2 and the fan-out scratch are per group.
 // Warps per block: four when a warp carries several instances; ONE when a warp is an instance (G = 32): a block is then a
-// single instance, its index arithmetic folds away (5 192 instead of 5 600 SASS instructions) and blocks retire one by one —
-// measured (profiles/r2p_ab_wide_warps.txt) 1 024 x 4: 2.48 ms against 3.81 with four-warp blocks, a lone instance 3.66 against
-// 4.44 ms; 8 lanes per instance (8 192 x 64) is indifferent: 838 / 842 / 840 ms for 4 / 2 / 1 warps.
+// single instance, its index arithmetic folds away and blocks retire one by one, which shortens small batches; with 8 lanes
+// per instance the block size makes no difference.
 #ifndef LBFT_WIDE_WARPS
 #define LBFT_WIDE_WARPS 4  // (blocks of the G < 32 kernels)
 #endif
@@ -170,7 +169,35 @@ cudaError_t launch_calendar(const KernelSel& k, const Params& P, cudaStream_t st
 cudaError_t launch_heap(const KernelSel& k, const Params& P, cudaStream_t stream);
 cudaError_t launch_wide(const KernelSel& k, const Params& P, cudaStream_t stream);
 
+// Lets `kernel` take up to the device's opt-in limit of shared memory per block, beyond the 48 KB default (the QMODE 2
+// queues of four warps, the wide kernel's shared-memory instance state); `whole_carveout` also asks for the largest
+// shared-memory carveout (4 such QMODE 2 blocks per SM).  The attributes belong to the kernel's handle in each device's
+// context, so they are set before every launch on the current device (one process may drive several GPUs), and always to
+// the same values, so host threads launching concurrently cannot undo each other's setting.
+template <class Kernel>
+inline cudaError_t allow_optin_smem(Kernel kernel, bool whole_carveout) {
+  int dev = 0, optin = 0;
+  cudaFuncAttributes fa{};
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, kernel);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes);
+  if (e == cudaSuccess && whole_carveout)
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
+  return e;
+}
+
 // Shared by the launchers of the thread-per-instance kernel.
+template <int NMAX, int QMODE, int FX = FX_NONE, bool REC = false, bool RES = false, bool EP = false, bool TDS = false, int TILE = 32>
+inline cudaError_t launch_thread(uint32_t blocks, size_t dyn, const Params& P, cudaStream_t stream) {
+  auto kernel = lbft_event_loop_kernel<NMAX, QMODE, FX, REC, RES, EP, TDS, TILE>;
+  if (dyn > 0) {
+    cudaError_t e = allow_optin_smem(kernel, QMODE == 2);
+    if (e != cudaSuccess) return e;
+  }
+  kernel<<<blocks, LaunchShape<QMODE>::kThreads, dyn, stream>>>(P);
+  return cudaGetLastError();
+}
 template <int NMAX, int QM, int TILE, int FX = FX_NONE>
 inline cudaError_t launch_sparse_tiles(const Params& P, cudaStream_t stream) {
   constexpr int T = LaunchShape<QM>::kThreads;
@@ -178,8 +205,7 @@ inline cudaError_t launch_sparse_tiles(const Params& P, cudaStream_t stream) {
   const size_t dyn = QM == 2 ? (size_t)(T / 32) * P.L.queue_cap * (32 * 4 + 32 * 2)
                              : (size_t)(T / 32) * calendar_kmask_words(P.L) * TILE * sizeof(uint32_t);  // (QMODE 3: sim_core.cuh KS)
   if (dyn > 48 * 1024) return cudaErrorInvalidValue;  // (the host keeps sparse tiles to horizons whose occupancy words fit)
-  lbft_event_loop_kernel<NMAX, QM, FX, false, false, false, false, TILE><<<blocks, T, dyn, stream>>>(P);
-  return cudaGetLastError();
+  return launch_thread<NMAX, QM, FX, false, false, false, false, TILE>(blocks, dyn, P, stream);
 }
 template <int NMAX, int QM>
 inline cudaError_t launch_thread_variants(const KernelSel& k, const Params& P, cudaStream_t stream) {
@@ -188,15 +214,14 @@ inline cudaError_t launch_thread_variants(const KernelSel& k, const Params& P, c
   const size_t dyn = QM == 2 ? (size_t)(T / 32) * P.L.queue_cap * (32 * 4 + 32 * 2) : 0;
   if (k.tds) {
     if (k.rec || k.res || k.epochs) return cudaErrorInvalidValue;  // (refused at lbft_create)
-    lbft_event_loop_kernel<NMAX, QM, FX_NONE, false, false, false, true><<<blocks, T, dyn, stream>>>(P);
+    return launch_thread<NMAX, QM, FX_NONE, false, false, false, true>(blocks, dyn, P, stream);
   } else if (k.epochs) {
     if (k.rec || k.res) return cudaErrorInvalidValue;  // (refused at lbft_create)
-    lbft_event_loop_kernel<NMAX, QM, FX_NONE, false, false, true><<<blocks, T, dyn, stream>>>(P);
-  } else if (k.rec && k.res) lbft_event_loop_kernel<NMAX, QM, FX_NONE, true, true><<<blocks, T, dyn, stream>>>(P);
-  else if (k.res) lbft_event_loop_kernel<NMAX, QM, FX_NONE, false, true><<<blocks, T, dyn, stream>>>(P);
-  else if (k.rec) lbft_event_loop_kernel<NMAX, QM, FX_NONE, true><<<blocks, T, dyn, stream>>>(P);
-  else lbft_event_loop_kernel<NMAX, QM><<<blocks, T, dyn, stream>>>(P);
-  return cudaGetLastError();
+    return launch_thread<NMAX, QM, FX_NONE, false, false, true>(blocks, dyn, P, stream);
+  } else if (k.rec && k.res) return launch_thread<NMAX, QM, FX_NONE, true, true>(blocks, dyn, P, stream);
+  else if (k.res) return launch_thread<NMAX, QM, FX_NONE, false, true>(blocks, dyn, P, stream);
+  else if (k.rec) return launch_thread<NMAX, QM, FX_NONE, true>(blocks, dyn, P, stream);
+  return launch_thread<NMAX, QM>(blocks, dyn, P, stream);
 }
 
 template <int NMAX, int QM, bool SMEM, int G, bool EP, int FX = FX_NONE>
@@ -204,11 +229,9 @@ inline cudaError_t launch_wide_variant(const Params& P, cudaStream_t stream) {
   constexpr uint32_t kPerBlock = wide_warps(G) * 32 / G;
   const uint32_t blocks = (P.num_instances + kPerBlock - 1) / kPerBlock;
   const size_t dyn = (size_t)kPerBlock * wide_smem_words_per_group(P.L, QM, SMEM) * sizeof(uint32_t);
-  static size_t attr_set = 48 * 1024;  // (per instantiation; two threads racing set the same or a larger value)
-  if (dyn > attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(lbft_wide_kernel<NMAX, QM, SMEM, G, EP, FX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
+  if (dyn > 48 * 1024) {  // (the wide kernel has no static shared memory)
+    cudaError_t e = allow_optin_smem(lbft_wide_kernel<NMAX, QM, SMEM, G, EP, FX>, false);
     if (e != cudaSuccess) return e;
-    attr_set = dyn;
   }
   lbft_wide_kernel<NMAX, QM, SMEM, G, EP, FX><<<blocks, wide_warps(G) * 32, dyn, stream>>>(P);
   return cudaGetLastError();

@@ -1,4 +1,4 @@
-// lbft_api.cu — the C ABI of include/lbft.h over the sm_100a event-loop kernel.
+// lbft_api.cu — the C ABI of include/lbft.h over the sm_90a event-loop kernel.
 //
 // Replaces, for a whole batch of instances at once, the reference call sequence
 //   Simulator::new(seed, nodes, RandomDelay::new(mean, variance), context_factory)   simulator.rs:200-250

@@ -44,7 +44,7 @@
 #include <cmath>
 #endif
 
-// A/B switches of two exact optimisations (profiles/r2r_ab_exact.txt): see enqueue_network_event and st_u16.
+// A/B switches of two exact optimisations: see enqueue_network_event and st_u16.
 #ifndef LBFT_ELIDE_SILENT
 #define LBFT_ELIDE_SILENT 1
 #endif
@@ -318,8 +318,8 @@ LBFT_COLD PartitionSpan partition_span(Mem m, uint32_t part_base, uint32_t windo
 // the reference's own delay model (LogNormal served by the threshold table), so the other delay branches — and, where
 // the shape excludes them, silent nodes and partitions — are compiled out as well.
 // REC: keep DataWriter's round-switch table (LBFT_FLAG_ROUND_SWITCHES, Params::record_rs).  A template parameter rather
-// than a run-time test so that the non-recording instantiations carry no trace of it (the run-time test measured
-// +0.8..2.0 % on the generic kernels, profiles/README.md).
+// than a run-time test so that the non-recording instantiations carry no trace of it (a run-time test slows the
+// generic kernels).
 // RES: resumable run (LBFT_FLAG_RESUMABLE): the loop stops at P.stop_clock the way loop_until(max_clock) does
 // (simulator.rs:383-391: the first event beyond it is popped and dropped), the instance registers are saved to /
 // restored from the save area, and finalize() leaves the queue alone.
@@ -1158,8 +1158,8 @@ struct Core {
   // DataSyncNode::create_notification (data_sync.rs:82-111) into a payload slot
   // ------------------------------------------------------------------------------------------
   // hcbr snapshot words (N <= 4: two words per vector) fetched BEFORE the send loop so that their latency hides
-  // behind the delay sampling; measured -5.8 % kernel time.  (Prefetching the notification words before the node
-  // load, by contrast, measured +9.7 % and is not done.)
+  // behind the delay sampling.  (Prefetching the notification words before the node load, by contrast, is slower and
+  // is not done.)
   struct HcbrRegs {
     uint32_t tc[2], cur[2];
   };

@@ -205,7 +205,7 @@ struct Params {
   uint32_t delay_kmax;       // > 0: delay_thr[k] (k = 0..delay_kmax) is valid and replaces exp() on the device
   uint32_t pad1;
   // the voting rights travel in the parameter block itself (constant bank: no memory round trip when a vote or a
-  // timeout is tallied; measured -2.3 % kernel time.  Doing the same for leader/duration/period measured slower.)
+  // timeout is tallied.  Doing the same for leader/duration/period is slower.)
   uint32_t c_weights[64];
   // device pointers
   const uint64_t* seeds;      // [num_instances]

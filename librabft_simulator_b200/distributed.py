@@ -1,7 +1,7 @@
 """Instance-level data parallelism (SURVEY.md §8e): simulator instances are independent (own seed, own RNG,
 own nodes — simulator.rs:200-250), so the batch is sharded contiguously over ranks with NO data-path
 collective; one all-gather of the per-instance summaries ``{commit_count[N], state_key[N], rounds}`` happens at
-the end of a run.  One process per GPU, ``torch.distributed`` (NCCL over NVLink/NVSwitch on the B200 box, gloo in
+the end of a run.  One process per GPU, ``torch.distributed`` (NCCL over NVLink/NVSwitch between H100s, gloo in
 the CPU tests).
 
 ``ShardedBatchSimulator`` is the product's multi-GPU entry: it owns the sharding (``shard_bounds``), this rank's

@@ -9,7 +9,7 @@ Reference surface being mirrored (novifinancial/librabft_simulator):
 * ``SimulatedContext::committed_history()`` / ``last_committed_state()``            simulated_context.rs:98-100,194-196
 
 ``BatchSimulator`` is the batched form (one handle = many independent ``Simulator`` instances, one per seed,
-advanced in lockstep on one B200); ``Simulator`` is the single-instance spelling of the reference.  All the
+advanced in lockstep on one H100); ``Simulator`` is the single-instance spelling of the reference.  All the
 simulation work happens in the CUDA library; this module only marshals arguments and results.
 """
 import ctypes

@@ -3,7 +3,9 @@
  * device h % (number of devices); on a one-GPU box the eight handles share device 0.  Each handle runs two batches:
  * while batch 1 is in flight the results of batch 0 must stay readable and the seeds of batch 1 are staged with
  * lbft_set_seeds.  Everything is compared with synchronous lbft_run on a ninth handle, and the bulk commit-log
- * export (lbft_commit_logs) with lbft_commit_log.  Built and run by tests/test_gpu_cabi_c.py. */
+ * export (lbft_commit_logs) with lbft_commit_log.  Then one batch of BIG instances per device (at least two handles), which
+ * selects the thread-per-instance kernel with its shared-memory queues (a per-device opt-in beyond 48 KB of shared
+ * memory per block), run concurrently; every handle must agree with the first.  Built and run by tests/test_gpu_cabi_c.py. */
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -14,11 +16,13 @@
 #define I 96
 #define N 4
 #define CAP 64
+#define BIG 65536
+#define MAXB 16
 
-static void config(lbft_config* c, const uint64_t* seeds, int device) {
+static void config(lbft_config* c, const uint64_t* seeds, uint32_t count, int device) {
   memset(c, 0, sizeof *c);
   c->struct_size = sizeof *c;
-  c->num_instances = I;
+  c->num_instances = count;
   c->num_nodes = N;
   c->seeds = seeds;
   c->max_clock = 1000;
@@ -51,7 +55,7 @@ int main(void) {
       for (int i = 0; i < I; i++) seeds[h][b][i] = 1000u * (unsigned)h + 100000u * (unsigned)b + (unsigned)i + 7u;
   lbft_config c;
   for (int h = 0; h < H; h++) {
-    config(&c, seeds[h][0], h % ndev);
+    config(&c, seeds[h][0], I, h % ndev);
     CHECK(lbft_create(&c, &sim[h]));
   }
   /* batch 0 on every handle at once */
@@ -74,7 +78,7 @@ int main(void) {
   for (int h = 0; h < H; h++) CHECK(lbft_wait(sim[h]));
   for (int h = 0; h < H; h++) CHECK(lbft_last_states(sim[h], states[h][1]));
   /* the same batches, synchronously, on one more handle */
-  config(&c, seeds[0][0], 0);
+  config(&c, seeds[0][0], I, 0);
   CHECK(lbft_create(&c, &ref));
   int bad = 0;
   for (int h = 0; h < H; h++)
@@ -102,6 +106,25 @@ int main(void) {
   printf("%d handles x 2 batches on %d device(s) from one thread; %zu commit-log rows checked\n", H, ndev, total);
   for (int h = 0; h < H; h++) lbft_destroy(sim[h]);
   lbft_destroy(ref);
+  /* BIG instances per handle, one handle per device (two on a one-GPU box), launched together */
+  static uint64_t big_seeds[BIG], big_states[MAXB][BIG * N];
+  lbft_sim* big[MAXB];
+  const int nb = ndev < 2 ? 2 : (ndev > MAXB ? MAXB : ndev);
+  for (int i = 0; i < BIG; i++) big_seeds[i] = (uint64_t)i;
+  char kernel[128];
+  for (int b = 0; b < nb; b++) {
+    config(&c, big_seeds, BIG, b % ndev);
+    CHECK(lbft_create(&c, &big[b]));
+  }
+  CHECK(lbft_kernel_info(big[0], kernel, sizeof kernel));
+  for (int b = 0; b < nb; b++) CHECK(lbft_run_async(big[b]));
+  for (int b = 0; b < nb; b++) CHECK(lbft_wait(big[b]));
+  for (int b = 0; b < nb; b++) {
+    CHECK(lbft_last_states(big[b], big_states[b]));
+    if (memcmp(big_states[b], big_states[0], sizeof big_states[0])) { fprintf(stderr, "big handle %d differs from handle 0\n", b); bad = 1; }
+    lbft_destroy(big[b]);
+  }
+  printf("%d handles of %d instances (%s) on %d device(s)\n", nb, BIG, kernel, ndev);
   puts(bad ? "MISMATCH" : "async handles agree with synchronous runs");
   return bad;
 }

@@ -59,10 +59,12 @@ def test_c_caller_staged_run_snapshot_and_round_switches(tmp_path, oracle):
 @pytest.mark.gpu
 def test_c_caller_drives_eight_handles_from_one_thread(tmp_path):
     """lbft_run_async / lbft_wait: one thread, eight handles (spread over every visible GPU), double-buffered host staging;
-    lbft_commit_logs against lbft_commit_log."""
+    lbft_commit_logs against lbft_commit_log; then a 65 536-instance batch per GPU (at least two handles) on the
+    thread-per-instance kernel, whose shared-memory opt-in must hold on every device."""
     import torch
     exe = build_c_caller(tmp_path, "multi_handle")
     env = dict(os.environ, LBFT_TEST_DEVICES=str(torch.cuda.device_count()))
     p = subprocess.run([exe], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=300, env=env)
     assert p.returncode == 0, p.stdout
     assert "async handles agree with synchronous runs" in p.stdout
+    assert "instances (lbft_event_loop_kernel<16,2," in p.stdout

@@ -1,4 +1,4 @@
-"""GPU parity tests proper: the sm_100a kernel, called through the C ABI (ctypes -> liblbft_b200.so), against
+"""GPU parity tests proper: the sm_90a kernel, called through the C ABI (ctypes -> liblbft_b200.so), against
 the CPU oracle on the same seeded inputs; plus size-independent properties at BASELINE.json's full sizes.
 Bit-exact: commit counts, SipHash state keys of the full commit logs, the logs themselves, and the event /
 RNG counters."""
