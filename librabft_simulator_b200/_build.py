@@ -42,23 +42,23 @@ def nvcc_path():
     return shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 
 
-def build_product(force=False, verbose_ptxas=False, extra_flags=(), lib_path=None):
+def build_product(force=False, verbose_ptxas=False, lib_path=None):
     """nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo on every unit (objects in csrc/build/, in parallel), then one
     shared library.  Only units older than their sources are recompiled."""
     from concurrent.futures import ThreadPoolExecutor
     lib_path = lib_path or LIB_PATH
     headers = [os.path.join(CSRC, f) for f in PRODUCT_HEADERS] + [os.path.join(ROOT, "include", "lbft.h")]
     sources = headers + [os.path.join(CSRC, u) for u in PRODUCT_UNITS]
-    if not (force or verbose_ptxas or extra_flags) and _newer(lib_path, sources):
+    if not (force or verbose_ptxas) and _newer(lib_path, sources):
         return lib_path  # (the objects need not exist: on the GPU box only the library travels)
     objdir = os.path.join(CSRC, "build" if lib_path == LIB_PATH else "build_" + os.path.basename(lib_path))
     os.makedirs(objdir, exist_ok=True)
     jobs = []
     for unit in PRODUCT_UNITS:
         obj = os.path.join(objdir, unit.replace(".cu", ".o"))
-        if force or verbose_ptxas or extra_flags or not _newer(obj, headers + [os.path.join(CSRC, unit)]):
+        if force or verbose_ptxas or not _newer(obj, headers + [os.path.join(CSRC, unit)]):
             jobs.append((unit, obj))
-    flags = NVCC_FLAGS + list(extra_flags) + (["-Xptxas", "-v"] if verbose_ptxas else [])
+    flags = NVCC_FLAGS + (["-Xptxas", "-v"] if verbose_ptxas else [])
     with ThreadPoolExecutor(max_workers=min(len(PRODUCT_UNITS), os.cpu_count() or 2)) as pool:
         outs = list(pool.map(lambda j: _run([nvcc_path()] + flags + ["-c", "-o", j[1], j[0]], CSRC), jobs))
     if verbose_ptxas:
@@ -110,8 +110,6 @@ def build_oracle_native():
 
 
 def build_hostcore(force=False):
-    if os.environ.get("LBFT_HOSTCORE_PATH"):  # an alternatively built copy (A/B of compile-time switches)
-        return os.environ["LBFT_HOSTCORE_PATH"]
     srcs = [os.path.join(HOSTCORE_DIR, "hostcore.cpp")] + [
         os.path.join(CSRC, f) for f in ("sim_core.cuh", "sim_params.h", "host_setup.hpp")]
     if not force and _newer(HOSTCORE_PATH, srcs):

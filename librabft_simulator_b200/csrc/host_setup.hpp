@@ -72,6 +72,55 @@ inline uint32_t pow2_ceil(uint32_t v) {
   return p;
 }
 
+constexpr uint32_t kThrSmem = 256;  // doubles: delay thresholds held in shared memory when they fit
+
+// The kernel instantiation a handle launches (kernels.cuh), decided once by HostSetup::build.
+struct KernelSel {
+  bool wide;   // lbft_wide_kernel instead of lbft_event_loop_kernel
+  bool smem;   // wide kernel: instance state in shared memory
+  int group;   // wide kernel: lanes per instance (8 / 32)
+  bool epochs; // Layout::epochs > 1: the instantiation with the epoch machinery (plain kernels only)
+  bool tds;    // LBFT_FLAG_TRUE_DATA_SYNC (plain single-epoch thread kernels only)
+  int tile;    // instances per warp tile, the lane interleaving of the state (thread kernel: 32, or 8 / 16 = sparse tiles on
+               // plain calendar-queue kernels; wide kernel: 1)
+  int nmax;    // 16 / 32 / 64: width of the author masks
+  int qmode;   // Layout::queue_scan
+  int fixed;   // FX_* (sim_params.h): the instantiation with that compile-time layout; FX_NONE = generic
+  bool rec, res;
+};
+
+// The kernel's name, spelled like the symbol cuobjdump shows (lbft_kernel_info).
+inline std::string kernel_name(const KernelSel& k) {
+  char buf[96];
+  if (k.wide)
+    snprintf(buf, sizeof buf, "lbft_wide_kernel<%d,%d,%s,%d,%s,%d>", k.nmax, k.qmode, k.smem ? "true" : "false", k.group, k.epochs ? "true" : "false", k.fixed);
+  else
+    snprintf(buf, sizeof buf, "lbft_event_loop_kernel<%d,%d,%d,%s,%s,%s,%s,%d>", k.nmax, k.qmode, k.fixed, k.rec ? "true" : "false",
+             k.res ? "true" : "false", k.epochs ? "true" : "false", k.tds ? "true" : "false", k.tile);
+  return buf;
+}
+// Whether two selections name the same kernel (the fields kernel_name prints).
+constexpr bool same_kernel(const KernelSel& a, const KernelSel& b) {
+  return a.wide == b.wide && a.nmax == b.nmax && a.qmode == b.qmode && a.epochs == b.epochs && a.fixed == b.fixed &&
+         (a.wide ? a.smem == b.smem && a.group == b.group
+                 : a.rec == b.rec && a.res == b.res && a.tds == b.tds && a.tile == b.tile);
+}
+
+// The compile-time layout (sim_params.h fixed_layout) a configuration matches: its layout is bit-identical to the constant
+// (which also pins the queue mode and a single-epoch, non-data-sync handle), it neither records nor resumes, and the delay
+// model is the reference's (LogNormal served by the threshold table; FX_DEFAULT4 / FX_PART7 also need the table in shared
+// memory and no silent nodes).  The kernel family, tile and lane-group conditions are the product's: HostSetup::build.
+inline int fixed_shape_of(const Params& P) {
+  constexpr Layout kDefault4 = fixed_layout(FX_DEFAULT4), kPart7 = fixed_layout(FX_PART7), kCommittee64 = fixed_layout(FX_COMMITTEE64);
+  const bool table_delay = P.delay_kind == LBFT_DELAY_LOGNORMAL && !P.delay_const && P.delay_kmax != 0;
+  const bool plain_model = table_delay && P.delay_kmax + 2 <= kThrSmem && P.silent_mask == 0;
+  if (P.record_rs || P.resumable) return FX_NONE;
+  if (plain_model && memcmp(&P.L, &kDefault4, sizeof(Layout)) == 0) return FX_DEFAULT4;
+  if (plain_model && memcmp(&P.L, &kPart7, sizeof(Layout)) == 0) return FX_PART7;
+  if (table_delay && memcmp(&P.L, &kCommittee64, sizeof(Layout)) == 0) return FX_COMMITTEE64;
+  return FX_NONE;
+}
+
 struct HostSetup {
   Params params{};  // pointer members are left null; the runtime fills in device addresses
   std::vector<double> zig_x, zig_f;
@@ -80,10 +129,7 @@ struct HostSetup {
   std::vector<uint32_t> weights;
   std::vector<double> delay_thr;  // see build_delay_table()
   std::string error;
-  uint32_t tile_stride = 32;  // instances per state tile (lane interleaving); 1 for the warp-per-instance kernel
-  bool use_wide = false;      // launch lbft_wide_kernel (one warp per instance) instead of one thread per instance
-  bool wide_smem = false;     // ... with the instance state in shared memory (committees of <= 16, short horizons)
-  uint32_t wide_group = 32;   // ... lanes per instance: 8 / 16 / 32
+  KernelSel sel{};
 
   bool build(const lbft_config& c) {
     if (c.struct_size != sizeof(lbft_config)) return fail("lbft_config.struct_size does not match this library (ABI mismatch)");
@@ -155,41 +201,38 @@ struct HostSetup {
     // lanes, and for committees of <= 16 keeps the whole instance in shared memory: committees of <= 5 switch below ~4 K
     // instances, larger ones always profit (H100: 1 024 x 4 takes 2.5 ms wide against 9.2 ms on the thread kernel, 65 536 x 4
     // 49.5 ms on the thread kernel against 68.4 ms wide).  Recording / resumable handles
-    // stay on the thread kernel (the wide one has no save area).  LBFT_FORCE_KERNEL=wide|thread overrides (A/B runs).
+    // stay on the thread kernel (the wide one has no save area).
+    // LBFT_FORCE_KERNEL=wide|thread is a test seam, read here only: it runs one configuration through both families (and any
+    // value turns off the sparse tiles below).
     const bool modes = (c.flags & (LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE)) != 0;
-    use_wide = !modes && !tds && (N >= 6 || c.num_instances <= 4096);
-    if (const char* f = std::getenv("LBFT_FORCE_KERNEL")) {
-      if (!strcmp(f, "wide") && !modes && !tds) use_wide = true;
-      if (!strcmp(f, "thread")) use_wide = false;
-    }
+    const char* force = std::getenv("LBFT_FORCE_KERNEL");
+    bool wide = !modes && !tds && (N >= 6 || c.num_instances <= 4096);
+    if (force && !strcmp(force, "wide") && !modes && !tds) wide = true;
+    if (force && !strcmp(force, "thread")) wide = false;
     // Sparse warp tiles of the thread kernel (kernels.cuh TILE: 8 or 16 instances per warp, the other lanes retire at once):
     // the instances of a warp serialise through each other's code paths, so as long as the batch does not fill the machine
     // with full warps (2 112 warps of <= 128 registers = one wave on 132 SMs), fewer instances per warp finish sooner.
     // Measured on BASELINE configs[4] (16 384 x 7, H100): 8 per warp 42.0 ms, full tiles 77.7, the wide kernel (8 lanes per
     // instance) 60.4.  So for committees of 6..16 (calendar queue, plain
     // single-epoch handles): about one wave of 8-instance warps -> tile 8, of 16-instance warps -> tile 16, more -> full
-    // tiles; below that the wide kernel.  LBFT_THREAD_TILE=8|16 / LBFT_FORCE_KERNEL override (A/B runs); honoured further
-    // down, once the queue mode is known.
-    uint32_t want_tile = 32;
-    const bool env_family = std::getenv("LBFT_FORCE_KERNEL") != nullptr;
-    if (const char* f = std::getenv("LBFT_THREAD_TILE")) {
-      const int v = atoi(f);
-      if (v == 8 || v == 16) want_tile = (uint32_t)v;
-    } else if (!env_family && use_wide && N >= 6 && N <= 16 && c.max_clock <= 4095 && c.num_instances > 12288 &&
-               c.commands_per_epoch >= rcap && c.queue_cap <= 0xfff0u) {
-      use_wide = false;
-      want_tile = c.num_instances <= 24576 ? 8u : (c.num_instances <= 49152 ? 16u : 32u);
+    // tiles; below that the wide kernel.
+    uint32_t tile = 32;
+    if (!force && wide && N >= 6 && N <= 16 && c.max_clock <= 4095 && c.num_instances > 12288 && c.commands_per_epoch >= rcap &&
+        c.queue_cap <= 0xfff0u) {
+      wide = false;
+      tile = c.num_instances <= 24576 ? 8u : (c.num_instances <= 49152 ? 16u : 32u);
+      // (these handles get the calendar queue: the sparse-tile kernels keep the occupancy words of their instances in shared
+      // memory, sim_core.cuh KS — ((max_clock + 8) / 8) x tile words per warp: horizons up to ~3 500 ms at 8 per warp, ~1 750
+      // at 16)
+      if ((uint64_t)(((uint32_t)c.max_clock + 8) / 8) * tile > 3584) tile = 32;
     }
-    tile_stride = use_wide ? 1u : 32u;
+    sel.wide = wide;
+    sel.tile = wide ? 1 : (int)tile;
     // lanes per instance: enough for the committee's fan-out, few enough that a warp carries several instances
     // (8 lanes per instance — four instances per warp — win once the batch fills the machine with warps, committees of 64
     // included: on an H100 8 192 x 64 takes 0.86 s against 1.32 s with a warp per instance; below ~4 K instances a whole warp
     // per instance has the lower latency)
-    wide_group = c.num_instances > 4096 ? 8u : 32u;
-    if (const char* g = std::getenv("LBFT_WIDE_GROUP")) {
-      const int v = atoi(g);
-      if (v == 8 || v == 32) wide_group = (uint32_t)v;
-    }
+    sel.group = c.num_instances > 4096 ? 8 : 32;
     // (recording round switches queues the duplicate timers the normal path elides — measured high-water marks
     // roughly double, 46 -> 64+ at N = 4 — so the smallest committees get 128 entries and the HBM scan queue)
     // (resumable runs queue them too: the event dropped at a stop must be the one the reference drops)
@@ -214,7 +257,7 @@ struct HostSetup {
     if (qscan == 1 && events_per_ms * (double)c.max_clock > 2.0e6) qscan = 0;
     // The wide kernel scans its (single) shared-memory queue with all 32 lanes, so the same compact entries serve committees
     // up to 16 (4-bit sender/receiver) and queues up to 1 024 entries.
-    if (use_wide && N <= 16 && c.max_clock < (1 << 14) - 64 && pcap <= 255 && events_per_ms * (double)c.max_clock < 32768.0) {
+    if (wide && N <= 16 && c.max_clock < (1 << 14) - 64 && pcap <= 255 && events_per_ms * (double)c.max_clock < 32768.0) {
       const uint32_t want = c.queue_cap ? c.queue_cap : (N <= 4 ? 64u : 8 * N * N);
       if (want <= 1024) {
         qscan = 2;
@@ -237,27 +280,19 @@ struct HostSetup {
     uint32_t epochs = 1;
     if (c.commands_per_epoch < rcap) {
       if (tds) return fail("LBFT_FLAG_TRUE_DATA_SYNC needs commands_per_epoch >= round_cap (single-epoch runs)");
-      wide_group = 32;
-      epochs = (uint32_t)(rcap / c.commands_per_epoch) + 2;
+      sel.group = 32;
+      epochs =(uint32_t)(rcap / c.commands_per_epoch) + 2;
       if (epochs > MAX_EPOCHS) epochs = MAX_EPOCHS;
       while (epochs > 2 && (uint64_t)epochs * rcap > 32768) epochs--;
       if (qcap < (epochs * rcap + 1) / 2 && qscan) qcap = (epochs * rcap + 1) / 2;  // read-out scratch (see above)
       if (qcap < epochs * rcap && !qscan) qcap = pow2_ceil(epochs * rcap);
-      if (qscan == 2 && qcap > (use_wide ? 1024u : 64u)) qscan = N <= 5 ? 1u : (c.max_clock <= 4095 ? 3u : 0u);
+      if (qscan == 2 && qcap > (wide ? 1024u : 64u)) qscan = N <= 5 ? 1u : (c.max_clock <= 4095 ? 3u : 0u);
     }
     p.L = make_layout(N, rcap, qcap, pcap, c.partition_windows, qscan, (uint32_t)c.max_clock, p.record_rs != 0, p.resumable != 0, epochs, tds);
-    // (calendar queue: the sparse-tile kernels keep the occupancy words of their instances in shared memory, sim_core.cuh KS —
-    // ((max_clock + 8) / 8) x tile words per warp: horizons up to ~3 500 ms at 8 per warp, ~1 750 at 16)
-    const bool ks_fits = (uint64_t)(((uint32_t)c.max_clock + 8) / 8) * want_tile <= 3584;
-    if (!use_wide && want_tile != 32 && ((qscan == 3 && ks_fits && (want_tile == 8 || N <= 16)) || (qscan == 2 && want_tile == 8)) && !modes && !tds && epochs == 1)
-      tile_stride = want_tile;
     // wide kernel: the whole instance lives in shared memory when the instances of 16 resident warps (32 / group each) fit on
     // an SM
-    {
-      const size_t bytes = sizeof(uint32_t) * (size_t)p.L.total_words + 6u * (size_t)qcap + 1024u;
-      wide_smem = use_wide && qscan == 2 && epochs == 1 && bytes * (128u / wide_group) <= 56u * 1024u;
-      if (const char* f = std::getenv("LBFT_WIDE_SMEM")) wide_smem = wide_smem && atoi(f) != 0;
-    }
+    const size_t smem_bytes = sizeof(uint32_t) * (size_t)p.L.total_words + 6u * (size_t)qcap + 1024u;
+    sel.smem = wide && qscan == 2 && epochs == 1 && smem_bytes * (128u / sel.group) <= 56u * 1024u;
     // leader(round) for every representable round (+1: the pacemaker looks at active_round <= round_cap)
     leader.resize(rcap + 1);
     for (uint32_t r = 0; r <= rcap; r++) leader[r] = (uint8_t)pick_author(weights, total, siphash13_u64(r));
@@ -276,6 +311,17 @@ struct HostSetup {
     for (uint32_t i = 0; i < 64; i++) p.c_weights[i] = i < N ? weights[i] : 0;
     build_ziggurat();
     build_delay_table();
+    sel.qmode = (int)qscan;
+    sel.nmax = (qscan == 1 || qscan == 2) ? 16 : (N <= 16 ? 16 : (N <= 32 ? 32 : 64));
+    sel.epochs = epochs > 1;
+    sel.tds = tds;
+    sel.rec = p.record_rs != 0;
+    sel.res = p.resumable != 0;
+    // compile-time layouts: FX_DEFAULT4 on the thread kernel, FX_PART7 on its 8-instance warp tiles, FX_COMMITTEE64 on the wide
+    // kernel with 8 lanes per instance
+    const int fx = fixed_shape_of(p);
+    sel.fixed = (fx == FX_DEFAULT4 && !wide) || (fx == FX_PART7 && !wide && tile == 8) || (fx == FX_COMMITTEE64 && wide && sel.group == 8)
+                    ? fx : FX_NONE;
     return true;
   }
 

@@ -2,20 +2,9 @@
 #include "kernels.cuh"
 namespace lbft {
 cudaError_t launch_calendar(const KernelSel& k, const Params& P, cudaStream_t stream) {
-  if (k.wide || k.qmode != 3) return cudaErrorInvalidValue;
-  if (k.fixed == FX_PART7) {  // (lbft_api.cu select_kernel: the seven-author partition shape on 8-instance warp tiles)
-    if (k.tile != 8 || k.nmax != 16 || k.rec || k.res || k.epochs || k.tds) return cudaErrorInvalidValue;
-    return launch_sparse_tiles<16, 3, 8, FX_PART7>(P, stream);
-  }
-  if (k.fixed) return cudaErrorInvalidValue;
-  if (k.tile != 32) {  // sparse tiles (plain kernels; the host only asks for them there)
-    if (k.rec || k.res || k.epochs || k.tds) return cudaErrorInvalidValue;
-    if (k.tile == 8) return k.nmax == 16 ? launch_sparse_tiles<16, 3, 8>(P, stream) : (k.nmax == 32 ? launch_sparse_tiles<32, 3, 8>(P, stream) : launch_sparse_tiles<64, 3, 8>(P, stream));
-    if (k.tile == 16) return k.nmax == 16 ? launch_sparse_tiles<16, 3, 16>(P, stream) : cudaErrorInvalidValue;
-    return cudaErrorInvalidValue;
-  }
-  if (k.nmax == 16) return launch_thread_variants<16, 3>(k, P, stream);
-  if (k.nmax == 32) return launch_thread_variants<32, 3>(k, P, stream);
-  return launch_thread_variants<64, 3>(k, P, stream);
+  // sparse tiles: plain kernels for committees of 6..16, among them the seven-author partition shape (BASELINE configs[4])
+  using SparseTiles = Kernels<ThreadKernel<16, 3, FX_PART7, false, false, false, false, 8>, ThreadKernel<16, 3, FX_NONE, false, false, false, false, 8>,
+                              ThreadKernel<16, 3, FX_NONE, false, false, false, false, 16>>;
+  return launch_listed<Kernels<SparseTiles, ThreadVariants<16, 3>, ThreadVariants<32, 3>, ThreadVariants<64, 3>>>(k, P, stream);
 }
 }  // namespace lbft

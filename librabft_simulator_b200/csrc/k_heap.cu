@@ -2,9 +2,6 @@
 #include "kernels.cuh"
 namespace lbft {
 cudaError_t launch_heap(const KernelSel& k, const Params& P, cudaStream_t stream) {
-  if (k.wide || k.fixed || k.qmode != 0 || k.tile != 32) return cudaErrorInvalidValue;
-  if (k.nmax == 16) return launch_thread_variants<16, 0>(k, P, stream);
-  if (k.nmax == 32) return launch_thread_variants<32, 0>(k, P, stream);
-  return launch_thread_variants<64, 0>(k, P, stream);
+  return launch_listed<Kernels<ThreadVariants<16, 0>, ThreadVariants<32, 0>, ThreadVariants<64, 0>>>(k, P, stream);
 }
 }  // namespace lbft

@@ -3,11 +3,6 @@
 #include "kernels.cuh"
 namespace lbft {
 cudaError_t launch_scan(const KernelSel& k, const Params& P, cudaStream_t stream) {
-  if (k.wide || k.fixed) return cudaErrorInvalidValue;
-  if (k.qmode == 2 && k.tile == 8 && !k.rec && !k.res && !k.epochs && !k.tds) return launch_sparse_tiles<16, 2, 8>(P, stream);
-  if (k.tile != 32) return cudaErrorInvalidValue;
-  if (k.qmode == 2) return launch_thread_variants<16, 2>(k, P, stream);
-  if (k.qmode == 1) return launch_thread_variants<16, 1>(k, P, stream);
-  return cudaErrorInvalidValue;
+  return launch_listed<Kernels<ThreadVariants<16, 2>, ThreadVariants<16, 1>>>(k, P, stream);
 }
 }  // namespace lbft

@@ -2,18 +2,10 @@
 #include "kernels.cuh"
 namespace lbft {
 cudaError_t launch_wide(const KernelSel& k, const Params& P, cudaStream_t stream) {
-  if (!k.wide || (k.fixed != FX_NONE && k.fixed != FX_COMMITTEE64) || k.rec || k.res) return cudaErrorInvalidValue;
-  switch (k.qmode) {
-    case 2: return k.smem ? launch_wide_groups<16, 2, true>(k, P, stream) : launch_wide_groups<16, 2, false>(k, P, stream);
-    case 1: return launch_wide_groups<16, 1, false>(k, P, stream);
-    case 3:
-      if (k.nmax == 16) return launch_wide_groups<16, 3, false>(k, P, stream);
-      if (k.nmax == 32) return launch_wide_groups<32, 3, false>(k, P, stream);
-      return launch_wide_groups<64, 3, false>(k, P, stream);
-    default:
-      if (k.nmax == 16) return launch_wide_groups<16, 0, false>(k, P, stream);
-      if (k.nmax == 32) return launch_wide_groups<32, 0, false>(k, P, stream);
-      return launch_wide_groups<64, 0, false>(k, P, stream);
-  }
+  // QMODE 2 also with the instance state in shared memory; 64 authors on the calendar queue also with the compile-time
+  // layout of BASELINE configs[3]
+  using Special = Kernels<WideKernel<16, 2, true, 8>, WideKernel<16, 2, true, 32>, WideKernel<64, 3, false, 8, false, FX_COMMITTEE64>>;
+  return launch_listed<Kernels<Special, WideVariants<16, 2>, WideVariants<16, 1>, WideVariants<16, 3>, WideVariants<32, 3>,
+                               WideVariants<64, 3>, WideVariants<16, 0>, WideVariants<32, 0>, WideVariants<64, 0>>>(k, P, stream);
 }
 }  // namespace lbft

@@ -9,34 +9,24 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "host_setup.hpp"
 #include "sim_core.cuh"
 
 namespace lbft {
 
-#ifndef LBFT_NO_KS
-#define LBFT_NO_KS 0  // A/B switch: 1 keeps the calendar's occupancy words in the instance's HBM block everywhere
-#endif
-// The wide kernels keep them in HBM: the words are L1-resident there anyway, and shared memory gains nothing; the sparse-tile
-// thread kernel keeps them in shared memory.
-#ifndef LBFT_WIDE_KS
-#define LBFT_WIDE_KS 0
-#endif
+// The sparse-tile thread kernels keep the calendar's occupancy words in shared memory (sim_core.cuh KS); the wide kernels keep
+// them in HBM: the words are L1-resident there anyway, and shared memory gains nothing.
 LBFT_LAYOUT_FN uint32_t calendar_kmask_words(const Layout& L) { return (L.cal_times + 7) / 8; }
-constexpr uint32_t kThrSmem = 256;  // doubles: delay thresholds held in shared memory when they fit
 
 // Launch shapes of the thread-per-instance kernel: 16 warp tiles per SM, so that the 2 048 tiles of a 65 536-instance batch
 // are resident in one wave on the 132 SMs of an H100 (14 per SM would leave 200 tiles for a second wave).  16 warps are four
 // per SM sub-partition, i.e. <= 128 registers/thread — the bound ptxas already applies at 14.  QMODE 0/1/3: one-warp blocks.
 // QMODE 2: four-warp blocks, 4 per SM, so that the ziggurat/threshold tables (6 KB) are shared by four tiles and the per-tile
 // event queues (queue_cap x 32 x 6 B: 48 KB per block at queue_cap 64) fit in the 228 KB of shared memory of an SM.
-#ifndef LBFT_Q2_WARPS
-#define LBFT_Q2_WARPS 4   // warps per block of the shared-memory-queue kernels (they share the 6 KB of tables)
-#define LBFT_Q2_BLOCKS 4  // ... and blocks per SM: WARPS x BLOCKS = 16 tiles per SM
-#endif
 template <int QMODE>
 struct LaunchShape {
-  static constexpr int kThreads = QMODE == 2 ? 32 * LBFT_Q2_WARPS : 32;
-  static constexpr int kBlocksPerSm = QMODE == 2 ? LBFT_Q2_BLOCKS : 16;
+  static constexpr int kThreads = QMODE == 2 ? 32 * 4 : 32;  // QMODE 2: four warps per block share the 6 KB of tables
+  static constexpr int kBlocksPerSm = QMODE == 2 ? 4 : 16;   // ... and four blocks per SM: 16 tiles per SM
 };
 
 // TILE: instances per warp tile.  32 fills every lane; 8 / 4 ("sparse" tiles: the other lanes of the warp retire at once) trade
@@ -79,7 +69,7 @@ __global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMOD
   }
   // sparse tiles over the calendar queue: the kind-occupancy words of the tile's instances in shared memory, a column per
   // lane (sim_core.cuh KS; the host only selects sparse tiles when 14 warps' worth fits, host_setup.hpp)
-  constexpr bool KS = QMODE == 3 && TILE < 32 && !LBFT_NO_KS;
+  constexpr bool KS = QMODE == 3 && TILE < 32;
   Core<TileMem<TILE>, NMAX, QMODE, FX, REC, RES, 1, EP, TDS, KS> core(P, mem, s_zx, s_zf, thr_fits ? s_thr : P.delay_thr, sk, sd);
   if (KS) core.km = s_queue + (size_t)(threadIdx.x >> 5) * calendar_kmask_words(FX ? fixed_layout(FX) : P.L) * TILE + lane;
   if (RES && (P.run_flags & 1u)) core.restore_regs();  // a later lbft_run_until: continue where the last launch stopped
@@ -97,10 +87,7 @@ __global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMOD
 // Warps per block: four when a warp carries several instances; ONE when a warp is an instance (G = 32): a block is then a
 // single instance, its index arithmetic folds away and blocks retire one by one, which shortens small batches; with 8 lanes
 // per instance the block size makes no difference.
-#ifndef LBFT_WIDE_WARPS
-#define LBFT_WIDE_WARPS 4  // (blocks of the G < 32 kernels)
-#endif
-LBFT_LAYOUT_FN int wide_warps(int g) { return g == 32 ? 1 : LBFT_WIDE_WARPS; }
+LBFT_LAYOUT_FN int wide_warps(int g) { return g == 32 ? 1 : 4; }
 // blocks per SM the register allocation is bounded for: 16 warps per SM, <= 128 registers
 LBFT_LAYOUT_FN int wide_blocks_per_sm(int g) { return 16 / wide_warps(g); }
 
@@ -110,8 +97,7 @@ LBFT_LAYOUT_FN uint32_t wide_queue_words(uint32_t queue_cap, int qmode) {
   return qmode == 2 ? ((queue_cap + (queue_cap + 1) / 2 + 1) & ~1u) : 0u;  // even: what follows holds 64-bit entries
 }
 LBFT_LAYOUT_FN uint32_t wide_smem_words_per_group(const Layout& L, int qmode, bool smem_state) {
-  return wide_scratch_words() + wide_queue_words(L.queue_cap, qmode) + (smem_state ? ((L.total_words + 1) & ~1u) : 0u) +
-         (qmode == 3 && LBFT_WIDE_KS ? ((calendar_kmask_words(L) + 1) & ~1u) : 0u);  // QMODE 3: the calendar's occupancy words (sim_core.cuh KS)
+  return wide_scratch_words() + wide_queue_words(L.queue_cap, qmode) + (smem_state ? ((L.total_words + 1) & ~1u) : 0u);
 }
 
 // SMEM: the instance's state words live in shared memory for the whole run; only the chain table (and the epoch table) is
@@ -131,9 +117,7 @@ __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbf
   uint32_t* gstate = P.state + (size_t)inst * KL.total_words;
   uint32_t* state = SMEM ? sk + wide_queue_words(KL.queue_cap, QMODE) : gstate;
   TileMem<1> mem{state, 0};
-  constexpr bool KS = QMODE == 3 && LBFT_WIDE_KS;
-  Core<TileMem<1>, NMAX, QMODE, FX, false, false, G, EP, false, KS> core(P, mem, P.zig_x, P.zig_f, P.delay_thr, sk, sd);
-  if (KS) core.km = base + wide_scratch_words();  // (QMODE 3 has no shared-memory queue and no shared-memory state: the words follow the scratch)
+  Core<TileMem<1>, NMAX, QMODE, FX, false, false, G, EP> core(P, mem, P.zig_x, P.zig_f, P.delay_thr, sk, sd);
   core.wl = wl;
   core.gm = G == 32 ? 0xffffffffu : (((1u << (G & 31)) - 1u) << ((threadIdx.x & 31u) & ~(uint32_t)(G - 1)));
   core.ws = ws;
@@ -148,21 +132,8 @@ __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbf
   }
 }
 
-// What the host decided to launch for a handle (host_setup.hpp / lbft_api.cu select_kernel).
-struct KernelSel {
-  bool wide;   // lbft_wide_kernel instead of lbft_event_loop_kernel
-  bool smem;   // wide kernel: instance state in shared memory
-  int group;   // wide kernel: lanes per instance (8 / 32)
-  bool epochs; // Layout::epochs > 1: the instantiation with the epoch machinery (plain kernels only)
-  bool tds;    // LBFT_FLAG_TRUE_DATA_SYNC (plain single-epoch thread kernels only)
-  int tile;    // thread kernel: instances per warp tile (32; 8 / 4 = sparse tiles, plain calendar-queue kernels)
-  int nmax;    // 16 / 32 / 64: width of the author masks
-  int qmode;   // Layout::queue_scan
-  int fixed;   // FX_* (sim_params.h): the instantiation with that compile-time layout; FX_NONE = generic
-  bool rec, res;
-};
-
-// One per translation unit; each returns cudaErrorInvalidValue if the selection is not one of its instantiations.
+// One per translation unit: launches the instantiation the selection names, or returns cudaErrorInvalidValue if the unit
+// has none (lbft_api.cu reports that with the kernel's name).
 cudaError_t launch_fixed(const KernelSel& k, const Params& P, cudaStream_t stream);
 cudaError_t launch_scan(const KernelSel& k, const Params& P, cudaStream_t stream);
 cudaError_t launch_calendar(const KernelSel& k, const Params& P, cudaStream_t stream);
@@ -187,68 +158,66 @@ inline cudaError_t allow_optin_smem(Kernel kernel, bool whole_carveout) {
   return e;
 }
 
-// Shared by the launchers of the thread-per-instance kernel.
-template <int NMAX, int QMODE, int FX = FX_NONE, bool REC = false, bool RES = false, bool EP = false, bool TDS = false, int TILE = 32>
-inline cudaError_t launch_thread(uint32_t blocks, size_t dyn, const Params& P, cudaStream_t stream) {
-  auto kernel = lbft_event_loop_kernel<NMAX, QMODE, FX, REC, RES, EP, TDS, TILE>;
-  if (dyn > 0) {
-    cudaError_t e = allow_optin_smem(kernel, QMODE == 2);
-    if (e != cudaSuccess) return e;
+// One instantiation of a kernel template: the selection that names it, and its launch.  try_launch launches it if `k` names
+// it and reports whether it did.
+template <int NMAX, int QM, int FX = FX_NONE, bool REC = false, bool RES = false, bool EP = false, bool TDS = false, int TILE = 32>
+struct ThreadKernel {
+  static constexpr KernelSel sel{/*wide*/ false, /*smem*/ false, /*group*/ 0, EP, TDS, TILE, NMAX, QM, FX, REC, RES};
+  static bool try_launch(const KernelSel& k, const Params& P, cudaStream_t stream, cudaError_t& e) {
+    if (!same_kernel(k, sel)) return false;
+    constexpr int T = LaunchShape<QM>::kThreads;
+    const uint32_t tiles = (P.num_instances + TILE - 1) / TILE, blocks = (tiles * 32 + T - 1) / T;
+    // QMODE 2: per warp the queue keys and payload halves; sparse tiles over the calendar queue: per warp the occupancy
+    // words of its instances (sim_core.cuh KS)
+    const size_t dyn = QM == 2 ? (size_t)(T / 32) * P.L.queue_cap * (32 * 4 + 32 * 2)
+                               : (QM == 3 && TILE < 32 ? (size_t)calendar_kmask_words(P.L) * TILE * sizeof(uint32_t) : 0);
+    auto kernel = lbft_event_loop_kernel<NMAX, QM, FX, REC, RES, EP, TDS, TILE>;
+    e = dyn > 0 ? allow_optin_smem(kernel, QM == 2) : cudaSuccess;
+    if (e == cudaSuccess) {
+      kernel<<<blocks, T, dyn, stream>>>(P);
+      e = cudaGetLastError();
+    }
+    return true;
   }
-  kernel<<<blocks, LaunchShape<QMODE>::kThreads, dyn, stream>>>(P);
-  return cudaGetLastError();
-}
-template <int NMAX, int QM, int TILE, int FX = FX_NONE>
-inline cudaError_t launch_sparse_tiles(const Params& P, cudaStream_t stream) {
-  constexpr int T = LaunchShape<QM>::kThreads;
-  const uint32_t tiles = (P.num_instances + TILE - 1) / TILE, blocks = (tiles * 32 + T - 1) / T;
-  const size_t dyn = QM == 2 ? (size_t)(T / 32) * P.L.queue_cap * (32 * 4 + 32 * 2)
-                             : (size_t)(T / 32) * calendar_kmask_words(P.L) * TILE * sizeof(uint32_t);  // (QMODE 3: sim_core.cuh KS)
-  if (dyn > 48 * 1024) return cudaErrorInvalidValue;  // (the host keeps sparse tiles to horizons whose occupancy words fit)
-  return launch_thread<NMAX, QM, FX, false, false, false, false, TILE>(blocks, dyn, P, stream);
-}
-template <int NMAX, int QM>
-inline cudaError_t launch_thread_variants(const KernelSel& k, const Params& P, cudaStream_t stream) {
-  constexpr int T = LaunchShape<QM>::kThreads;
-  const uint32_t blocks = (P.num_instances + T - 1) / T;
-  const size_t dyn = QM == 2 ? (size_t)(T / 32) * P.L.queue_cap * (32 * 4 + 32 * 2) : 0;
-  if (k.tds) {
-    if (k.rec || k.res || k.epochs) return cudaErrorInvalidValue;  // (refused at lbft_create)
-    return launch_thread<NMAX, QM, FX_NONE, false, false, false, true>(blocks, dyn, P, stream);
-  } else if (k.epochs) {
-    if (k.rec || k.res) return cudaErrorInvalidValue;  // (refused at lbft_create)
-    return launch_thread<NMAX, QM, FX_NONE, false, false, true>(blocks, dyn, P, stream);
-  } else if (k.rec && k.res) return launch_thread<NMAX, QM, FX_NONE, true, true>(blocks, dyn, P, stream);
-  else if (k.res) return launch_thread<NMAX, QM, FX_NONE, false, true>(blocks, dyn, P, stream);
-  else if (k.rec) return launch_thread<NMAX, QM, FX_NONE, true>(blocks, dyn, P, stream);
-  return launch_thread<NMAX, QM>(blocks, dyn, P, stream);
+};
+template <int NMAX, int QM, bool SMEM, int G, bool EP = false, int FX = FX_NONE>
+struct WideKernel {
+  static constexpr KernelSel sel{/*wide*/ true, SMEM, G, EP, /*tds*/ false, /*tile*/ 1, NMAX, QM, FX, /*rec*/ false, /*res*/ false};
+  static bool try_launch(const KernelSel& k, const Params& P, cudaStream_t stream, cudaError_t& e) {
+    if (!same_kernel(k, sel)) return false;
+    constexpr uint32_t kPerBlock = wide_warps(G) * 32 / G;
+    const uint32_t blocks = (P.num_instances + kPerBlock - 1) / kPerBlock;
+    const size_t dyn = (size_t)kPerBlock * wide_smem_words_per_group(P.L, QM, SMEM) * sizeof(uint32_t);
+    auto kernel = lbft_wide_kernel<NMAX, QM, SMEM, G, EP, FX>;
+    e = dyn > 48 * 1024 ? allow_optin_smem(kernel, false) : cudaSuccess;  // (the wide kernel has no static shared memory)
+    if (e == cudaSuccess) {
+      kernel<<<blocks, wide_warps(G) * 32, dyn, stream>>>(P);
+      e = cudaGetLastError();
+    }
+    return true;
+  }
+};
+// A list of instantiations (or of lists).
+template <class... Ks>
+struct Kernels {
+  static bool try_launch(const KernelSel& k, const Params& P, cudaStream_t stream, cudaError_t& e) {
+    return (Ks::try_launch(k, P, stream, e) || ...);
+  }
+};
+template <class List>
+inline cudaError_t launch_listed(const KernelSel& k, const Params& P, cudaStream_t stream) {
+  cudaError_t e = cudaErrorInvalidValue;
+  List::try_launch(k, P, stream, e);
+  return e;
 }
 
-template <int NMAX, int QM, bool SMEM, int G, bool EP, int FX = FX_NONE>
-inline cudaError_t launch_wide_variant(const Params& P, cudaStream_t stream) {
-  constexpr uint32_t kPerBlock = wide_warps(G) * 32 / G;
-  const uint32_t blocks = (P.num_instances + kPerBlock - 1) / kPerBlock;
-  const size_t dyn = (size_t)kPerBlock * wide_smem_words_per_group(P.L, QM, SMEM) * sizeof(uint32_t);
-  if (dyn > 48 * 1024) {  // (the wide kernel has no static shared memory)
-    cudaError_t e = allow_optin_smem(lbft_wide_kernel<NMAX, QM, SMEM, G, EP, FX>, false);
-    if (e != cudaSuccess) return e;
-  }
-  lbft_wide_kernel<NMAX, QM, SMEM, G, EP, FX><<<blocks, wide_warps(G) * 32, dyn, stream>>>(P);
-  return cudaGetLastError();
-}
-// the lanes-per-instance / epoch dimensions of an instantiation family (the host only selects these combinations)
-template <int NMAX, int QM, bool SMEM>
-inline cudaError_t launch_wide_groups(const KernelSel& k, const Params& P, cudaStream_t stream) {
-  if (k.epochs) {
-    if (SMEM || k.group != 32) return cudaErrorInvalidValue;
-    return launch_wide_variant<NMAX, QM, false, 32, true>(P, stream);
-  }
-  if (k.fixed == FX_COMMITTEE64) {  // (lbft_api.cu select_kernel: 64 authors, calendar queue, 8 lanes per instance, state in HBM)
-    if (NMAX != 64 || QM != 3 || SMEM || k.group != 8) return cudaErrorInvalidValue;
-    return launch_wide_variant<64, 3, false, 8, false, (NMAX == 64 && QM == 3 && !SMEM) ? FX_COMMITTEE64 : FX_NONE>(P, stream);
-  }
-  if (k.group == 8) return launch_wide_variant<NMAX, QM, SMEM, 8, false>(P, stream);
-  return launch_wide_variant<NMAX, QM, SMEM, 32, false>(P, stream);
-}
+// The recording / resumable / epoch / true-data-sync variants of a generic thread kernel.
+template <int NMAX, int QM>
+using ThreadVariants = Kernels<ThreadKernel<NMAX, QM>, ThreadKernel<NMAX, QM, FX_NONE, true>, ThreadKernel<NMAX, QM, FX_NONE, false, true>,
+                               ThreadKernel<NMAX, QM, FX_NONE, true, true>, ThreadKernel<NMAX, QM, FX_NONE, false, false, true>,
+                               ThreadKernel<NMAX, QM, FX_NONE, false, false, false, true>>;
+// The lane groups and the epoch variant of a generic wide kernel with its state in HBM.
+template <int NMAX, int QM>
+using WideVariants = Kernels<WideKernel<NMAX, QM, false, 8>, WideKernel<NMAX, QM, false, 32>, WideKernel<NMAX, QM, false, 32, true>>;
 
 }  // namespace lbft

@@ -228,7 +228,7 @@ int lbft_create(const lbft_config* config, lbft_sim** out_sim) {
   s->I = config->num_instances;
   s->N = config->num_nodes;
   s->device = config->device;
-  s->stride = s->hs.tile_stride;
+  s->stride = (uint32_t)s->hs.sel.tile;
   s->seeds_host.assign(config->seeds, config->seeds + s->I);
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -418,58 +418,18 @@ int lbft_run_until(lbft_sim* s, int64_t stop_clock) {
 
 }  // extern "C"
 
-// Which instantiation this handle launches (host_setup.hpp decided wide vs thread-per-instance and the queue mode).
-static KernelSel select_kernel(const lbft_sim* s) {
-  KernelSel k{};
-  k.wide = s->hs.use_wide;
-  k.smem = s->hs.wide_smem;
-  k.group = (int)s->hs.wide_group;
-  k.epochs = s->P.L.epochs > 1;
-  k.tds = s->P.L.tds != 0;
-  k.tile = (int)s->stride;
-  k.qmode = (int)s->P.L.queue_scan;
-  k.nmax = (k.qmode == 1 || k.qmode == 2) ? 16 : (s->N <= 16 ? 16 : (s->N <= 32 ? 32 : 64));
-  k.rec = s->P.record_rs != 0;
-  k.res = s->P.resumable != 0;
-  // shapes with a kernel instantiation with compile-time field offsets (sim_params.h fixed_layout): the handle's layout must
-  // be bit-identical and the delay model the reference's (LogNormal served by the threshold table)
-  constexpr Layout kDefault4 = fixed_layout(FX_DEFAULT4), kPart7 = fixed_layout(FX_PART7), kCommittee64 = fixed_layout(FX_COMMITTEE64);
-  const bool table_delay = s->P.delay_kind == LBFT_DELAY_LOGNORMAL && !s->P.delay_const && s->P.delay_kmax != 0;
-  const bool plain_model = table_delay && s->P.delay_kmax + 2 <= kThrSmem && s->P.silent_mask == 0;
-  const bool plain_handle = !k.rec && !k.res && !k.tds && !k.epochs;
-  k.fixed = FX_NONE;
-  if (!k.wide && k.qmode == 2 && plain_model && plain_handle && memcmp(&s->P.L, &kDefault4, sizeof(Layout)) == 0) k.fixed = FX_DEFAULT4;
-  else if (!k.wide && k.qmode == 3 && k.tile == 8 && plain_model && plain_handle && memcmp(&s->P.L, &kPart7, sizeof(Layout)) == 0) k.fixed = FX_PART7;
-  else if (k.wide && k.qmode == 3 && k.group == 8 && !k.smem && table_delay && plain_handle && memcmp(&s->P.L, &kCommittee64, sizeof(Layout)) == 0)
-    k.fixed = FX_COMMITTEE64;
-  if (const char* f = std::getenv("LBFT_NO_FIXED_SHAPES"))  // A/B runs: the generic instantiations for the shapes other than the default one
-    if (atoi(f) != 0 && k.fixed != FX_DEFAULT4) k.fixed = FX_NONE;
-  return k;
-}
-// ... spelled like the symbol ncu / cuobjdump show.
-static std::string kernel_name(const lbft_sim* s) {
-  const KernelSel k = select_kernel(s);
-  char buf[96];
-  if (k.wide)
-    snprintf(buf, sizeof buf, "lbft_wide_kernel<%d,%d,%s,%d,%s,%d>", k.nmax, k.qmode, k.smem ? "true" : "false", k.group, k.epochs ? "true" : "false", k.fixed);
-  else
-    snprintf(buf, sizeof buf, "lbft_event_loop_kernel<%d,%d,%d,%s,%s,%s,%s,%d>", k.nmax, k.qmode, k.fixed, k.rec ? "true" : "false",
-             k.res ? "true" : "false", k.epochs ? "true" : "false", k.tds ? "true" : "false", k.tile);
-  return buf;
-}
-
 static int enqueue_kernel(lbft_sim* s) {
   s->P.stop_clock = (int32_t)(s->P.resumable ? s->next_stop : (int64_t)s->P.max_clock);
   s->P.run_flags = (s->P.resumable && s->started) ? 1u : 0u;
   CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
   CUDA_TRY(cudaEventRecord(s->ev[2], s->stream));
-  const KernelSel k = select_kernel(s);
+  const KernelSel& k = s->hs.sel;
   cudaError_t e = k.wide ? launch_wide(k, s->P, s->stream)
                   : k.fixed == FX_DEFAULT4 ? launch_fixed(k, s->P, s->stream)
                   : (k.qmode == 1 || k.qmode == 2) ? launch_scan(k, s->P, s->stream)
                   : k.qmode == 3 ? launch_calendar(k, s->P, s->stream)
                                  : launch_heap(k, s->P, s->stream);
-  if (e != cudaSuccess) return set_error(LBFT_ERR_CUDA, std::string("kernel launch (") + kernel_name(s) + "): " + cudaGetErrorString(e));
+  if (e != cudaSuccess) return set_error(LBFT_ERR_CUDA, std::string("kernel launch (") + kernel_name(k) + "): " + cudaGetErrorString(e));
   CUDA_TRY(cudaEventRecord(s->ev[3], s->stream));
   return LBFT_OK;
 }
@@ -585,7 +545,7 @@ int lbft_timing_info(lbft_sim* s, lbft_timing* out) {
 }
 int lbft_kernel_info(lbft_sim* s, char* buf, size_t cap) {
   if (!s || !buf || cap == 0) return set_error(LBFT_ERR_INVALID, "NULL argument");
-  snprintf(buf, cap, "%s", kernel_name(s).c_str());
+  snprintf(buf, cap, "%s", kernel_name(s->hs.sel).c_str());
   return LBFT_OK;
 }
 int lbft_memory_info(lbft_sim* s, uint64_t* device_bytes, uint32_t* words_per_instance) {

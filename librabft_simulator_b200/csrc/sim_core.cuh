@@ -44,14 +44,6 @@
 #include <cmath>
 #endif
 
-// A/B switches of two exact optimisations: see enqueue_network_event and st_u16.
-#ifndef LBFT_ELIDE_SILENT
-#define LBFT_ELIDE_SILENT 1
-#endif
-#ifndef LBFT_ST16
-#define LBFT_ST16 1
-#endif
-
 namespace lbft {
 
 // Status bits — keep in sync with include/lbft.h (static_asserted in lbft_api.cu).
@@ -338,12 +330,12 @@ LBFT_COLD PartitionSpan partition_span(Mem m, uint32_t part_base, uint32_t windo
 // variant; plain thread-per-instance kernels only.
 // KS: (QMODE 3) the calendar's kind-occupancy words live in shared memory (`km`) for the whole run instead of the instance's
 // HBM block: the first hop of every pop and the occupancy test of every push become shared-memory accesses, and a push
-// into an empty list issues no load at all.  Sparse-tile thread kernels and the wide kernels (a handful of instances per
-// warp: (max_clock + 8) / 8 words each fit); plain one-shot runs only (nothing is kept between launches).
+// into an empty list issues no load at all.  Sparse-tile thread kernels (a handful of instances per warp: (max_clock + 8) / 8
+// words each fit); plain one-shot runs only (nothing is kept between launches).
 template <class Mem, int NMAX, int QMODE, int FX = 0, bool REC = false, bool RES = false, int G = 1, bool EP = false,
           bool TDS = false, bool KS = false>
 struct Core {
-  static_assert(!KS || (QMODE == 3 && !RES), "shared-memory occupancy words: calendar queue, one-shot runs");
+  static_assert(!KS || (QMODE == 3 && !RES && G == 1), "shared-memory occupancy words: calendar queue, one-shot thread kernels");
   static constexpr bool FIXED = FX != FX_NONE;                               // compile-time layout, reference delay model
   static constexpr bool MAY_SILENT = FX == FX_NONE || FX == FX_COMMITTEE64;  // silent nodes (extension D.2) reachable
   static_assert(!(FIXED && EP), "the compile-time layout is single-epoch");
@@ -366,11 +358,10 @@ struct Core {
   // dropped at a stop must be the one the reference drops).
   static constexpr bool ELIDE = !(REC || RES);
   static constexpr int S = Mem::STRIDE;
-  static constexpr int KSTR = WIDE ? 1 : S;  // KS: stride between this instance's occupancy words (a column per lane / contiguous)
-  uint32_t* km = nullptr;                    // KS: this instance's occupancy words in shared memory
-  LBFT_HD uint32_t km_ld(uint32_t w) const { return KS ? km[w * KSTR] : m.ld(L.cal_kmask + w); }
+  uint32_t* km = nullptr;  // KS: this instance's occupancy words in shared memory, a column per lane
+  LBFT_HD uint32_t km_ld(uint32_t w) const { return KS ? km[w * S] : m.ld(L.cal_kmask + w); }
   LBFT_HD void km_st(uint32_t w, uint32_t v) const {
-    if (KS) km[w * KSTR] = v;
+    if (KS) km[w * S] = v;
     else m.st(L.cal_kmask + w, v);
   }
   const Params& P;
@@ -490,13 +481,7 @@ struct Core {
   // (a 16-bit store: the read-modify-write of the containing word put a dependent load — a DRAM miss in the 64-author
   // configuration — in front of every accepted timeout)
   LBFT_HD static void st_u16(uint32_t* p, uint32_t i, uint32_t v) {
-    if (LBFT_ST16) {
-      reinterpret_cast<uint16_t*>(p + (i >> 1) * S)[i & 1] = (uint16_t)v;  // little-endian halves, as ld_u16 reads them
-      return;
-    }
-    uint32_t x = p[(i >> 1) * S];
-    uint32_t sh = 16 * (i & 1);
-    p[(i >> 1) * S] = (x & ~(0xffffu << sh)) | (v << sh);
+    reinterpret_cast<uint16_t*>(p + (i >> 1) * S)[i & 1] = (uint16_t)v;  // little-endian halves, as ld_u16 reads them
   }
   LBFT_HD bool mbit_test(uint32_t w, uint32_t r) const { return (m.ld(w + (r >> 5)) >> (r & 31)) & 1u; }
   LBFT_HD void mbit_set(uint32_t w, uint32_t r) const { m.st(w + (r >> 5), m.ld(w + (r >> 5)) | (1u << (r & 31))); }
@@ -1353,7 +1338,7 @@ struct Core {
     // event up to max_clock is popped before a one-shot run ends — and keep the event, a third of the 64-author
     // configuration's traffic, out of the queue and out of the snapshot's reference count.  It still takes its creation
     // stamp and its delay draw.  Not while recording / resumable / true-data-sync (every pop is observable there).
-    if (LBFT_ELIDE_SILENT && ELIDE && !TDS && MAY_SILENT && P.silent_mask && kind != EV_RESPONSE &&
+    if (ELIDE && !TDS && MAY_SILENT && P.silent_mask && kind != EV_RESPONSE &&
         ((P.silent_mask >> (kind == EV_NOTIFY ? receiver : sender)) & 1)) {
       stamp++;
       if (stamp >= kStampLimit) status |= ST_QUEUE_OVERFLOW;

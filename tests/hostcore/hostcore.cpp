@@ -39,9 +39,9 @@ static void run_all(const Params& P, std::vector<uint32_t>& state, const double*
   else run_all_ep<NMAX, QMODE, REC, RES, false>(P, state, zx, zf);
 }
 
-// The instantiations with a compile-time layout (sim_core.cuh FX, sim_params.h fixed_layout) on the host: selected the way
-// lbft_api.cu select_kernel does (minus the kernel family / tile / lane-group conditions, which do not exist here), so that
-// the CPU tests of those shapes exercise the very state machine the BASELINE configurations run on the GPU.
+// The instantiations with a compile-time layout (sim_core.cuh FX, sim_params.h fixed_layout) on the host: selected by the
+// product's fixed_shape_of (host_setup.hpp; the kernel family / tile / lane-group conditions do not exist here), so that the
+// CPU tests of those shapes exercise the very state machine the BASELINE configurations run on the GPU.
 template <int NMAX, int QMODE, int FX>
 static void run_all_fx(const Params& P, std::vector<uint32_t>& state, const double* zx, const double* zf) {
   for (uint32_t inst = 0; inst < P.num_instances; inst++) {
@@ -49,7 +49,7 @@ static void run_all_fx(const Params& P, std::vector<uint32_t>& state, const doub
     TileMem<32> mem{state.data() + (size_t)tile * P.L.total_words * 32, lane};
     std::vector<uint32_t> sk(QMODE == 2 ? (size_t)P.L.queue_cap * 32 : 1);
     std::vector<uint16_t> sd(QMODE == 2 ? (size_t)P.L.queue_cap * 32 : 1);
-    // (calendar queue: with the occupancy words in a stand-in for shared memory, as the sparse-tile / wide kernels hold them)
+    // (calendar queue: with the occupancy words in a stand-in for shared memory, as the sparse-tile kernels hold them)
     constexpr bool KS = QMODE == 3;
     std::vector<uint32_t> km(KS ? (size_t)((P.L.cal_times + 7) / 8) * 32 : 1);
     Core<TileMem<32>, NMAX, QMODE, FX, false, false, 1, false, false, KS> core(P, mem, zx, zf, P.delay_thr, sk.data() + lane, sd.data() + lane);
@@ -59,17 +59,6 @@ static void run_all_fx(const Params& P, std::vector<uint32_t>& state, const doub
     core.finalize(inst);
   }
 }
-static int fixed_selected(const Params& P) {
-  constexpr Layout kDefault4 = fixed_layout(FX_DEFAULT4), kPart7 = fixed_layout(FX_PART7), kCommittee64 = fixed_layout(FX_COMMITTEE64);
-  const bool table_delay = P.delay_kind == LBFT_DELAY_LOGNORMAL && !P.delay_const && P.delay_kmax != 0;
-  const bool plain_model = table_delay && P.delay_kmax + 2 <= 256 && P.silent_mask == 0;
-  if (P.record_rs || P.resumable) return FX_NONE;
-  if (P.L.queue_scan == 2 && plain_model && memcmp(&P.L, &kDefault4, sizeof(Layout)) == 0) return FX_DEFAULT4;
-  if (P.L.queue_scan == 3 && plain_model && memcmp(&P.L, &kPart7, sizeof(Layout)) == 0) return FX_PART7;
-  if (P.L.queue_scan == 3 && table_delay && memcmp(&P.L, &kCommittee64, sizeof(Layout)) == 0) return FX_COMMITTEE64;
-  return FX_NONE;
-}
-
 static int run_impl(const lbft_config* c, uint32_t* commit_counts, uint64_t* last_states, uint32_t* lc_round,
                     uint32_t* counters, uint32_t* status, uint32_t* words_per_instance, std::vector<uint32_t>& state,
                     Params& P, const int64_t* stops = nullptr, size_t nstops = 0);
@@ -109,7 +98,16 @@ int hostcore_setup_info(const lbft_config* c, uint32_t* out6) {
 int hostcore_fixed_shape(const lbft_config* c) {
   HostSetup hs;
   if (!hs.build(*c)) { g_err = hs.error; return -1; }
-  return getenv("HOSTCORE_NO_FIXED") ? (int)FX_NONE : fixed_selected(hs.params);
+  return getenv("HOSTCORE_NO_FIXED") ? (int)FX_NONE : fixed_shape_of(hs.params);
+}
+
+// The product's lbft_kernel_info for this configuration: the kernel HostSetup selects (LBFT_FORCE_KERNEL included).
+int hostcore_kernel_info(const lbft_config* c, char* buf, size_t cap) {
+  HostSetup hs;
+  if (!hs.build(*c)) { g_err = hs.error; return LBFT_ERR_INVALID; }
+  if (!buf || cap == 0) { g_err = "NULL argument"; return LBFT_ERR_INVALID; }
+  snprintf(buf, cap, "%s", kernel_name(hs.sel).c_str());
+  return LBFT_OK;
 }
 
 // Same outputs as the product's lbft_* getters; chain_out (optional) receives, per instance,
@@ -194,7 +192,7 @@ static int run_impl(const lbft_config* c, uint32_t* commit_counts, uint64_t* las
                               : run_all<NMAX, QS, false, true>(P, state, P.zig_x, P.zig_f))                          \
                : (P.record_rs ? run_all<NMAX, QS, true, false>(P, state, P.zig_x, P.zig_f)                          \
                               : run_all<NMAX, QS, false, false>(P, state, P.zig_x, P.zig_f)))
-  const int fx = getenv("HOSTCORE_NO_FIXED") ? (int)FX_NONE : fixed_selected(P);
+  const int fx = getenv("HOSTCORE_NO_FIXED") ? (int)FX_NONE : fixed_shape_of(P);
   if (fx == FX_DEFAULT4) run_all_fx<16, 2, FX_DEFAULT4>(P, state, P.zig_x, P.zig_f);
   else if (fx == FX_PART7) run_all_fx<16, 3, FX_PART7>(P, state, P.zig_x, P.zig_f);
   else if (fx == FX_COMMITTEE64) run_all_fx<64, 3, FX_COMMITTEE64>(P, state, P.zig_x, P.zig_f);

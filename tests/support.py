@@ -201,6 +201,14 @@ class HostCore:
         cfg, keep = make_config([1], num_nodes, max_clock, **kw)
         return self.lib.hostcore_fixed_shape(ctypes.byref(cfg))
 
+    def kernel_info(self, seeds, num_nodes, max_clock=1000, **kw):
+        """The product's lbft_kernel_info for this configuration (the kernel the host selects; honours LBFT_FORCE_KERNEL)."""
+        cfg, keep = make_config(seeds, num_nodes, max_clock, **kw)
+        buf = ctypes.create_string_buffer(128)
+        if self.lib.hostcore_kernel_info(ctypes.byref(cfg), buf, ctypes.sizeof(buf)) != 0:
+            raise RuntimeError(self.lib.hostcore_last_error().decode())
+        return buf.value.decode()
+
     def run(self, seeds, num_nodes, max_clock=1000, **kw):
         cfg, keep = make_config(seeds, num_nodes, max_clock, **kw)
         I = cfg.num_instances

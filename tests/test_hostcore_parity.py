@@ -130,3 +130,57 @@ def test_compile_time_shapes_match_the_oracle_and_the_generic_instantiation(orac
     assert hostcore.fixed_shape(7, 1000, partition_windows=4, partition_max_len=150, silent=[1, 0, 0, 0, 0, 0, 0]) == 0
     assert hostcore.fixed_shape(48, 1000) == 0
     assert hostcore.fixed_shape(4, 1000, flags=1) == 0                                          # recording
+
+
+def test_kernel_choice(hostcore, monkeypatch):
+    """The kernel the host selects (lbft_kernel_info, through the host setup the product runs): the automatic picks that
+    tests/test_gpu_wide.py::test_automatic_choice asserts on the GPU, and what LBFT_FORCE_KERNEL makes of the same cases."""
+    cases = (("config2", 1024, 4, {}), ("config3", 65536, 4, {}), ("config5", 16384, 7, {}),
+             ("config5p", 16384, 7, {"partition_windows": 4, "partition_max_len": 150}),
+             ("mid7", 8192, 7, {}), ("full7", 65536, 7, {}), ("big64", 8192, 64, {}),
+             ("small64", 64, 64, {}), ("resumable", 64, 4, {"flags": 2}),
+             ("recording", 64, 7, {"flags": 1}), ("mid4", 8192, 4, {}),
+             ("long7", 64, 7, {"max_clock": 20000}))
+
+    def picks(family):
+        if family:
+            monkeypatch.setenv("LBFT_FORCE_KERNEL", family)
+        else:
+            monkeypatch.delenv("LBFT_FORCE_KERNEL", raising=False)
+        out = {}
+        for name, count, nodes, kw in cases:
+            kw = dict(kw)
+            max_clock = kw.pop("max_clock", 1000)
+            out[name] = hostcore.kernel_info(np.arange(1, count + 1, dtype=np.uint64), nodes, max_clock, **kw)
+        return out
+
+    # <NMAX, QMODE, SMEM, lanes per instance, EP, FX> / <NMAX, QMODE, FX, REC, RES, EP, TDS, instances per warp tile>
+    auto = picks(None)
+    assert auto["config2"] == "lbft_wide_kernel<16,2,true,32,false,0>"    # a warp per instance, whole instance in shared memory
+    assert auto["config3"] == auto["mid4"] == "lbft_event_loop_kernel<16,2,1,false,false,false,false,32>"
+    assert auto["config5"] == "lbft_event_loop_kernel<16,3,0,false,false,false,false,8>"  # one wave of 8-instance warp tiles
+    assert auto["config5p"] == "lbft_event_loop_kernel<16,3,2,false,false,false,false,8>"  # ... BASELINE configs[4]: its compile-time shape
+    assert auto["mid7"] == "lbft_wide_kernel<16,2,false,8,false,0>"       # 8 lanes per instance, four instances per warp
+    assert auto["full7"] == "lbft_event_loop_kernel<16,3,0,false,false,false,false,32>"
+    assert auto["small64"] == "lbft_wide_kernel<64,3,false,32,false,0>"
+    assert auto["big64"] == "lbft_wide_kernel<64,3,false,8,false,3>"      # BASELINE configs[3]: compile-time shape, 8 lanes per instance
+    assert auto["long7"] == "lbft_wide_kernel<16,0,false,32,false,0>"     # beyond the 14-bit times of the compact queue
+    assert auto["resumable"] == "lbft_event_loop_kernel<16,1,0,false,true,false,false,32>"
+    assert auto["recording"] == "lbft_event_loop_kernel<16,3,0,true,false,false,false,32>"
+
+    # forced to one thread per instance: full warp tiles; the compile-time layout only where it is the thread kernel's
+    thread = picks("thread")
+    assert thread["config2"] == thread["config3"] == thread["mid4"] == "lbft_event_loop_kernel<16,2,1,false,false,false,false,32>"
+    for name in ("config5", "config5p", "mid7", "full7"):
+        assert thread[name] == "lbft_event_loop_kernel<16,3,0,false,false,false,false,32>", name
+    assert thread["big64"] == thread["small64"] == "lbft_event_loop_kernel<64,3,0,false,false,false,false,32>"
+    assert thread["long7"] == "lbft_event_loop_kernel<16,0,0,false,false,false,false,32>"
+
+    # forced to the wide kernel: the shared-memory queue up to 16 authors; recording / resumable handles stay on the thread kernel
+    wide = picks("wide")
+    assert wide["config2"] == "lbft_wide_kernel<16,2,true,32,false,0>"
+    for name in ("config3", "mid4", "config5", "config5p", "mid7", "full7"):
+        assert wide[name] == "lbft_wide_kernel<16,2,false,8,false,0>", name
+    assert wide["big64"] == auto["big64"] and wide["small64"] == auto["small64"] and wide["long7"] == auto["long7"]
+    assert thread["resumable"] == wide["resumable"] == auto["resumable"]
+    assert thread["recording"] == wide["recording"] == auto["recording"]

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
-"""Compare the SASS of every lbft_event_loop_kernel instantiation in two builds of the library (addresses and
-encodings stripped).  Usage: python tools/sass_compare.py OLD.so NEW.so"""
+"""Compare the SASS of every kernel in two builds of the library, symbol by symbol under the full mangled name (addresses
+and encodings stripped), and list the kernels present in only one of them.  Usage: python tools/sass_compare.py OLD.so NEW.so
+Exits non-zero if any kernel differs or is missing on one side."""
 import re
 import subprocess
 import sys
@@ -22,16 +23,16 @@ def kernels(path):
     return res
 
 
-def key(name):  # <NMAX, QMODE, FIXED, REC, RES>; REC / RES default to 0 for builds that predate them
-    m = re.search(r"kernelILi(\d+)ELi(\d)ELb([01])E(?:Lb([01])E)?(?:Lb([01])E)?", name)
-    return None if not m else (int(m.group(1)), int(m.group(2)), int(m.group(3)), int(m.group(4) or 0), int(m.group(5) or 0))
-
-
-old = {key(k): v for k, v in kernels(sys.argv[1]).items() if key(k)}
-new = {key(k): v for k, v in kernels(sys.argv[2]).items() if key(k)}
-for k in sorted(new):
-    if k not in old:
-        verdict = "new instantiation"
+old, new = kernels(sys.argv[1]), kernels(sys.argv[2])
+same = 0
+for k in sorted(set(old) | set(new)):
+    if k not in new:
+        print("only in OLD  %6d instructions  %s" % (len(old[k]), k))
+    elif k not in old:
+        print("only in NEW  %6d instructions  %s" % (len(new[k]), k))
+    elif old[k] != new[k]:
+        print("DIFFERS      %6d -> %d instructions  %s" % (len(old[k]), len(new[k]), k))
     else:
-        verdict = "IDENTICAL" if old[k] == new[k] else "differs (%d -> %d instructions)" % (len(old[k]), len(new[k]))
-    print("<%d,%d,%d,%d,%d> %6d instructions  %s" % (k + (len(new[k]), verdict)))
+        same += 1
+print("%d kernels identical, %d in OLD, %d in NEW" % (same, len(old), len(new)))
+sys.exit(0 if same == len(old) == len(new) else 1)
