@@ -302,8 +302,251 @@ LBFT_COLD PartitionSpan partition_span(Mem m, uint32_t part_base, uint32_t windo
   return sp;
 }
 
-// QMODE: 0 binary heap (3-word entries, HBM) | 1 scan queue, 64-bit keys in HBM | 2 scan queue, 32-bit keys +
-// 16-bit payload words in shared memory (small committees, short horizons) | 3 calendar queue in HBM
+// ---- the pending-event queue, ordered by (time, 3-kind, stamp)  (simulator.rs:149-161) ----------------------------------
+// One type per QMODE (Core::Queue).  Core::push_event assigns the creation stamp, drops what cannot be queued and counts the
+// queued events (n); the type stores and retrieves entries: attach(sk, sd), put(m, L, n, time, kind, stamp, data) with n <
+// queue_cap, take(m, L, n, wl, gm, time, kind, data) with n >= 1 (wl, gm: lane and group), clear(m, L, wl, km) at init; for
+// resumable runs walk_regs(v) (its save-area words) and save / restore(m, L, at, n).  Stamps stay below kStampLimit.
+
+template <int G>
+LBFT_HD void group_sync(uint32_t gm) {
+#if defined(__CUDA_ARCH__)
+  if (G > 1) __syncwarp(gm);
+#endif
+}
+
+// The payload word of the scan queues' entries: slot:8 | sender:4 | receiver:4 (slot 0xff: none).
+LBFT_HD uint32_t pack_data16(uint32_t data) { return (((data >> 16) & 0xffu) << 8) | (((data >> 8) & 0xfu) << 4) | (data & 0xfu); }
+LBFT_HD uint32_t unpack_data16(uint32_t lo) {
+  const uint32_t slot = lo >> 8;
+  return (lo & 0xfu) | (((lo >> 4) & 0xfu) << 8) | ((slot == 0xffu ? PAY_NONE : slot) << 16);
+}
+
+// Min-scan of the scan queues' keys k[0], k[stride], ..., k[(n - 1) * stride], n >= 1: the index of the least key, which is
+// left in `mn`.  The type of `stride` sets the width of the index arithmetic (32-bit in shared memory, size_t in HBM).
+template <int G, class K, class I>
+LBFT_HD uint32_t min_scan(const K* k, I stride, uint32_t n, uint32_t wl, uint32_t gm, K& mn) {
+  if constexpr (G == 1) {  // one lane: independent loads, no data-dependent chains
+    mn = k[0];
+    uint32_t bi = 0, j = 1;
+#pragma unroll 1
+    for (; j + 3 < n; j += 4) {
+      const K k0 = k[j * stride], k1 = k[(j + 1) * stride], k2 = k[(j + 2) * stride], k3 = k[(j + 3) * stride];
+      if (k0 < mn) { mn = k0; bi = j; }
+      if (k1 < mn) { mn = k1; bi = j + 1; }
+      if (k2 < mn) { mn = k2; bi = j + 2; }
+      if (k3 < mn) { mn = k3; bi = j + 3; }
+    }
+#pragma unroll 1
+    for (; j < n; j++) {
+      const K k0 = k[j * stride];
+      if (k0 < mn) { mn = k0; bi = j; }
+    }
+    return bi;
+  } else {  // the group (mask gm) scans together: lane wl looks at entries wl, wl + G, ...; keys are unique (creation stamps)
+#if defined(__CUDA_ARCH__)
+    __syncwarp(gm);  // entries pushed by this iteration's sends
+    K best = ~(K)0;
+    uint32_t bi = 0;
+    for (uint32_t j = wl; j < n; j += G) {
+      const K k0 = k[j * stride];
+      if (k0 < best) { best = k0; bi = j; }
+    }
+    if constexpr (sizeof(K) == 8) {
+      // 64-bit minimum over the group: high words first, then low words among the lanes that hold the minimal high word
+      const uint32_t hi = __reduce_min_sync(gm, (uint32_t)(best >> 32));
+      const uint32_t lo = __reduce_min_sync(gm, (uint32_t)(best >> 32) == hi ? (uint32_t)best : 0xffffffffu);
+      mn = ((uint64_t)hi << 32) | lo;
+    } else {
+      mn = __reduce_min_sync(gm, best);
+    }
+    const uint32_t src = (uint32_t)__ffs((int)__ballot_sync(gm, best == mn)) - 1u;  // a lane of this group (absolute index)
+    return __shfl_sync(gm, bi, (int)src);
+#else
+    return 0;  // (the host harness runs one thread per instance)
+#endif
+  }
+}
+
+// What a queue does that has nothing to clear, no registers and no entries outside the instance state.  Its three register
+// words of the save area hold what a fresh calendar queue holds, so that the save area reads the same whichever queue wrote it.
+template <class Mem>
+struct QueueDefaults {
+  LBFT_HD static void attach(uint32_t*, uint16_t*) {}
+  LBFT_HD static void clear(const Mem&, const Layout&, uint32_t, uint32_t*) {}
+  template <class V>
+  LBFT_HD static void walk_regs(V& v) { uint32_t cur = 0, pool_free = PAY_NONE, pool_next = 0; v(cur); v(pool_free); v(pool_next); }
+  LBFT_HD static void save(const Mem&, const Layout&, uint32_t, uint32_t) {}
+  LBFT_HD static void restore(const Mem&, const Layout&, uint32_t, uint32_t) {}
+};
+
+// QMODE 0: binary min-heap of 3-word entries (time | 3-kind:2 stamp:30 | data) in the instance's queue area.
+template <class Mem, int G>
+struct HeapQueue : QueueDefaults<Mem> {
+  static constexpr uint32_t kStampLimit = 1u << 30;
+  LBFT_HD static uint64_t key_at(const Mem& m, const Layout& L, uint32_t i) { return ((uint64_t)m.ld(L.heap_time + i) << 32) | m.ld(L.heap_key + i); }
+  LBFT_HD static void move(const Mem& m, const Layout& L, uint32_t dst, uint32_t src) {
+    m.st(L.heap_time + dst, m.ld(L.heap_time + src));
+    m.st(L.heap_key + dst, m.ld(L.heap_key + src));
+    m.st(L.heap_data + dst, m.ld(L.heap_data + src));
+  }
+  LBFT_HD static void store(const Mem& m, const Layout& L, uint32_t i, uint32_t t, uint32_t k, uint32_t d) { m.st(L.heap_time + i, t); m.st(L.heap_key + i, k); m.st(L.heap_data + i, d); }
+  LBFT_HD void put(const Mem& m, const Layout& L, uint32_t i, int32_t time, uint32_t kind, uint32_t st, uint32_t data) {
+    uint32_t klo = ((3u - kind) << 30) | st;
+    uint64_t key = ((uint64_t)(uint32_t)time << 32) | klo;
+    while (i > 0) {
+      uint32_t p = (i - 1) >> 1;
+      if (key_at(m, L, p) <= key) break;
+      move(m, L, i, p);
+      i = p;
+    }
+    store(m, L, i, (uint32_t)time, klo, data);
+  }
+  LBFT_HD void take(const Mem& m, const Layout& L, uint32_t n, uint32_t, uint32_t, int32_t& time, uint32_t& kind, uint32_t& data) {
+    time = (int32_t)m.ld(L.heap_time);
+    uint32_t klo = m.ld(L.heap_key);
+    data = m.ld(L.heap_data);
+    kind = 3u - (klo >> 30);
+    if (--n == 0) return;
+    uint32_t lt = m.ld(L.heap_time + n), lk = m.ld(L.heap_key + n), ld_ = m.ld(L.heap_data + n);
+    uint64_t key = ((uint64_t)lt << 32) | lk;
+    uint32_t i = 0;
+    for (;;) {
+      uint32_t c = 2 * i + 1;
+      if (c >= n) break;
+      uint64_t kc = key_at(m, L, c);
+      if (c + 1 < n) {
+        uint64_t kr = key_at(m, L, c + 1);
+        if (kr < kc) { kc = kr; c = c + 1; }
+      }
+      if (key <= kc) break;
+      move(m, L, i, c);
+      i = c;
+    }
+    store(m, L, i, lt, lk, ld_);
+  }
+};
+
+// QMODE 1: unsorted array in the instance's queue area, O(1) append, min-scan on take.  64-bit keys
+// time:24 | 3-kind:2 | stamp:22 | payload word:16; stamps are unique, so the payload bits below them never decide a comparison.
+template <class Mem, int G>
+struct HbmScanQueue : QueueDefaults<Mem> {
+  static constexpr uint32_t kStampLimit = 1u << 22;
+  static constexpr size_t S = Mem::STRIDE;
+  LBFT_HD void put(const Mem& m, const Layout& L, uint32_t n, int32_t time, uint32_t kind, uint32_t st, uint32_t data) {
+    uint64_t key = ((uint64_t)(uint32_t)time << 40) | ((uint64_t)(3u - kind) << 38) | ((uint64_t)st << 16) | (uint64_t)pack_data16(data);
+    m.at64(L.heap_time)[n * S] = key;
+  }
+  LBFT_HD void take(const Mem& m, const Layout& L, uint32_t n, uint32_t wl, uint32_t gm, int32_t& time, uint32_t& kind, uint32_t& data) {
+    uint64_t* q = m.at64(L.heap_time);
+    uint64_t mn;
+    const uint32_t bi = min_scan<G>(q, S, n, wl, gm, mn);
+    if constexpr (G > 1) {
+      const uint64_t last = q[(n - 1) * S];
+      group_sync<G>(gm);  // everyone has read its share of the keys and the last entry
+      if (bi != n - 1) q[bi * S] = last;
+    } else if (bi != n - 1) q[bi * S] = q[(n - 1) * S];
+    time = (int32_t)(mn >> 40);
+    kind = 3u - ((uint32_t)(mn >> 38) & 3u);
+    data = unpack_data16((uint32_t)mn & 0xffffu);
+  }
+};
+
+// QMODE 2: unsorted array in shared memory (small committees, short horizons), O(1) append, min-scan on take.  32-bit keys
+// time:14 | 3-kind:2 | stamp:16 (stamps are unique, so they decide every comparison) and 16-bit payload words beside them.
+// Thread kernel: a column per lane; wide kernel: one contiguous queue per group.
+template <class Mem, int G>
+struct SmemScanQueue : QueueDefaults<Mem> {
+  static constexpr uint32_t kStampLimit = 1u << 16;
+  static constexpr uint32_t QS = G > 1 ? 1 : 32;  // stride between entries
+  uint32_t* sk = nullptr;  // keys, sk[j * QS]
+  uint16_t* sd = nullptr;  // payload words, sd[j * QS]
+  LBFT_HD void attach(uint32_t* k, uint16_t* d) { sk = k; sd = d; }
+  LBFT_HD void put(const Mem&, const Layout&, uint32_t n, int32_t time, uint32_t kind, uint32_t st, uint32_t data) {
+    sk[n * QS] = ((uint32_t)time << 18) | ((3u - kind) << 16) | (st & 0xffffu);
+    sd[n * QS] = (uint16_t)pack_data16(data);
+  }
+  LBFT_HD void take(const Mem&, const Layout&, uint32_t n, uint32_t wl, uint32_t gm, int32_t& time, uint32_t& kind, uint32_t& data) {
+    uint32_t mn;
+    const uint32_t bi = min_scan<G>(sk, QS, n, wl, gm, mn);
+    const uint32_t lo = sd[bi * QS];
+    group_sync<G>(gm);  // everyone has read sd[bi] / its share of the keys
+    if (bi != n - 1) { sk[bi * QS] = sk[(n - 1) * QS]; sd[bi * QS] = sd[(n - 1) * QS]; }
+    time = (int32_t)(mn >> 18);
+    kind = 3u - ((mn >> 16) & 3u);
+    data = unpack_data16(lo);
+  }
+  // Resumable runs (thread kernel only) keep the entries in the save area between two launches: n keys, then at
+  // at + queue_cap the payload words, two to a word.
+  LBFT_HD void save(const Mem& m, const Layout& L, uint32_t at, uint32_t n) const {
+    for (uint32_t j = 0; j < n; j++) m.st(at + j, sk[j * QS]);
+    for (uint32_t j = 0; j < n; j += 2) m.st(at + L.queue_cap + (j >> 1), (uint32_t)sd[j * QS] | (j + 1 < n ? (uint32_t)sd[(j + 1) * QS] << 16 : 0u));
+  }
+  LBFT_HD void restore(const Mem& m, const Layout& L, uint32_t at, uint32_t n) const {
+    for (uint32_t j = 0; j < n; j++) { sk[j * QS] = m.ld(at + j); sd[j * QS] = (uint16_t)(m.ld(at + L.queue_cap + (j >> 1)) >> ((j & 1) * 16)); }
+  }
+};
+
+// QMODE 3: calendar queue in HBM: one FIFO list per (time, kind) threaded through an entry pool (heap_time: `next` links,
+// heap_key: data words), a head | tail << 16 word per list, and kind-occupancy nibbles per time slot.  Stamps grow with every
+// put, so FIFO order inside a list IS stamp order, and take() serves the kinds in priority order: exactly (time, kind desc, stamp).
+// KS: the occupancy words live in shared memory (`km`, a column per lane, given at init) for the whole run instead of the
+// instance's HBM block, so the first hop of every take and the occupancy test of every put are shared-memory accesses.
+// Sparse-tile thread kernels ((max_clock + 8) / 8 words per instance fit); plain one-shot runs only.
+template <class Mem, int G, bool KS>
+struct CalendarQueue : QueueDefaults<Mem> {
+  static constexpr uint32_t kStampLimit = 0xfffffff0u;
+  uint32_t* km = nullptr;
+  uint32_t cur, pool_free, pool_next;  // current time slot, pool free list head, pool bump pointer
+  LBFT_HD uint32_t km_ld(const Mem& m, const Layout& L, uint32_t w) const { return KS ? km[w * Mem::STRIDE] : m.ld(L.cal_kmask + w); }
+  LBFT_HD void km_st(const Mem& m, const Layout& L, uint32_t w, uint32_t v) const { if (KS) km[w * Mem::STRIDE] = v; else m.st(L.cal_kmask + w, v); }
+  LBFT_HD void put(const Mem& m, const Layout& L, uint32_t, int32_t time, uint32_t kind, uint32_t, uint32_t data) {
+    uint32_t e;
+    if (pool_free != PAY_NONE) { e = pool_free; pool_free = m.ld(L.heap_time + e); }
+    else e = pool_next++;
+    m.st(L.heap_key + e, data);
+    const uint32_t t = (uint32_t)time, kw = t >> 3, sh = (t & 7) * 4 + kind, hw = L.cal_ht + t * 4 + kind;
+    uint32_t occ = km_ld(m, L, kw);
+    if ((occ >> sh) & 1) {
+      uint32_t ht = m.ld(hw);
+      m.st(L.heap_time + (ht >> 16), e);  // old tail -> e
+      m.st(hw, (ht & 0xffffu) | (e << 16));
+    } else {
+      m.st(hw, e | (e << 16));
+      km_st(m, L, kw, occ | (1u << sh));
+    }
+  }
+  LBFT_HD void take(const Mem& m, const Layout& L, uint32_t, uint32_t, uint32_t, int32_t& time, uint32_t& kind, uint32_t& data) {
+    // advance to the first time slot with a pending list (puts never go below the current slot)
+    uint32_t kw = cur >> 3;
+    uint32_t occ = km_ld(m, L, kw) >> ((cur & 7) * 4);
+    while (occ == 0) { cur = (cur | 7) + 1; kw++; occ = km_ld(m, L, kw); }
+    while ((occ & 15u) == 0) { occ >>= 4; cur++; }
+    const uint32_t nib = occ & 15u;
+    kind = nib & 8u ? 3u : (nib & 4u ? 2u : (nib & 2u ? 1u : 0u));  // Timer 3 > Response 2 > Request 1 > Notify 0
+    const uint32_t hw = L.cal_ht + cur * 4 + kind;
+    const uint32_t ht = m.ld(hw), e = ht & 0xffffu;
+    data = m.ld(L.heap_key + e);
+    if (e == (ht >> 16)) km_st(m, L, kw, km_ld(m, L, kw) & ~(1u << ((cur & 7) * 4 + kind)));  // list became empty
+    else m.st(hw, (ht & 0xffff0000u) | m.ld(L.heap_time + e));
+    m.st(L.heap_time + e, pool_free);
+    pool_free = e;
+    time = (int32_t)cur;
+  }
+  LBFT_HD void clear(const Mem& m, const Layout& L, uint32_t wl, uint32_t* km_) {
+    km = km_; cur = 0; pool_free = PAY_NONE; pool_next = 0;
+    for (uint32_t w = wl; w < (L.cal_times + 7) / 8; w += G) km_st(m, L, w, 0);
+  }
+  template <class V>
+  LBFT_HD void walk_regs(V& v) { v(cur); v(pool_free); v(pool_next); }
+};
+
+template <int QMODE, class Mem, int G, bool KS>
+using QueueFor = typename std::conditional<QMODE == 0, HeapQueue<Mem, G>, typename std::conditional<QMODE == 1, HbmScanQueue<Mem, G>,
+    typename std::conditional<QMODE == 2, SmemScanQueue<Mem, G>, CalendarQueue<Mem, G, KS>>::type>::type>::type;
+
+// QMODE: the event queue (Queue, above): 0 binary heap (3-word entries, HBM) | 1 scan queue, 64-bit keys in HBM |
+// 2 scan queue, 32-bit keys + 16-bit payload words in shared memory | 3 calendar queue in HBM
 // FX (FIXED = FX != 0): the layout is the compile-time constant fixed_layout(FX) (sim_params.h: the default four-author
 // shape of BASELINE configs 1-3, the seven-author partition shape of configs[4], the 64-author shape of configs[3])
 // instead of the launch parameter block: every field offset folds into an immediate.  The host only selects one for
@@ -328,10 +571,7 @@ LBFT_COLD PartitionSpan partition_span(Mem m, uint32_t part_base, uint32_t windo
 // and the response's records are inserted by the requester (what data_sync.rs:183-240 is written for), instead of the
 // reference simulator's dispatch to the requester itself (simulator.rs:446, SURVEY fact 5).  An opt-in NON-PARITY
 // variant; plain thread-per-instance kernels only.
-// KS: (QMODE 3) the calendar's kind-occupancy words live in shared memory (`km`) for the whole run instead of the instance's
-// HBM block: the first hop of every pop and the occupancy test of every push become shared-memory accesses, and a push
-// into an empty list issues no load at all.  Sparse-tile thread kernels (a handful of instances per warp: (max_clock + 8) / 8
-// words each fit); plain one-shot runs only (nothing is kept between launches).
+// KS: (QMODE 3) the calendar's kind-occupancy words live in shared memory (CalendarQueue).
 template <class Mem, int NMAX, int QMODE, int FX = 0, bool REC = false, bool RES = false, int G = 1, bool EP = false,
           bool TDS = false, bool KS = false>
 struct Core {
@@ -344,34 +584,23 @@ struct Core {
   static_assert(G == 1 || G == 8 || G == 16 || G == 32, "one thread, or a group of 8 / 16 / 32 lanes per instance");
   static_assert(G == 1 || !(REC || RES), "the wide kernel has no recording / resumable variants");
   static constexpr bool WIDE = G > 1;
-  static constexpr int QS = WIDE ? 1 : 32;  // QMODE 2: stride between queue entries in shared memory (a column per lane / contiguous)
   uint32_t wl = 0;            // this thread's lane inside the group (0 when G == 1)
   uint32_t gm = 0xffffffffu;  // wide kernel: the lanes of this thread's group, as a warp mask
   WideScratch* ws = nullptr;  // wide kernel: the group's scratch
-  LBFT_HD void grp_sync() const {
-#if defined(__CUDA_ARCH__)
-    if (WIDE) __syncwarp(gm);
-#endif
-  }
   // Duplicate timers are accounted at push time instead of being queued (push_timer) only when every pop does not
   // matter individually: not while recording (each pop is a sampling point) and not in resumable runs (the event
   // dropped at a stop must be the one the reference drops).
   static constexpr bool ELIDE = !(REC || RES);
   static constexpr int S = Mem::STRIDE;
-  uint32_t* km = nullptr;  // KS: this instance's occupancy words in shared memory, a column per lane
-  LBFT_HD uint32_t km_ld(uint32_t w) const { return KS ? km[w * S] : m.ld(L.cal_kmask + w); }
-  LBFT_HD void km_st(uint32_t w, uint32_t v) const {
-    if (KS) km[w * S] = v;
-    else m.st(L.cal_kmask + w, v);
-  }
   const Params& P;
   const Layout L;
   Mem m;
   const double* zx;
   const double* zf;
   const double* thr;  // delay thresholds (shared-memory copy on the device when it fits)
-  uint32_t* sk;       // QMODE 2: this lane's key column,  sk[j * 32] = time:14 | 3-kind:2 | stamp:16
-  uint16_t* sd;       // QMODE 2: this lane's data column, sd[j * 32] = slot:8 | sender:4 | receiver:4
+  using Queue = QueueFor<QMODE, Mem, G, KS>;
+  Queue q;                 // given its shared memory by the constructor (QMODE 2: sk / sd, or the host harness's stand-in) and init (km)
+  uint32_t* km = nullptr;  // KS: the calendar's occupancy words in shared memory, a column per lane, set by the kernel
   // ---- per-instance registers ----
   uint64_t s0, s1, s2, s3;  // Xoshiro256** (simulator.rs:32)
   uint32_t draws;
@@ -382,15 +611,14 @@ struct Core {
   uint32_t pay_free, pay_next;
   uint32_t proc0, proc1, proc2, proc3, cancelled, max_queue, sched_notify, dedup;
   uint32_t win;                 // bitset word index speculatively loaded with the node (hint = last node handled)
-  uint32_t cal_t, cal_free, cal_next;  // QMODE 3: current bucket time, pool free list head, pool bump pointer
   int32_t part_until;  // partition plan: part_open holds for every clock below this (0: not computed yet)
   uint64_t part_open;  // ... the windows open in that span, a bit per window
   uint32_t rs_pend;  // recording only: node << 16 | active round of the round switch not yet stamped with a pop time (0: none)
   uint32_t cc0, cc1, cc2, cc3;  // chain cache: (round << 16) | previous QC round
 
-  LBFT_HD Core(const Params& p, Mem mem, const double* zx_, const double* zf_, const double* thr_, uint32_t* sk_ = nullptr,
-               uint16_t* sd_ = nullptr)
-      : P(p), L(FIXED ? fixed_layout(FX) : p.L), m(mem), zx(zx_), zf(zf_), thr(thr_), sk(sk_), sd(sd_) {}
+  LBFT_HD Core(const Params& p, Mem mem, const double* zx_, const double* zf_, const double* thr_, uint32_t* sk = nullptr,
+               uint16_t* sd = nullptr)
+      : P(p), L(FIXED ? fixed_layout(FX) : p.L), m(mem), zx(zx_), zf(zf_), thr(thr_) { q.attach(sk, sd); }
 
   // ------------------------------------------------------------------------------------------
   // RNG (rand_xoshiro 0.6.0 / rand 0.8.3 / rand_distr 0.4.0)
@@ -583,241 +811,24 @@ struct Core {
   LBFT_HD static uint32_t leader_of(const NodeRegs& d) { return (d.f[F_FLAGS] >> FL_LEADER_SHIFT) & 0xffu; }
 
   // ------------------------------------------------------------------------------------------
-  // pending-event queue, ordered by (time, 3-kind, stamp)  (simulator.rs:149-161)
-  //   QMODE 1/2: unsorted array, O(1) append, linear min-scan on pop (64-bit keys in HBM / 32-bit keys in smem)
-  //   QMODE 0  : binary min-heap with 3-word entries
+  // pending-event queue (Queue), ordered by (time, 3-kind, stamp)  (simulator.rs:149-161)
   // ------------------------------------------------------------------------------------------
-  LBFT_HD uint64_t heap_key_at(uint32_t i) const { return ((uint64_t)m.ld(L.heap_time + i) << 32) | m.ld(L.heap_key + i); }
-  LBFT_HD void heap_move(uint32_t dst, uint32_t src) const {
-    m.st(L.heap_time + dst, m.ld(L.heap_time + src));
-    m.st(L.heap_key + dst, m.ld(L.heap_key + src));
-    m.st(L.heap_data + dst, m.ld(L.heap_data + src));
-  }
   // schedule_event (simulator.rs:252-264).  Events beyond max_clock can never be popped before the
   // loop ends (:389-391): they consume their creation stamp and are dropped.  Returns true if queued.
   // `data` = receiver | sender << 8 | slot << 16.
-  static constexpr uint32_t kStampLimit = QMODE == 2 ? (1u << 16) : (QMODE == 1 ? (1u << 22) : (QMODE == 3 ? 0xfffffff0u : (1u << 30)));  // width of the stamp field of the queue's keys
   LBFT_HD bool push_event(int32_t time, uint32_t kind, uint32_t data) {
     uint32_t st = stamp++;
-    if (stamp >= kStampLimit) status |= ST_QUEUE_OVERFLOW;
+    if (stamp >= Queue::kStampLimit) status |= ST_QUEUE_OVERFLOW;
     if (time > P.max_clock) return false;
     if (qsize >= L.queue_cap) { status |= ST_QUEUE_OVERFLOW; return false; }
-    if (QMODE == 3) {
-      // calendar queue: one FIFO list per (time, kind).  Creation stamps grow with every push, so FIFO order inside
-      // a list IS stamp order, and the pop below takes kinds in priority order: exactly (time, kind desc, stamp).
-      uint32_t e;
-      if (cal_free != PAY_NONE) { e = cal_free; cal_free = m.ld(L.heap_time + e); }
-      else e = cal_next++;
-      m.st(L.heap_key + e, data);
-      const uint32_t t = (uint32_t)time, kw = t >> 3, sh = (t & 7) * 4 + kind, hw = L.cal_ht + t * 4 + kind;
-      uint32_t occ = km_ld(kw);
-      if ((occ >> sh) & 1) {
-        uint32_t ht = m.ld(hw);
-        m.st(L.heap_time + (ht >> 16), e);       // old tail -> e
-        m.st(hw, (ht & 0xffffu) | (e << 16));
-      } else {
-        m.st(hw, e | (e << 16));
-        km_st(kw, occ | (1u << sh));
-      }
-      qsize++;
-      if (qsize > max_queue) max_queue = qsize;
-      return true;
-    }
-    if (QMODE == 2) {
-      // stamps are unique, so a 32-bit key decides every comparison; the payload word is not compared
-      sk[qsize * QS] = ((uint32_t)time << 18) | ((3u - kind) << 16) | (st & 0xffffu);
-      sd[qsize * QS] = (uint16_t)((((data >> 16) & 0xffu) << 8) | (((data >> 8) & 0xfu) << 4) | (data & 0xfu));
-      qsize++;
-      if (qsize > max_queue) max_queue = qsize;
-      return true;
-    }
-    if (QMODE == 1) {
-      // key = time:24 | 3-kind:2 | stamp:22 | slot:8 | sender:4 | receiver:4; stamps are unique, so the
-      // payload bits below them never decide a comparison.
-      uint64_t key = ((uint64_t)(uint32_t)time << 40) | ((uint64_t)(3u - kind) << 38) | ((uint64_t)st << 16) |
-                     (uint64_t)(((data >> 16) & 0xffu) << 8) | (uint64_t)(((data >> 8) & 0xfu) << 4) | (uint64_t)(data & 0xfu);
-      m.at64(L.heap_time)[(size_t)qsize * S] = key;
-      qsize++;
-      if (qsize > max_queue) max_queue = qsize;
-      return true;
-    }
-    uint32_t klo = ((3u - kind) << 30) | st;
-    uint64_t key = ((uint64_t)(uint32_t)time << 32) | klo;
-    uint32_t i = qsize++;
+    q.put(m, L, qsize, time, kind, st, data);
+    qsize++;
     if (qsize > max_queue) max_queue = qsize;
-    while (i > 0) {
-      uint32_t p = (i - 1) >> 1;
-      if (heap_key_at(p) <= key) break;
-      heap_move(i, p);
-      i = p;
-    }
-    m.st(L.heap_time + i, (uint32_t)time);
-    m.st(L.heap_key + i, klo);
-    m.st(L.heap_data + i, data);
     return true;
   }
   LBFT_HD void pop_event(int32_t& time, uint32_t& kind, uint32_t& data) {
-    if (QMODE == 3) {
-      // advance to the first time slot with a pending list (pushes never go below the current slot)
-      uint32_t kw = cal_t >> 3;
-      uint32_t occ = km_ld(kw) >> ((cal_t & 7) * 4);
-      while (occ == 0) {
-        cal_t = (cal_t | 7) + 1;
-        kw++;
-        occ = km_ld(kw);
-      }
-      while ((occ & 15u) == 0) { occ >>= 4; cal_t++; }
-      const uint32_t nib = occ & 15u;
-      kind = nib & 8u ? 3u : (nib & 4u ? 2u : (nib & 2u ? 1u : 0u));  // Timer 3 > Response 2 > Request 1 > Notify 0
-      const uint32_t hw = L.cal_ht + cal_t * 4 + kind;
-      const uint32_t ht = m.ld(hw), e = ht & 0xffffu;
-      data = m.ld(L.heap_key + e);
-      if (e == (ht >> 16)) km_st(kw, km_ld(kw) & ~(1u << ((cal_t & 7) * 4 + kind)));  // list became empty
-      else m.st(hw, (ht & 0xffff0000u) | m.ld(L.heap_time + e));
-      m.st(L.heap_time + e, cal_free);
-      cal_free = e;
-      time = (int32_t)cal_t;
-      qsize--;
-      return;
-    }
-    if (QMODE == 2 && WIDE) {
-#if defined(__CUDA_ARCH__)
-      // the warp scans its one queue together: lane l looks at entries l, l + 32, ...; keys are unique (creation stamps)
-      __syncwarp(gm);  // entries pushed by this iteration's sends
-      const uint32_t n = qsize;
-      uint32_t best = 0xffffffffu, bi = 0;
-      for (uint32_t j = wl; j < n; j += G) {
-        const uint32_t k0 = sk[j];
-        if (k0 < best) { best = k0; bi = j; }
-      }
-      const uint32_t mn = __reduce_min_sync(gm, best);
-      const uint32_t src = (uint32_t)__ffs((int)__ballot_sync(gm, best == mn)) - 1u;  // a lane of this group (absolute index)
-      bi = __shfl_sync(gm, bi, (int)src);
-      const uint32_t lo = sd[bi];
-      qsize = n - 1;
-      __syncwarp(gm);  // everyone has read sd[bi] / its share of the keys
-      if (bi != n - 1) {
-        sk[bi] = sk[n - 1];
-        sd[bi] = sd[n - 1];
-      }
-      time = (int32_t)(mn >> 18);
-      kind = 3u - ((mn >> 16) & 3u);
-      const uint32_t slot = lo >> 8;
-      data = (lo & 0xfu) | (((lo >> 4) & 0xfu) << 8) | ((slot == 0xffu ? PAY_NONE : slot) << 16);
-#endif
-      return;
-    }
-    if (QMODE == 2) {
-      uint32_t best = sk[0], bi = 0;
-      const uint32_t n = qsize;
-      uint32_t j = 1;
-#pragma unroll 1
-      for (; j + 3 < n; j += 4) {
-        uint32_t k0 = sk[j * 32], k1 = sk[(j + 1) * 32], k2 = sk[(j + 2) * 32], k3 = sk[(j + 3) * 32];
-        if (k0 < best) { best = k0; bi = j; }
-        if (k1 < best) { best = k1; bi = j + 1; }
-        if (k2 < best) { best = k2; bi = j + 2; }
-        if (k3 < best) { best = k3; bi = j + 3; }
-      }
-#pragma unroll 1
-      for (; j < n; j++) {
-        uint32_t k0 = sk[j * 32];
-        if (k0 < best) { best = k0; bi = j; }
-      }
-      uint32_t lo = sd[bi * 32];
-      qsize = n - 1;
-      if (bi != n - 1) {
-        sk[bi * 32] = sk[(n - 1) * 32];
-        sd[bi * 32] = sd[(n - 1) * 32];
-      }
-      time = (int32_t)(best >> 18);
-      kind = 3u - ((best >> 16) & 3u);
-      uint32_t slot = lo >> 8;
-      data = (lo & 0xfu) | (((lo >> 4) & 0xfu) << 8) | ((slot == 0xffu ? PAY_NONE : slot) << 16);
-      return;
-    }
-    if (QMODE == 1 && WIDE) {
-#if defined(__CUDA_ARCH__)
-      __syncwarp(gm);
-      const uint64_t* q = m.at64(L.heap_time);
-      const uint32_t n = qsize;
-      uint64_t best = ~0ULL;
-      uint32_t bi = 0;
-      for (uint32_t j = wl; j < n; j += G) {
-        const uint64_t k0 = q[(size_t)j * S];
-        if (k0 < best) { best = k0; bi = j; }
-      }
-      // 64-bit minimum over the warp: high words first, then low words among the lanes that hold the minimal high word
-      const uint32_t hi = __reduce_min_sync(gm, (uint32_t)(best >> 32));
-      const uint32_t lo32 = __reduce_min_sync(gm, (uint32_t)(best >> 32) == hi ? (uint32_t)best : 0xffffffffu);
-      const uint64_t mn = ((uint64_t)hi << 32) | lo32;
-      const uint32_t src = (uint32_t)__ffs((int)__ballot_sync(gm, best == mn)) - 1u;
-      bi = __shfl_sync(gm, bi, (int)src);
-      qsize = n - 1;
-      uint64_t* qw = m.at64(L.heap_time);
-      const uint64_t last = qw[(size_t)(n - 1) * S];
-      __syncwarp(gm);
-      if (bi != n - 1) qw[(size_t)bi * S] = last;
-      time = (int32_t)(mn >> 40);
-      kind = 3u - ((uint32_t)(mn >> 38) & 3u);
-      const uint32_t lo = (uint32_t)mn & 0xffffu, slot = lo >> 8;
-      data = (lo & 0xfu) | (((lo >> 4) & 0xfu) << 8) | ((slot == 0xffu ? PAY_NONE : slot) << 16);
-#endif
-      return;
-    }
-    if (QMODE == 1) {
-      // linear min-scan: independent, fully coalesced loads; no data-dependent sift chains
-      const uint64_t* q = m.at64(L.heap_time);
-      uint64_t best = q[0];
-      uint32_t bi = 0;
-      const uint32_t n = qsize;
-      uint32_t j = 1;
-#pragma unroll 1
-      for (; j + 3 < n; j += 4) {
-        uint64_t k0 = q[(size_t)j * S], k1 = q[(size_t)(j + 1) * S], k2 = q[(size_t)(j + 2) * S], k3 = q[(size_t)(j + 3) * S];
-        if (k0 < best) { best = k0; bi = j; }
-        if (k1 < best) { best = k1; bi = j + 1; }
-        if (k2 < best) { best = k2; bi = j + 2; }
-        if (k3 < best) { best = k3; bi = j + 3; }
-      }
-#pragma unroll 1
-      for (; j < n; j++) {
-        uint64_t k0 = q[(size_t)j * S];
-        if (k0 < best) { best = k0; bi = j; }
-      }
-      qsize = n - 1;
-      uint64_t* qw = m.at64(L.heap_time);
-      if (bi != n - 1) qw[(size_t)bi * S] = qw[(size_t)(n - 1) * S];
-      time = (int32_t)(best >> 40);
-      kind = 3u - ((uint32_t)(best >> 38) & 3u);
-      uint32_t lo = (uint32_t)best & 0xffffu, slot = lo >> 8;
-      data = (lo & 0xfu) | (((lo >> 4) & 0xfu) << 8) | ((slot == 0xffu ? PAY_NONE : slot) << 16);
-      return;
-    }
-    time = (int32_t)m.ld(L.heap_time);
-    uint32_t klo = m.ld(L.heap_key);
-    data = m.ld(L.heap_data);
-    kind = 3u - (klo >> 30);
-    uint32_t n = --qsize;
-    if (n == 0) return;
-    uint32_t lt = m.ld(L.heap_time + n), lk = m.ld(L.heap_key + n), ld_ = m.ld(L.heap_data + n);
-    uint64_t key = ((uint64_t)lt << 32) | lk;
-    uint32_t i = 0;
-    for (;;) {
-      uint32_t c = 2 * i + 1;
-      if (c >= n) break;
-      uint64_t kc = heap_key_at(c);
-      if (c + 1 < n) {
-        uint64_t kr = heap_key_at(c + 1);
-        if (kr < kc) { kc = kr; c = c + 1; }
-      }
-      if (key <= kc) break;
-      heap_move(i, c);
-      i = c;
-    }
-    m.st(L.heap_time + i, lt);
-    m.st(L.heap_key + i, lk);
-    m.st(L.heap_data + i, ld_);
+    q.take(m, L, qsize, wl, gm, time, kind, data);
+    qsize--;
   }
 
   // notification payload pool (DataSyncNotification snapshots, shared by all receivers of one send)
@@ -931,9 +942,9 @@ struct Core {
     d.f[F_TOW] += P.c_weights[author];
     if (d.f[F_TOW] >= P.quorum) {
       d.tcmask = d.tmask;
-      grp_sync();  // the st_u16 above is read by another lane below
+      group_sync<G>(gm);  // the st_u16 above is read by another lane below
       for (uint32_t i = wl; i < L.hcbr_words; i += G) d.nb[(L.n_tchcbr + i) * S] = d.nb[(L.n_thcbr + i) * S];
-      grp_sync();
+      group_sync<G>(gm);
       d.f[F_TC_ROUND] = d.f[F_CUR];
       d.f[F_FLAGS] |= FL_HAS_TC;
       d.f[F_HTC] = d.f[F_CUR];
@@ -1186,7 +1197,7 @@ struct Core {
         for (uint32_t i = wl; i < L.hcbr_words; i += G) pb[(L.p_tchcbr + i) * S] = d.nb[(L.n_tchcbr + i) * S];
       if (d.tmask)
         for (uint32_t i = wl; i < L.hcbr_words; i += G) pb[(L.p_curhcbr + i) * S] = d.nb[(L.n_thcbr + i) * S];
-      grp_sync();
+      group_sync<G>(gm);
     }
   }
   // DataSyncNode::handle_notification (data_sync.rs:113-177).  Returns should_sync.
@@ -1341,7 +1352,7 @@ struct Core {
     if (ELIDE && !TDS && MAY_SILENT && P.silent_mask && kind != EV_RESPONSE &&
         ((P.silent_mask >> (kind == EV_NOTIFY ? receiver : sender)) & 1)) {
       stamp++;
-      if (stamp >= kStampLimit) status |= ST_QUEUE_OVERFLOW;
+      if (stamp >= Queue::kStampLimit) status |= ST_QUEUE_OVERFLOW;
       if (t <= P.max_clock) {
         if (kind == EV_NOTIFY) proc0++;
         else proc1++;
@@ -1382,20 +1393,18 @@ struct Core {
     proc0 = proc1 = proc2 = proc3 = cancelled = max_queue = sched_notify = dedup = 0;
     win = 0;
     cc0 = cc1 = cc2 = cc3 = 0;
-    cal_t = 0; cal_free = PAY_NONE; cal_next = 0;
     part_until = 0; part_open = 0;
     if (REC) {
       rs_pend = 0;
       for (uint32_t w = 0; w < N * (L.round_cap + 1); w++) m.st(rs_table_base(L) + w, 0);
     }
     // (table clears are split over the lanes of the group; G == 1: wl == 0, the plain loops)
-    if (QMODE == 3)
-      for (uint32_t w = wl; w < (L.cal_times + 7) / 8; w += G) km_st(w, 0);
+    q.clear(m, L, wl, km);
     for (uint32_t w = wl; w < N * L.node_words; w += G) m.st(L.node_base + w, 0);
     for (uint32_t w = wl; w < 2 * L.rset_words; w += G) m.st(L.created_base + w, 0);
     if (multi())
       for (uint32_t w = wl; w < L.epochs; w += G) m.st(L.einit_base + w, 0);
-    grp_sync();
+    group_sync<G>(gm);
     // EXTENSION D.3: partition plan from a separate stream; must match oracle_capi.cpp make_partition_plan
     if (L.part_windows) {
       uint64_t k0 = s0, k1 = s1, k2 = s2, k3 = s3;
@@ -1565,9 +1574,9 @@ struct Core {
         const bool staged = WIDE && list.len > 1 && (FIXED || (P.delay_kind == 0u && !P.delay_const && P.delay_kmax != 0));
         if (staged) {
           for (uint32_t i = 0; i < list.len; i++) ws->z[i] = standard_normal();
-          grp_sync();
+          group_sync<G>(gm);
           for (uint32_t i = wl; i < list.len; i += G) ws->dly[i] = (uint16_t)delay_from_z(ws->z[i]);
-          grp_sync();
+          group_sync<G>(gm);
         }
 #pragma unroll 1
         for (uint32_t i = 0; i < list.len; i++) {
@@ -1598,47 +1607,37 @@ struct Core {
   }
 
   // ------------------------------------------------------------------------------------------
-  // read-out: commit counts, last committed round and state key per node; counters; status
+  // Resumable runs: the per-instance registers and the queue's entries kept outside the instance state, between launches
   // ------------------------------------------------------------------------------------------
-  // ------------------------------------------------------------------------------------------
-  // Resumable runs: the per-instance registers (and, QMODE 2, the shared-memory queue) between two launches
-  // ------------------------------------------------------------------------------------------
+  // The registers in save-area order (a 64-bit register takes two words, low half first): save_regs and restore_regs both
+  // apply their `v` to each in turn.
+  template <class V>
+  LBFT_HD void walk_regs(V& v) {
+    v(s0); v(s1); v(s2); v(s3); v(draws); v(stamp); v(qsize); v(status); v(clock); v(pay_free); v(pay_next);
+    v(proc0); v(proc1); v(proc2); v(proc3); v(cancelled); v(max_queue); v(sched_notify); v(dedup); v(win);
+    q.walk_regs(v);
+    uint32_t no_rs = 0;  // (only recording runs have a pending round switch)
+    v(REC ? rs_pend : no_rs); v(cc0); v(cc1); v(cc2); v(cc3);
+  }
   LBFT_HD void save_regs() {
     const uint32_t b = res_area_base(L, REC);
     uint32_t w = b;
-    const uint64_t sx[4] = {s0, s1, s2, s3};
-    for (int i = 0; i < 4; i++) { m.st(w++, (uint32_t)sx[i]); m.st(w++, (uint32_t)(sx[i] >> 32)); }
-    const uint32_t r[] = {draws, stamp, qsize, status, (uint32_t)clock, pay_free, pay_next, proc0, proc1, proc2, proc3, cancelled,
-                          max_queue, sched_notify, dedup, win, cal_t, cal_free, cal_next, REC ? rs_pend : 0u, cc0, cc1, cc2, cc3};
-    static_assert(8 + sizeof(r) / 4 <= RES_REG_WORDS, "save area too small");
-    for (uint32_t i = 0; i < sizeof(r) / 4; i++) m.st(w++, r[i]);
-    if (QMODE == 2) {
-      const uint32_t q = b + RES_REG_WORDS + L.round_cap, qd = q + L.queue_cap;
-      for (uint32_t j = 0; j < qsize; j++) m.st(q + j, sk[j * 32]);
-      for (uint32_t j = 0; j < qsize; j += 2) m.st(qd + (j >> 1), (uint32_t)sd[j * 32] | (j + 1 < qsize ? (uint32_t)sd[(j + 1) * 32] << 16 : 0u));
-    }
+    auto save = [&](auto& r) { m.st(w++, (uint32_t)r); if (sizeof(r) == 8) m.st(w++, (uint32_t)((uint64_t)r >> 32)); };
+    walk_regs(save);
+    q.save(m, L, b + RES_REG_WORDS + L.round_cap, qsize);
   }
   LBFT_HD void restore_regs() {
     const uint32_t b = res_area_base(L, REC);
     uint32_t w = b;
     part_until = 0; part_open = 0;  // recomputed at the first send
-    uint64_t sx[4];
-    for (int i = 0; i < 4; i++) { uint64_t lo = m.ld(w++); uint64_t hi = m.ld(w++); sx[i] = lo | (hi << 32); }
-    s0 = sx[0]; s1 = sx[1]; s2 = sx[2]; s3 = sx[3];
-    draws = m.ld(w++); stamp = m.ld(w++); qsize = m.ld(w++); status = m.ld(w++); clock = (int32_t)m.ld(w++);
-    pay_free = m.ld(w++); pay_next = m.ld(w++); proc0 = m.ld(w++); proc1 = m.ld(w++); proc2 = m.ld(w++); proc3 = m.ld(w++);
-    cancelled = m.ld(w++); max_queue = m.ld(w++); sched_notify = m.ld(w++); dedup = m.ld(w++); win = m.ld(w++);
-    cal_t = m.ld(w++); cal_free = m.ld(w++); cal_next = m.ld(w++);
-    const uint32_t rp = m.ld(w++);
-    if (REC) rs_pend = rp;
-    cc0 = m.ld(w++); cc1 = m.ld(w++); cc2 = m.ld(w++); cc3 = m.ld(w++);
-    if (QMODE == 2) {
-      const uint32_t q = b + RES_REG_WORDS + L.round_cap, qd = q + L.queue_cap;
-      for (uint32_t j = 0; j < qsize; j++) {
-        sk[j * 32] = m.ld(q + j);
-        sd[j * 32] = (uint16_t)(m.ld(qd + (j >> 1)) >> ((j & 1) * 16));
-      }
-    }
+    auto restore = [&](auto& r) {
+      uint64_t v = m.ld(w++);
+      if (sizeof(r) == 8) v |= (uint64_t)m.ld(w++) << 32;
+      r = (typename std::remove_reference<decltype(r)>::type)v;
+    };
+    walk_regs(restore);
+    if (w - b > RES_REG_WORDS) status |= ST_INVARIANT;  // (w - b is a constant: folds away unless the list outgrew its words)
+    q.restore(m, L, b + RES_REG_WORDS + L.round_cap, qsize);
   }
 
   LBFT_HD void finalize(uint32_t inst) {
