@@ -47,6 +47,26 @@ pub mod ffi {
         pub reserved: u32,
     }
 
+    /// include/lbft.h `lbft_param_set`: one parameter set of a sweep handle (`lbft_create_sweep`) — the network delay
+    /// and `NodeConfig` of the instances assigned to it
+    #[repr(C)]
+    #[derive(Clone, Copy, Default, Debug, PartialEq)]
+    pub struct LbftParamSet {
+        pub delay_kind: u32,
+        pub reserved: u32,
+        pub delay_mean: f64,
+        pub delay_variance: f64,
+        pub delay_lo: i64,
+        pub delay_hi: i64,
+        pub target_commit_interval: i64,
+        pub delta: i64,
+        pub gamma: f64,
+        pub lambda: f64,
+    }
+    /// The header's spelling of `LbftParamSet`, as the `extern "C"` block names it.
+    #[allow(non_camel_case_types)]
+    pub type lbft_param_set = LbftParamSet;
+
     /// include/lbft.h `lbft_commit`: one row of `committed_history()`
     #[repr(C)]
     #[derive(Clone, Copy, Default, Debug, PartialEq)]
@@ -93,6 +113,8 @@ pub mod ffi {
         pub fn lbft_abi_version() -> u32;
         pub fn lbft_last_error() -> *const c_char;
         pub fn lbft_create(config: *const LbftConfig, out_sim: *mut *mut LbftSim) -> c_int;
+        pub fn lbft_create_sweep(config: *const LbftConfig, sets: *const lbft_param_set, num_sets: u32, set_of_instance: *const u32,
+                                 out_sim: *mut *mut LbftSim) -> c_int;
         pub fn lbft_destroy(sim: *mut LbftSim);
         pub fn lbft_set_seeds(sim: *mut LbftSim, seeds: *const u64) -> c_int;
         pub fn lbft_run(sim: *mut LbftSim) -> c_int;

@@ -145,6 +145,29 @@ typedef struct lbft_sim lbft_sim;
  * durations — all libm calls stay on the host), allocate device state.  Does not run anything. */
 int lbft_create(const lbft_config* config, lbft_sim** out_sim);
 
+/* The per-instance part of lbft_config for a parameter sweep: the network delay (main.rs --mean / --variance, or the
+ * uniform extension) and NodeConfig (--delta, --gamma, --lambda, --target_commit_interval). */
+typedef struct lbft_param_set {
+  uint32_t delay_kind;            /* LBFT_DELAY_*                                                      */
+  uint32_t reserved;              /* 0                                                                 */
+  double delay_mean, delay_variance;
+  int64_t delay_lo, delay_hi;
+  int64_t target_commit_interval, delta;
+  double gamma, lambda;
+} lbft_param_set;
+
+/* A sweep handle: one batch whose instances run under num_sets parameter sets — instance i under
+ * sets[set_of_instance[i]] — and share everything else of `config` (committee, voting rights, silent nodes, partition
+ * plan, commands_per_epoch, max_clock, capacities, device); the delay / NodeConfig fields of `config` are ignored.
+ * Every output of instance i is what lbft_create + lbft_run give it with that set's fields substituted into `config`
+ * (as long as neither run reports LBFT_ERR_CAPACITY: the sweep's layout is the one the set with the shortest mean delay
+ * would get).  Each set is validated like lbft_create validates those fields.  Refused (LBFT_ERR_INVALID, before any device
+ * work): num_sets == 0 or > min(num_instances, 65536), NULL sets / set_of_instance, an index >= num_sets, any flags bit,
+ * and commands_per_epoch < round_cap (sweeps are plain single-epoch runs).  Every other entry point works on the handle
+ * as on a plain one; lbft_set_seeds keeps the set assignment, and lbft_run_until / snapshots return LBFT_ERR_STATE. */
+int lbft_create_sweep(const lbft_config* config, const lbft_param_set* sets, uint32_t num_sets,
+                      const uint32_t* set_of_instance, lbft_sim** out_sim);
+
 /* Simulator::new for every instance followed by loop_until(max_clock) (simulator.rs:200-250,
  * 380-475): copies the seeds host->device, runs the event-loop kernel to completion, copies the
  * per-node summaries (commit counts, last-committed-state keys, counters, status) device->host.

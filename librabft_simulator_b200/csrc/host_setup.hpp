@@ -87,12 +87,17 @@ struct KernelSel {
   int qmode;   // Layout::queue_scan
   int fixed;   // FX_* (sim_params.h): the instantiation with that compile-time layout; FX_NONE = generic
   bool rec, res;
+  bool sweep;  // a sweep handle: lbft_sweep_event_loop_kernel / lbft_sweep_wide_kernel (per-instance parameter sets)
 };
 
 // The kernel's name, spelled like the symbol cuobjdump shows (lbft_kernel_info).
 inline std::string kernel_name(const KernelSel& k) {
   char buf[96];
-  if (k.wide)
+  if (k.sweep && k.wide)
+    snprintf(buf, sizeof buf, "lbft_sweep_wide_kernel<%d,%d,%s,%d>", k.nmax, k.qmode, k.smem ? "true" : "false", k.group);
+  else if (k.sweep)
+    snprintf(buf, sizeof buf, "lbft_sweep_event_loop_kernel<%d,%d,%d>", k.nmax, k.qmode, k.tile);
+  else if (k.wide)
     snprintf(buf, sizeof buf, "lbft_wide_kernel<%d,%d,%s,%d,%s,%d>", k.nmax, k.qmode, k.smem ? "true" : "false", k.group, k.epochs ? "true" : "false", k.fixed);
   else
     snprintf(buf, sizeof buf, "lbft_event_loop_kernel<%d,%d,%d,%s,%s,%s,%s,%d>", k.nmax, k.qmode, k.fixed, k.rec ? "true" : "false",
@@ -101,7 +106,7 @@ inline std::string kernel_name(const KernelSel& k) {
 }
 // Whether two selections name the same kernel (the fields kernel_name prints).
 constexpr bool same_kernel(const KernelSel& a, const KernelSel& b) {
-  return a.wide == b.wide && a.nmax == b.nmax && a.qmode == b.qmode && a.epochs == b.epochs && a.fixed == b.fixed &&
+  return a.sweep == b.sweep && a.wide == b.wide && a.nmax == b.nmax && a.qmode == b.qmode && a.epochs == b.epochs && a.fixed == b.fixed &&
          (a.wide ? a.smem == b.smem && a.group == b.group
                  : a.rec == b.rec && a.res == b.res && a.tds == b.tds && a.tile == b.tile);
 }
@@ -128,6 +133,8 @@ struct HostSetup {
   std::vector<int32_t> duration, period;
   std::vector<uint32_t> weights;
   std::vector<double> delay_thr;  // see build_delay_table()
+  std::vector<SweepSet> sets;     // sweep handles: one record per parameter set (build_sweep); empty otherwise
+  std::vector<uint32_t> set_of;   // sweep handles: [num_instances] the set of each instance
   std::string error;
   KernelSel sel{};
 
@@ -322,6 +329,78 @@ struct HostSetup {
     const int fx = fixed_shape_of(p);
     sel.fixed = (fx == FX_DEFAULT4 && !wide) || (fx == FX_PART7 && !wide && tile == 8) || (fx == FX_COMMITTEE64 && wide && sel.group == 8)
                     ? fx : FX_NONE;
+    return true;
+  }
+
+  // A sweep handle (lbft_create_sweep): `c` with each set's delay / NodeConfig fields substituted must be a valid plain
+  // configuration.  Layout and kernel are what build() picks for the set with the highest event rate (the shortest mean
+  // delay: the one the stamp-width and queue-mode tests are sized by), on the sweep kernels; per set, the delay model, the
+  // threshold table and the duration / period tables are built as build() builds them and concatenated.
+  bool build_sweep(const lbft_config& c, const lbft_param_set* ps, uint32_t num_sets, const uint32_t* set_of_instance) {
+    if (c.struct_size != sizeof(lbft_config)) return fail("lbft_config.struct_size does not match this library (ABI mismatch)");
+    if (!ps || !set_of_instance) return fail("sets and set_of_instance must not be NULL");
+    if (num_sets == 0 || num_sets > c.num_instances || num_sets > 65536u) return fail("num_sets must be in 1..min(num_instances, 65536)");
+    if (c.flags) return fail("sweep handles take no flags (recording, resumable and true data-sync runs are plain handles only)");
+    for (uint32_t i = 0; i < c.num_instances; i++)
+      if (set_of_instance[i] >= num_sets) return fail("set_of_instance has an index >= num_sets");
+    auto with_set = [&c](const lbft_param_set& q) {
+      lbft_config cs = c;
+      cs.delay_kind = q.delay_kind;
+      cs.delay_mean = q.delay_mean;
+      cs.delay_variance = q.delay_variance;
+      cs.delay_lo = q.delay_lo;
+      cs.delay_hi = q.delay_hi;
+      cs.target_commit_interval = q.target_commit_interval;
+      cs.delta = q.delta;
+      cs.gamma = q.gamma;
+      cs.lambda = q.lambda;
+      return cs;
+    };
+    const auto mean_delay = [](const lbft_param_set& q) {
+      return q.delay_kind == LBFT_DELAY_UNIFORM ? 0.5 * (double)(q.delay_lo + q.delay_hi) : q.delay_mean;
+    };
+    sets.resize(num_sets);
+    duration.clear();
+    period.clear();
+    std::vector<double> thr_all;
+    uint32_t fastest = 0;
+    for (uint32_t s = 0; s < num_sets; s++) {
+      HostSetup h;
+      if (!h.build(with_set(ps[s])) || ps[s].reserved) {
+        char buf[64];
+        snprintf(buf, sizeof buf, "parameter set %u: ", s);
+        return fail((buf + (ps[s].reserved ? std::string("reserved must be 0") : h.error)).c_str());
+      }
+      const Params& q = h.params;
+      SweepSet& w = sets[s];
+      w.delay_kind = q.delay_kind;
+      w.delay_const = q.delay_const;
+      w.delay_const_value = q.delay_const_value;
+      w.mu = q.mu;
+      w.sigma = q.sigma;
+      w.uni_lo = q.uni_lo;
+      w.uni_span = q.uni_span;
+      w.tci = q.tci;
+      w.delay_kmax = q.delay_kmax;
+      w.thr_off = (uint32_t)thr_all.size();
+      w.rt_off = (uint32_t)duration.size();
+      thr_all.insert(thr_all.end(), h.delay_thr.begin(), h.delay_thr.end());
+      duration.insert(duration.end(), h.duration.begin(), h.duration.end());
+      period.insert(period.end(), h.period.begin(), h.period.end());
+      if (mean_delay(ps[s]) < mean_delay(ps[fastest])) fastest = s;
+    }
+    std::vector<int32_t> dur_all, per_all;
+    dur_all.swap(duration);
+    per_all.swap(period);
+    if (!build(with_set(ps[fastest]))) return false;
+    if (c.commands_per_epoch < params.L.round_cap)
+      return fail("sweep handles need commands_per_epoch >= round_cap (single-epoch runs: epochs are plain handles only)");
+    duration.swap(dur_all);
+    period.swap(per_all);
+    delay_thr.swap(thr_all);
+    set_of.assign(set_of_instance, set_of_instance + c.num_instances);
+    sel.fixed = FX_NONE;
+    sel.sweep = true;
     return true;
   }
 

@@ -1,11 +1,13 @@
-// kernels.cuh — the two kernel templates over sim_core.cuh and the per-translation-unit launchers.
+// kernels.cuh — the two kernel templates over sim_core.cuh, their sweep twins and the per-translation-unit launchers.
 //
 //   lbft_event_loop_kernel<NMAX, QMODE, FIXED, REC, RES>   one THREAD per instance, 32 instances per warp tile (large batches)
 //   lbft_wide_kernel<NMAX, QMODE>                          one WARP per instance (small batches, large committees)
+//   lbft_sweep_event_loop_kernel / lbft_sweep_wide_kernel  the same bodies for sweep handles (lbft_create_sweep: per-instance
+//                                                          delay model and NodeConfig)
 //
-// Both do init -> event loop -> read-out in a single launch.  The instantiations are spread over several .cu files
-// (k_fixed.cu, k_scan.cu, k_calendar.cu, k_heap.cu, k_wide.cu) so that they compile in parallel and the bench kernel
-// can be rebuilt alone; lbft_api.cu only sees the launch_* functions declared at the end.
+// All do init -> event loop -> read-out in a single launch.  The instantiations are spread over several .cu files
+// (k_fixed.cu, k_scan.cu, k_calendar.cu, k_heap.cu, k_wide.cu, k_sweep_thread.cu, k_sweep_wide.cu) so that they compile in
+// parallel and the bench kernel can be rebuilt alone; lbft_api.cu only sees the launch_* functions declared at the end.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -34,22 +36,18 @@ struct LaunchShape {
 // each other's code paths, so a warp of 8 instances finishes far sooner than a warp of 32, and four times as many warps hide
 // each other's latency.  Plain kernels over the calendar queue and the shared-memory queue (whose columns keep their
 // 32-entry pitch); the state layout interleaves TILE instances.
-template <int NMAX, int QMODE, int FX = FX_NONE, bool REC = false, bool RES = false, bool EP = false, bool TDS = false, int TILE = 32>
-__global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMODE>::kBlocksPerSm) lbft_event_loop_kernel(const __grid_constant__ Params P) {
+// The body of both thread kernels (lbft_event_loop_kernel, lbft_sweep_event_loop_kernel), given the kernel's shared memory.
+// SW (sweep handles): the instance's parameter set supplies the delay model and NodeConfig; its thresholds are read through
+// L1 from the concatenated table, as the instances of one warp may belong to different sets.
+template <int NMAX, int QMODE, int FX, bool REC, bool RES, bool EP, bool TDS, int TILE, bool SW>
+__device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, double* s_zf, double* s_thr, uint32_t* s_queue,
+                                                const uint32_t* set_of, const SweepSet* sets) {
   static_assert(TILE == 32 || ((QMODE == 3 || QMODE == 2) && !REC && !RES && !EP && !TDS), "sparse tiles: plain kernels over the calendar / shared-memory queue");
-  // The ziggurat layers are indexed by a random byte per lane: a per-block shared-memory copy (4 KB) serves the 32
-  // scattered 8-byte reads of a warp in ~1-2 wavefronts; reading them through L1 from global memory instead makes the
-  // whole kernel markedly slower.
-  __shared__ double s_zx[257];
-  __shared__ double s_zf[257];
-  __shared__ double s_thr[kThrSmem];  // delay thresholds (same scattered access pattern), when they fit
-  extern __shared__ uint32_t s_queue[];  // QMODE 2: per warp [queue_cap][32] u32 keys, then [queue_cap][32] u16 payload words
-                                         // QMODE 3, sparse tiles: per warp [kmask words][TILE] calendar occupancy words
   for (int i = threadIdx.x; i < 257; i += blockDim.x) {
     s_zx[i] = P.zig_x[i];
     s_zf[i] = P.zig_f[i];
   }
-  const bool thr_fits = P.delay_kmax != 0 && P.delay_kmax + 2 <= kThrSmem;
+  const bool thr_fits = !SW && P.delay_kmax != 0 && P.delay_kmax + 2 <= kThrSmem;
   if (thr_fits)
     for (uint32_t i = threadIdx.x; i < P.delay_kmax + 2; i += blockDim.x) s_thr[i] = P.delay_thr[i];
   __syncthreads();
@@ -70,13 +68,36 @@ __global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMOD
   // sparse tiles over the calendar queue: the kind-occupancy words of the tile's instances in shared memory, a column per
   // lane (sim_core.cuh KS; the host only selects sparse tiles when 14 warps' worth fits, host_setup.hpp)
   constexpr bool KS = QMODE == 3 && TILE < 32;
-  Core<TileMem<TILE>, NMAX, QMODE, FX, REC, RES, 1, EP, TDS, KS> core(P, mem, s_zx, s_zf, thr_fits ? s_thr : P.delay_thr, sk, sd);
+  Core<TileMem<TILE>, NMAX, QMODE, FX, REC, RES, 1, EP, TDS, KS, SW> core(P, mem, s_zx, s_zf, thr_fits ? s_thr : P.delay_thr, sk, sd);
   if (KS) core.km = s_queue + (size_t)(threadIdx.x >> 5) * calendar_kmask_words(FX ? fixed_layout(FX) : P.L) * TILE + lane;
+  if constexpr (SW) core.bind_set(sets + set_of[inst]);
   if (RES && (P.run_flags & 1u)) core.restore_regs();  // a later lbft_run_until: continue where the last launch stopped
   else core.init(P.seeds[inst]);
   core.run();
   core.finalize(inst);
   if (RES) core.save_regs();
+}
+
+template <int NMAX, int QMODE, int FX = FX_NONE, bool REC = false, bool RES = false, bool EP = false, bool TDS = false, int TILE = 32>
+__global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMODE>::kBlocksPerSm) lbft_event_loop_kernel(const __grid_constant__ Params P) {
+  // The ziggurat layers are indexed by a random byte per lane: a per-block shared-memory copy (4 KB) serves the 32
+  // scattered 8-byte reads of a warp in ~1-2 wavefronts; reading them through L1 from global memory instead makes the
+  // whole kernel markedly slower.
+  __shared__ double s_zx[257];
+  __shared__ double s_zf[257];
+  __shared__ double s_thr[kThrSmem];  // delay thresholds (same scattered access pattern), when they fit
+  extern __shared__ uint32_t s_queue[];  // QMODE 2: per warp [queue_cap][32] u32 keys, then [queue_cap][32] u16 payload words
+                                         // QMODE 3, sparse tiles: per warp [kmask words][TILE] calendar occupancy words
+  event_loop_body<NMAX, QMODE, FX, REC, RES, EP, TDS, TILE, false>(P, s_zx, s_zf, s_thr, s_queue, nullptr, nullptr);
+}
+
+// A sweep handle's thread kernel (lbft_create_sweep): the generic plain kernel with per-instance parameter sets.
+template <int NMAX, int QMODE, int TILE = 32>
+__global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMODE>::kBlocksPerSm) lbft_sweep_event_loop_kernel(const __grid_constant__ SweepParams S) {
+  __shared__ double s_zx[257];
+  __shared__ double s_zf[257];
+  extern __shared__ uint32_t s_queue[];
+  event_loop_body<NMAX, QMODE, FX_NONE, false, false, false, false, TILE, true>(S.P, s_zx, s_zf, nullptr, s_queue, S.set_of, S.sets);
 }
 
 // ---- a group of G lanes per instance ("wide") ---------------------------------------------------------------------
@@ -102,9 +123,9 @@ LBFT_LAYOUT_FN uint32_t wide_smem_words_per_group(const Layout& L, int qmode, bo
 
 // SMEM: the instance's state words live in shared memory for the whole run; only the chain table (and the epoch table) is
 // copied to the instance's global extent at the end, for lbft_commit_log / lbft_commit_logs.
-template <int NMAX, int QMODE, bool SMEM, int G, bool EP = false, int FX = FX_NONE>
-__global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbft_wide_kernel(const __grid_constant__ Params P) {
-  extern __shared__ __align__(8) uint32_t s_wide[];
+// The body of both wide kernels (lbft_wide_kernel, lbft_sweep_wide_kernel).  SW: as event_loop_body.
+template <int NMAX, int QMODE, bool SMEM, int G, bool EP, int FX, bool SW>
+__device__ __forceinline__ void wide_body(const Params& P, uint32_t* s_wide, const uint32_t* set_of, const SweepSet* sets) {
   constexpr uint32_t kPerBlock = wide_warps(G) * 32 / G;
   const uint32_t grp = threadIdx.x / G, wl = threadIdx.x % G;
   const uint32_t inst = blockIdx.x * kPerBlock + grp;
@@ -117,10 +138,11 @@ __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbf
   uint32_t* gstate = P.state + (size_t)inst * KL.total_words;
   uint32_t* state = SMEM ? sk + wide_queue_words(KL.queue_cap, QMODE) : gstate;
   TileMem<1> mem{state, 0};
-  Core<TileMem<1>, NMAX, QMODE, FX, false, false, G, EP> core(P, mem, P.zig_x, P.zig_f, P.delay_thr, sk, sd);
+  Core<TileMem<1>, NMAX, QMODE, FX, false, false, G, EP, false, false, SW> core(P, mem, P.zig_x, P.zig_f, P.delay_thr, sk, sd);
   core.wl = wl;
   core.gm = G == 32 ? 0xffffffffu : (((1u << (G & 31)) - 1u) << ((threadIdx.x & 31u) & ~(uint32_t)(G - 1)));
   core.ws = ws;
+  if constexpr (SW) core.bind_set(sets + set_of[inst]);
   core.init(P.seeds[inst]);
   core.run();
   core.finalize(inst);
@@ -132,6 +154,19 @@ __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbf
   }
 }
 
+template <int NMAX, int QMODE, bool SMEM, int G, bool EP = false, int FX = FX_NONE>
+__global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbft_wide_kernel(const __grid_constant__ Params P) {
+  extern __shared__ __align__(8) uint32_t s_wide[];
+  wide_body<NMAX, QMODE, SMEM, G, EP, FX, false>(P, s_wide, nullptr, nullptr);
+}
+
+// A sweep handle's wide kernel (lbft_create_sweep).
+template <int NMAX, int QMODE, bool SMEM, int G>
+__global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbft_sweep_wide_kernel(const __grid_constant__ SweepParams S) {
+  extern __shared__ __align__(8) uint32_t s_wide[];
+  wide_body<NMAX, QMODE, SMEM, G, false, FX_NONE, true>(S.P, s_wide, S.set_of, S.sets);
+}
+
 // One per translation unit: launches the instantiation the selection names, or returns cudaErrorInvalidValue if the unit
 // has none (lbft_api.cu reports that with the kernel's name).
 cudaError_t launch_fixed(const KernelSel& k, const Params& P, cudaStream_t stream);
@@ -139,6 +174,8 @@ cudaError_t launch_scan(const KernelSel& k, const Params& P, cudaStream_t stream
 cudaError_t launch_calendar(const KernelSel& k, const Params& P, cudaStream_t stream);
 cudaError_t launch_heap(const KernelSel& k, const Params& P, cudaStream_t stream);
 cudaError_t launch_wide(const KernelSel& k, const Params& P, cudaStream_t stream);
+cudaError_t launch_sweep_thread(const KernelSel& k, const SweepParams& S, cudaStream_t stream);
+cudaError_t launch_sweep_wide(const KernelSel& k, const SweepParams& S, cudaStream_t stream);
 
 // Lets `kernel` take up to the device's opt-in limit of shared memory per block, beyond the 48 KB default (the QMODE 2
 // queues of four warps, the wide kernel's shared-memory instance state); `whole_carveout` also asks for the largest
@@ -158,56 +195,71 @@ inline cudaError_t allow_optin_smem(Kernel kernel, bool whole_carveout) {
   return e;
 }
 
+inline const Params& params_of(const Params& P) { return P; }
+inline const Params& params_of(const SweepParams& S) { return S.P; }
+
 // One instantiation of a kernel template: the selection that names it, and its launch.  try_launch launches it if `k` names
-// it and reports whether it did.
-template <int NMAX, int QM, int FX = FX_NONE, bool REC = false, bool RES = false, bool EP = false, bool TDS = false, int TILE = 32>
+// it and reports whether it did.  SW: the sweep twin of the generic plain instantiation (lbft_sweep_*_kernel).
+template <int NMAX, int QM, int FX = FX_NONE, bool REC = false, bool RES = false, bool EP = false, bool TDS = false, int TILE = 32,
+          bool SW = false>
 struct ThreadKernel {
-  static constexpr KernelSel sel{/*wide*/ false, /*smem*/ false, /*group*/ 0, EP, TDS, TILE, NMAX, QM, FX, REC, RES};
-  static bool try_launch(const KernelSel& k, const Params& P, cudaStream_t stream, cudaError_t& e) {
+  static_assert(!SW || (FX == FX_NONE && !REC && !RES && !EP && !TDS), "sweeps: plain single-epoch generic kernels only");
+  static constexpr KernelSel sel{/*wide*/ false, /*smem*/ false, /*group*/ 0, EP, TDS, TILE, NMAX, QM, FX, REC, RES, SW};
+  using KParams = typename std::conditional<SW, SweepParams, Params>::type;  // the kernel's parameter block
+  static bool try_launch(const KernelSel& k, const KParams& KP, cudaStream_t stream, cudaError_t& e) {
     if (!same_kernel(k, sel)) return false;
+    const Params& P = params_of(KP);
     constexpr int T = LaunchShape<QM>::kThreads;
     const uint32_t tiles = (P.num_instances + TILE - 1) / TILE, blocks = (tiles * 32 + T - 1) / T;
     // QMODE 2: per warp the queue keys and payload halves; sparse tiles over the calendar queue: per warp the occupancy
     // words of its instances (sim_core.cuh KS)
     const size_t dyn = QM == 2 ? (size_t)(T / 32) * P.L.queue_cap * (32 * 4 + 32 * 2)
                                : (QM == 3 && TILE < 32 ? (size_t)calendar_kmask_words(P.L) * TILE * sizeof(uint32_t) : 0);
-    auto kernel = lbft_event_loop_kernel<NMAX, QM, FX, REC, RES, EP, TDS, TILE>;
+    void (*kernel)(KParams);
+    if constexpr (SW) kernel = lbft_sweep_event_loop_kernel<NMAX, QM, TILE>;
+    else kernel = lbft_event_loop_kernel<NMAX, QM, FX, REC, RES, EP, TDS, TILE>;
     e = dyn > 0 ? allow_optin_smem(kernel, QM == 2) : cudaSuccess;
     if (e == cudaSuccess) {
-      kernel<<<blocks, T, dyn, stream>>>(P);
+      kernel<<<blocks, T, dyn, stream>>>(KP);
       e = cudaGetLastError();
     }
     return true;
   }
 };
-template <int NMAX, int QM, bool SMEM, int G, bool EP = false, int FX = FX_NONE>
+template <int NMAX, int QM, bool SMEM, int G, bool EP = false, int FX = FX_NONE, bool SW = false>
 struct WideKernel {
-  static constexpr KernelSel sel{/*wide*/ true, SMEM, G, EP, /*tds*/ false, /*tile*/ 1, NMAX, QM, FX, /*rec*/ false, /*res*/ false};
-  static bool try_launch(const KernelSel& k, const Params& P, cudaStream_t stream, cudaError_t& e) {
+  static_assert(!SW || (FX == FX_NONE && !EP), "sweeps: plain single-epoch generic kernels only");
+  static constexpr KernelSel sel{/*wide*/ true, SMEM, G, EP, /*tds*/ false, /*tile*/ 1, NMAX, QM, FX, /*rec*/ false, /*res*/ false, SW};
+  using KParams = typename std::conditional<SW, SweepParams, Params>::type;
+  static bool try_launch(const KernelSel& k, const KParams& KP, cudaStream_t stream, cudaError_t& e) {
     if (!same_kernel(k, sel)) return false;
+    const Params& P = params_of(KP);
     constexpr uint32_t kPerBlock = wide_warps(G) * 32 / G;
     const uint32_t blocks = (P.num_instances + kPerBlock - 1) / kPerBlock;
     const size_t dyn = (size_t)kPerBlock * wide_smem_words_per_group(P.L, QM, SMEM) * sizeof(uint32_t);
-    auto kernel = lbft_wide_kernel<NMAX, QM, SMEM, G, EP, FX>;
+    void (*kernel)(KParams);
+    if constexpr (SW) kernel = lbft_sweep_wide_kernel<NMAX, QM, SMEM, G>;
+    else kernel = lbft_wide_kernel<NMAX, QM, SMEM, G, EP, FX>;
     e = dyn > 48 * 1024 ? allow_optin_smem(kernel, false) : cudaSuccess;  // (the wide kernel has no static shared memory)
     if (e == cudaSuccess) {
-      kernel<<<blocks, wide_warps(G) * 32, dyn, stream>>>(P);
+      kernel<<<blocks, wide_warps(G) * 32, dyn, stream>>>(KP);
       e = cudaGetLastError();
     }
     return true;
   }
 };
-// A list of instantiations (or of lists).
+// A list of instantiations (or of lists) that take the same parameter block KP (Params, or SweepParams for sweep kernels).
 template <class... Ks>
 struct Kernels {
-  static bool try_launch(const KernelSel& k, const Params& P, cudaStream_t stream, cudaError_t& e) {
-    return (Ks::try_launch(k, P, stream, e) || ...);
+  template <class KP>
+  static bool try_launch(const KernelSel& k, const KP& kp, cudaStream_t stream, cudaError_t& e) {
+    return (Ks::try_launch(k, kp, stream, e) || ...);
   }
 };
-template <class List>
-inline cudaError_t launch_listed(const KernelSel& k, const Params& P, cudaStream_t stream) {
+template <class List, class KP>
+inline cudaError_t launch_listed(const KernelSel& k, const KP& kp, cudaStream_t stream) {
   cudaError_t e = cudaErrorInvalidValue;
-  List::try_launch(k, P, stream, e);
+  List::try_launch(k, kp, stream, e);
   return e;
 }
 
@@ -219,5 +271,11 @@ using ThreadVariants = Kernels<ThreadKernel<NMAX, QM>, ThreadKernel<NMAX, QM, FX
 // The lane groups and the epoch variant of a generic wide kernel with its state in HBM.
 template <int NMAX, int QM>
 using WideVariants = Kernels<WideKernel<NMAX, QM, false, 8>, WideKernel<NMAX, QM, false, 32>, WideKernel<NMAX, QM, false, 32, true>>;
+// The sweep twins of the plain generic instantiations: of a full-tile thread kernel, and of the two lane groups of a wide
+// kernel with its state in HBM.
+template <int NMAX, int QM>
+using SweepThread = ThreadKernel<NMAX, QM, FX_NONE, false, false, false, false, 32, true>;
+template <int NMAX, int QM>
+using SweepWideVariants = Kernels<WideKernel<NMAX, QM, false, 8, false, FX_NONE, true>, WideKernel<NMAX, QM, false, 32, false, FX_NONE, true>>;
 
 }  // namespace lbft

@@ -74,6 +74,8 @@ struct lbft_sim {
   int32_t* d_period = nullptr;
   uint32_t* d_weights = nullptr;
   double* d_delay_thr = nullptr;
+  SweepSet* d_sets = nullptr;    // sweep handles only
+  uint32_t* d_set_of = nullptr;  // sweep handles only
   uint32_t* d_state = nullptr;
   uint32_t* d_commit_counts = nullptr;
   uint32_t* d_lc_round = nullptr;
@@ -119,7 +121,7 @@ static void free_all(lbft_sim* s) {
   cudaFree(s->d_seeds); cudaFree(s->d_zx); cudaFree(s->d_zf); cudaFree(s->d_leader); cudaFree(s->d_duration);
   cudaFree(s->d_period); cudaFree(s->d_weights); cudaFree(s->d_delay_thr); cudaFree(s->d_state); cudaFree(s->d_summary);
   cudaFree(s->d_lc_round); cudaFree(s->d_counters); cudaFree(s->d_status);
-  cudaFree(s->d_error); cudaFree(s->d_logs);
+  cudaFree(s->d_error); cudaFree(s->d_logs); cudaFree(s->d_sets); cudaFree(s->d_set_of);
   for (int b = 0; b < 2; b++) {
     cudaFreeHost(s->h_seeds[b]);
     HostResults& r = s->res[b];
@@ -210,6 +212,8 @@ extern "C" {
 uint32_t lbft_abi_version(void) { return LBFT_ABI_VERSION; }
 const char* lbft_last_error(void) { return g_last_error.c_str(); }
 
+static int create_on_device(lbft_sim* s, const lbft_config* config, lbft_sim** out_sim);
+
 int lbft_create(const lbft_config* config, lbft_sim** out_sim) {
   if (!config || !out_sim) return set_error(LBFT_ERR_INVALID, "config and out_sim must not be NULL");
   *out_sim = nullptr;
@@ -225,6 +229,27 @@ int lbft_create(const lbft_config* config, lbft_sim** out_sim) {
     return set_error(LBFT_ERR_INVALID, "recording / resumable handles need commands_per_epoch >= round_cap: the kernels with the epoch "
                                        "machinery (node.rs:329-348) are built for plain runs only");
   }
+  return create_on_device(s, config, out_sim);
+}
+
+int lbft_create_sweep(const lbft_config* config, const lbft_param_set* sets, uint32_t num_sets, const uint32_t* set_of_instance,
+                      lbft_sim** out_sim) {
+  if (!config || !out_sim) return set_error(LBFT_ERR_INVALID, "config and out_sim must not be NULL");
+  *out_sim = nullptr;
+  lbft_sim* s = new (std::nothrow) lbft_sim();
+  if (!s) return set_error(LBFT_ERR_NOMEM, "out of host memory");
+  if (!s->hs.build_sweep(*config, sets, num_sets, set_of_instance)) {
+    std::string e = s->hs.error;
+    delete s;
+    return set_error(LBFT_ERR_INVALID, e);
+  }
+  return create_on_device(s, config, out_sim);
+}
+
+}  // extern "C"
+
+// The device half of lbft_create / lbft_create_sweep, once the host setup `s->hs` is built: takes ownership of `s`.
+static int create_on_device(lbft_sim* s, const lbft_config* config, lbft_sim** out_sim) {
   s->I = config->num_instances;
   s->N = config->num_nodes;
   s->device = config->device;
@@ -293,6 +318,12 @@ int lbft_create(const lbft_config* config, lbft_sim** out_sim) {
   CREATE_TRY(cudaMemcpy(s->d_weights, s->hs.weights.data(), N * sizeof(uint32_t), cudaMemcpyHostToDevice));
   if (s->d_delay_thr)
     CREATE_TRY(cudaMemcpy(s->d_delay_thr, s->hs.delay_thr.data(), s->hs.delay_thr.size() * sizeof(double), cudaMemcpyHostToDevice));
+  if (!s->hs.sets.empty()) {
+    CREATE_TRY(dev_alloc(s, &s->d_sets, s->hs.sets.size()));
+    CREATE_TRY(dev_alloc(s, &s->d_set_of, I));
+    CREATE_TRY(cudaMemcpy(s->d_sets, s->hs.sets.data(), s->hs.sets.size() * sizeof(SweepSet), cudaMemcpyHostToDevice));
+    CREATE_TRY(cudaMemcpy(s->d_set_of, s->hs.set_of.data(), I * sizeof(uint32_t), cudaMemcpyHostToDevice));
+  }
 #undef CREATE_TRY
   s->P = s->hs.params;
   s->P.seeds = s->d_seeds;
@@ -314,6 +345,8 @@ int lbft_create(const lbft_config* config, lbft_sim** out_sim) {
   *out_sim = s;
   return LBFT_OK;
 }
+
+extern "C" {
 
 int lbft_set_seeds(lbft_sim* s, const uint64_t* seeds) {
   if (!s || !seeds) return set_error(LBFT_ERR_INVALID, "NULL argument");
@@ -424,7 +457,9 @@ static int enqueue_kernel(lbft_sim* s) {
   CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
   CUDA_TRY(cudaEventRecord(s->ev[2], s->stream));
   const KernelSel& k = s->hs.sel;
-  cudaError_t e = k.wide ? launch_wide(k, s->P, s->stream)
+  const SweepParams sp{s->P, s->d_set_of, s->d_sets};
+  cudaError_t e = k.sweep ? (k.wide ? launch_sweep_wide(k, sp, s->stream) : launch_sweep_thread(k, sp, s->stream))
+                  : k.wide ? launch_wide(k, s->P, s->stream)
                   : k.fixed == FX_DEFAULT4 ? launch_fixed(k, s->P, s->stream)
                   : (k.qmode == 1 || k.qmode == 2) ? launch_scan(k, s->P, s->stream)
                   : k.qmode == 3 ? launch_calendar(k, s->P, s->stream)

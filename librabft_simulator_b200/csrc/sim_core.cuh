@@ -572,10 +572,13 @@ using QueueFor = typename std::conditional<QMODE == 0, HeapQueue<Mem, G>, typena
 // reference simulator's dispatch to the requester itself (simulator.rs:446, SURVEY fact 5).  An opt-in NON-PARITY
 // variant; plain thread-per-instance kernels only.
 // KS: (QMODE 3) the calendar's kind-occupancy words live in shared memory (CalendarQueue).
+// SW: a sweep handle (lbft_create_sweep) — the delay model and NodeConfig come from the instance's parameter set (bind_set)
+// instead of Params; every read of them goes through the accessors below.
 template <class Mem, int NMAX, int QMODE, int FX = 0, bool REC = false, bool RES = false, int G = 1, bool EP = false,
-          bool TDS = false, bool KS = false>
+          bool TDS = false, bool KS = false, bool SW = false>
 struct Core {
   static_assert(!KS || (QMODE == 3 && !RES && G == 1), "shared-memory occupancy words: calendar queue, one-shot thread kernels");
+  static_assert(!SW || (FX == FX_NONE && !REC && !RES && !EP && !TDS), "sweeps: plain single-epoch generic kernels only");
   static constexpr bool FIXED = FX != FX_NONE;                               // compile-time layout, reference delay model
   static constexpr bool MAY_SILENT = FX == FX_NONE || FX == FX_COMMITTEE64;  // silent nodes (extension D.2) reachable
   static_assert(!(FIXED && EP), "the compile-time layout is single-epoch");
@@ -597,7 +600,8 @@ struct Core {
   Mem m;
   const double* zx;
   const double* zf;
-  const double* thr;  // delay thresholds (shared-memory copy on the device when it fits)
+  const double* thr;  // delay thresholds (shared-memory copy on the device when it fits; SW: the instance's set's, bind_set)
+  const SweepSet* sw = nullptr;  // SW: the instance's parameter set
   using Queue = QueueFor<QMODE, Mem, G, KS>;
   Queue q;                 // given its shared memory by the constructor (QMODE 2: sk / sd, or the host harness's stand-in) and init (km)
   uint32_t* km = nullptr;  // KS: the calendar's occupancy words in shared memory, a column per lane, set by the kernel
@@ -619,6 +623,26 @@ struct Core {
   LBFT_HD Core(const Params& p, Mem mem, const double* zx_, const double* zf_, const double* thr_, uint32_t* sk = nullptr,
                uint16_t* sd = nullptr)
       : P(p), L(FIXED ? fixed_layout(FX) : p.L), m(mem), zx(zx_), zf(zf_), thr(thr_) { q.attach(sk, sd); }
+
+  // ------------------------------------------------------------------------------------------
+  // the swept settings: the launch's (Params) on a plain handle, the instance's parameter set on a sweep handle
+  // ------------------------------------------------------------------------------------------
+  // SW: binds the instance to its parameter set (SweepParams::sets[set_of[inst]]); before init.
+  LBFT_HD void bind_set(const SweepSet* set) {
+    sw = set;
+    thr = P.delay_thr + set->thr_off;
+  }
+  LBFT_HD uint32_t delay_kind() const { if constexpr (SW) return sw->delay_kind; else return P.delay_kind; }
+  LBFT_HD uint32_t delay_const() const { if constexpr (SW) return sw->delay_const; else return P.delay_const; }
+  LBFT_HD int64_t delay_const_value() const { if constexpr (SW) return sw->delay_const_value; else return P.delay_const_value; }
+  LBFT_HD double mu() const { if constexpr (SW) return sw->mu; else return P.mu; }
+  LBFT_HD double sigma() const { if constexpr (SW) return sw->sigma; else return P.sigma; }
+  LBFT_HD uint64_t uni_lo() const { if constexpr (SW) return sw->uni_lo; else return P.uni_lo; }
+  LBFT_HD uint64_t uni_span() const { if constexpr (SW) return sw->uni_span; else return P.uni_span; }
+  LBFT_HD uint32_t delay_kmax() const { if constexpr (SW) return sw->delay_kmax; else return P.delay_kmax; }
+  LBFT_HD int32_t tci() const { if constexpr (SW) return sw->tci; else return P.tci; }
+  LBFT_HD int32_t duration(uint32_t n) const { if constexpr (SW) return P.duration[sw->rt_off + n]; else return P.duration[n]; }
+  LBFT_HD int32_t period(uint32_t n) const { if constexpr (SW) return P.period[sw->rt_off + n]; else return P.period[n]; }
 
   // ------------------------------------------------------------------------------------------
   // RNG (rand_xoshiro 0.6.0 / rand 0.8.3 / rand_distr 0.4.0)
@@ -672,8 +696,8 @@ struct Core {
   // (exp(mu + sigma*z) as i64) == number of thresholds <= z; the thresholds were bisected on the host
   // with the host libm, so this is exact.  Any starting guess works; the walk fixes it up.
   LBFT_HD int32_t delay_from_z(double z) const {
-    float g = expf((float)P.mu + (float)P.sigma * (float)z);
-    int32_t k = g < (float)P.delay_kmax ? (int32_t)g : (int32_t)P.delay_kmax;
+    float g = expf((float)mu() + (float)sigma() * (float)z);
+    int32_t k = g < (float)delay_kmax() ? (int32_t)g : (int32_t)delay_kmax();
     if (k < 0) k = 0;
     while (z >= thr[k + 1]) k++;
     while (z < thr[k]) k--;
@@ -681,11 +705,11 @@ struct Core {
   }
   // GlobalTime::add_delay (simulator.rs:110-118): returns the delay in ms.
   LBFT_HD int32_t sample_delay() {
-    if (!FIXED && P.delay_kind == 1u) return (int32_t)(P.uni_lo + gen_range_u64(P.uni_span));
+    if (!FIXED && delay_kind() == 1u) return (int32_t)(uni_lo() + gen_range_u64(uni_span()));
     double z = standard_normal();
-    if (!FIXED && P.delay_const) return (int32_t)P.delay_const_value;  // sigma == 0: exp(mu) evaluated by the host libm
-    if (FIXED || P.delay_kmax) return delay_from_z(z);
-    int64_t r = delay_via_exp(P.mu, P.sigma, z);
+    if (!FIXED && delay_const()) return (int32_t)delay_const_value();  // sigma == 0: exp(mu) evaluated by the host libm
+    if (FIXED || delay_kmax()) return delay_from_z(z);
+    int64_t r = delay_via_exp(mu(), sigma(), z);
     if (r & (1LL << 62)) status |= ST_DELAY_NEAR_INT;
     if (r & (1LL << 61)) status |= ST_TIME_OVERFLOW;
     return (int32_t)(r & 0x7fffffff);
@@ -1062,8 +1086,8 @@ struct Core {
       d.f[F_FLAGS] = (d.f[F_FLAGS] & ~(0xffu << FL_LEADER_SHIFT)) | (ld << FL_LEADER_SHIFT);
       uint32_t base = d.f[F_HCR] > 0 ? d.f[F_HCR] + 2 : 0;  // duration(), :111-124
       if (!(active > base)) { status |= ST_INVARIANT; base = active - 1; }
-      d.f[F_PM_DUR] = (uint32_t)P.duration[active - base];
-      d.f[F_PM_PERIOD] = (uint32_t)P.period[active - base];
+      d.f[F_PM_DUR] = (uint32_t)duration(active - base);
+      d.f[F_PM_PERIOD] = (uint32_t)period(active - base);
       if (ld != n) a.send_to = (int32_t)ld;
     }
     const uint32_t leader = leader_of(d);
@@ -1140,10 +1164,10 @@ struct Core {
       d.f[F_TRK_TIME] = (uint32_t)clk;
     }
     int32_t tl = (int32_t)d.f[F_TRK_TIME] > (int32_t)d.f[F_LQA] ? (int32_t)d.f[F_TRK_TIME] : (int32_t)d.f[F_LQA];
-    int32_t deadline = tl + P.tci;
+    int32_t deadline = tl + tci();
     if (clk >= deadline) {
       a.query_all = true;
-      deadline = clk + P.tci;
+      deadline = clk + tci();
     }
     if (deadline < a.next) a.next = deadline;
     if (a.query_all) d.f[F_LQA] = (uint32_t)clk;
@@ -1571,7 +1595,7 @@ struct Core {
         // Wide kernel, table-served LogNormal delay: the normal deviates of the fan-out are drawn first (the RNG stream is
         // sequential), then each lane turns its share of them into delays, then the events are queued in list order.
         // Nothing else draws from the stream or takes a creation stamp in between, so the order of both is unchanged.
-        const bool staged = WIDE && list.len > 1 && (FIXED || (P.delay_kind == 0u && !P.delay_const && P.delay_kmax != 0));
+        const bool staged = WIDE && list.len > 1 && (FIXED || (delay_kind() == 0u && !delay_const() && delay_kmax() != 0));
         if (staged) {
           for (uint32_t i = 0; i < list.len; i++) ws->z[i] = standard_normal();
           group_sync<G>(gm);

@@ -185,6 +185,19 @@ LBFT_LAYOUT_FN uint32_t res_area_base(const Layout& L, bool record_rs) {
   return rs_table_base(L) + (record_rs ? L.num_nodes * (L.round_cap + 1) : 0);
 }
 
+// One parameter set of a sweep handle (lbft_create_sweep): the delay model and NodeConfig of the instances assigned to it,
+// evaluated on the host like the launch-uniform fields of Params, and where its tables start in the concatenated arrays.
+struct SweepSet {
+  uint32_t delay_kind, delay_const;
+  int64_t delay_const_value;
+  double mu, sigma;
+  uint64_t uni_lo, uni_span;
+  int32_t tci;
+  uint32_t delay_kmax;
+  uint32_t thr_off;  // its delay thresholds start at Params::delay_thr[thr_off]
+  uint32_t rt_off;   // its duration / period tables start at Params::duration[rt_off] / period[rt_off]
+};
+
 // Everything the kernel needs that is uniform over the launch.
 struct Params {
   Layout L;
@@ -233,6 +246,15 @@ struct Params {
   uint32_t* out_rounds;  // [I] max over nodes of the pacemaker's active round = counters[6] (the unit of the throughput metric)
   uint32_t* out_error;   // [1] OR of the status words of every instance that ended with an error bit: the host looks at one
                          //     word instead of scanning I statuses
+};
+
+// The parameter block of a sweep handle's kernels (lbft_create_sweep): instance i runs with sets[set_of[i]], and
+// P.delay_thr / P.duration / P.period are the concatenated tables of all sets.  (A block of its own rather than fields
+// appended to Params, so that no other kernel's parameters move.)
+struct SweepParams {
+  Params P;
+  const uint32_t* set_of;  // [num_instances]
+  const SweepSet* sets;    // [num_sets]
 };
 
 }  // namespace lbft

@@ -401,6 +401,57 @@ class BatchSimulator:
         write_data_files(path, self.num_nodes, self.round_switches(instance), int(counters[0]) + int(counters[1]) + int(counters[2]))
 
 
+@dataclass(frozen=True)
+class ParamSet:
+    """One point of a parameter sweep: the network delay and ``NodeConfig`` of the instances assigned to it
+    (main.rs --mean / --variance and --delta / --gamma / --lambda / --target_commit_interval)."""
+    network_delay: RandomDelay = RandomDelay()
+    node_config: NodeConfig = NodeConfig()
+
+    def to_c(self):
+        d, n = self.network_delay, self.node_config
+        return _lib.LbftParamSet(delay_kind=d.kind, reserved=0, delay_mean=d.mean, delay_variance=d.variance, delay_lo=d.lo,
+                                 delay_hi=d.hi, target_commit_interval=n.target_commit_interval, delta=n.delta, gamma=n.gamma,
+                                 lambda_=n.lambda_)
+
+
+class SweepSimulator(BatchSimulator):
+    """A parameter sweep as ONE batch (``lbft_create_sweep``): instance i runs ``Simulator::new(seeds[i], ..)`` under
+    ``param_sets[set_of_instance[i]]``; everything else (committee, voting rights, silent nodes, partitions,
+    ``commands_per_epoch``, capacities, device) is shared and passed as for ``BatchSimulator``.  Every result of instance i
+    is what a ``BatchSimulator`` with that set's delay and node config computes for it.  Running, re-seeding (the set
+    assignment stays), streaming and reading results work as on a ``BatchSimulator``."""
+
+    def __init__(self, seeds, num_nodes, param_sets, set_of_instance, **shared):
+        super().__init__(seeds, num_nodes, **shared)
+        self.param_sets = list(param_sets)
+        self.set_of_instance = np.ascontiguousarray(np.asarray(set_of_instance, dtype=np.uint32).reshape(-1))
+        if self.set_of_instance.shape[0] != self.num_instances:
+            raise ValueError("set_of_instance needs one entry per seed (%d)" % self.num_instances)
+
+    @classmethod
+    def grid(cls, seeds_per_point, delays, node_configs, num_nodes=4, **shared):
+        """The Cartesian product ``delays x node_configs`` (point p = i * len(node_configs) + j), each point run over the
+        same seeds (``seeds_per_point``: a sequence of seeds, or a count k for seeds 0..k-1) in a contiguous block of
+        instances: point p holds instances [p * k, (p + 1) * k).  ``set_of_instance`` and ``param_sets`` say which is which."""
+        seeds = np.arange(seeds_per_point, dtype=np.uint64) if np.isscalar(seeds_per_point) else \
+            np.asarray(seeds_per_point, dtype=np.uint64).reshape(-1)
+        sets = [ParamSet(d, n) for d in delays for n in node_configs]
+        k = seeds.shape[0]
+        return cls(np.tile(seeds, len(sets)), num_nodes, sets, np.repeat(np.arange(len(sets), dtype=np.uint32), k), **shared)
+
+    def create(self, max_clock):
+        """``lbft_create_sweep``: validate every set, build the per-set host tables, allocate device state."""
+        self.close()
+        handle = ctypes.c_void_p()
+        cfg = self.make_config(max_clock)
+        sets = (_lib.LbftParamSet * max(1, len(self.param_sets)))(*[p.to_c() for p in self.param_sets])
+        _lib.check(self._lib.lbft_create_sweep(ctypes.byref(cfg), sets, len(self.param_sets),
+                                               ctypes.c_void_p(self.set_of_instance.ctypes.data), ctypes.byref(handle)))
+        self._handle = handle
+        return self
+
+
 def format_round_switches_csv(num_nodes, switches):
     """Text of ``round_switches.txt`` (data_writer.rs:61-86) from ``[(node, round, time)]``.
 
