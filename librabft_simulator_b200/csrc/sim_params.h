@@ -169,7 +169,8 @@ LBFT_LAYOUT_FN Layout make_layout(uint32_t N, uint32_t round_cap, uint32_t queue
 // into an immediate and the extension branches the shape cannot reach are compiled out.  The host selects one only when the
 // handle's layout is bit-identical to the constant and the delay model is the reference's (LogNormal served by the
 // threshold table); every other handle runs the generic instantiations.
-//   FX_DEFAULT4     four authors, default capacities, shared-memory queue (BASELINE configs 1-3), thread kernel
+//   FX_DEFAULT4     four authors, default capacities, shared-memory queue (BASELINE configs 1-3), thread kernel; node blocks and
+//                   payload slots hold their state in the compact encoding of sim_core.cuh (Core::PACK) inside this layout
 //   FX_PART7        seven authors, four partition windows, max_clock 1000, calendar queue (BASELINE configs[4]), thread
 //                   kernel with 8-instance warp tiles
 //   FX_COMMITTEE64  64 authors, max_clock 1000, calendar queue (BASELINE configs[3]; voting rights and silent nodes stay
