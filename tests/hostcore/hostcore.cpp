@@ -61,7 +61,37 @@ static void run_all_fx(const Params& P, std::vector<uint32_t>& state, const doub
 }
 static int run_impl(const lbft_config* c, uint32_t* commit_counts, uint64_t* last_states, uint32_t* lc_round,
                     uint32_t* counters, uint32_t* status, uint32_t* words_per_instance, std::vector<uint32_t>& state,
-                    Params& P, const int64_t* stops = nullptr, size_t nstops = 0);
+                    Params& P, const int64_t* stops = nullptr, size_t nstops = 0, bool generic = false);
+
+// The FX_DEFAULT4 instantiation (the compact node / slot encoding, Core::PACK) as run_all_fx runs it, and the generic one
+// that the same layout takes without its compile-time shape (run_all_ep<16, 2, false, false, false>).
+using PackedCore = Core<TileMem<32>, 16, 2, FX_DEFAULT4, false, false, 1, false, false, false>;
+using GenericCore = Core<TileMem<32>, 16, 2, FX_NONE, false, false, 1, false, false, false>;
+static_assert(PackedCore::PACK && !GenericCore::PACK, "the two encodings of the four-author layout");
+
+// Words per (instance, node) of hostcore_final_state's decoded output: the F_NSCALAR scalars, vmask, tmask, tcmask, the
+// timeout hcbr of authors 0..3 and the TC hcbr of authors 0..3.
+constexpr uint32_t kDecodedWords = F_NSCALAR + 3 + 4 + 4;
+
+// Node n of the instance in `mem`, read back through C's own accessors: node_ld for the scalars, load_node for the masks,
+// hcbr_of on the node's timeout / TC hcbr vectors.  An hcbr entry is reported only for the authors of tmask / tcmask (0
+// otherwise): the other entries are left over from earlier rounds by design and nothing reads them.
+template <class C>
+static void decode_node(C& core, uint32_t n, uint32_t* out) {
+  const uint32_t b = core.nbase(n);
+  for (uint32_t f = 0; f < F_NSCALAR; f++) out[f] = core.node_ld(b, f);
+  typename C::NodeRegs d;
+  core.win = 0;  // (the bitset word load_node speculates on: any valid index)
+  core.load_node(n, d);
+  out[F_NSCALAR] = (uint32_t)d.vmask;
+  out[F_NSCALAR + 1] = (uint32_t)d.tmask;
+  out[F_NSCALAR + 2] = (uint32_t)d.tcmask;
+  const uint32_t th = C::PACK ? C::kPackedTimeoutHcbr : core.L.n_thcbr, tch = C::PACK ? C::kPackedTcHcbr : core.L.n_tchcbr;
+  for (uint32_t a = 0; a < 4; a++) {
+    out[F_NSCALAR + 3 + a] = ((d.tmask >> a) & 1) ? C::hcbr_of(core.m.at(b + th), a) : 0u;
+    out[F_NSCALAR + 7 + a] = ((d.tcmask >> a) & 1) ? C::hcbr_of(core.m.at(b + tch), a) : 0u;
+  }
+}
 
 static size_t read_round_switches(const Layout& L, const std::vector<uint32_t>& state, uint32_t num_nodes, uint32_t instance,
                                   lbft_round_switch* out, size_t cap) {
@@ -154,11 +184,103 @@ int hostcore_round_switches_staged(const lbft_config* c, uint32_t instance, cons
   if (n) *n = read_round_switches(P.L, state, c->num_nodes, instance, out, cap);
   return LBFT_OK;
 }
+
+// The compact encoding of FX_DEFAULT4 (sim_core.cuh Core::PACK) as the core defines it: [0] F_NSCALAR, [1] kPackedScalarWords,
+// [2] kPackedWords, [3] kPackedTimeoutHcbr, [4] kPackedTcHcbr; then word, shift, mask of packed_field(f) for f = 0 ..
+// F_NSCALAR + 2 (the scalars, then the vote / timeout / TC author masks); then the layout's node_base, node_words, n_hasblk,
+// rset_words, created_base, qcmade_base, chain_base, round_cap, pay_base, pay_words, payload_cap, total_words.  Returns the
+// number of words written, or -1 if `cap` is too small.
+int hostcore_packed_fields(uint32_t* out, size_t cap) {
+  constexpr Layout L = fixed_layout(FX_DEFAULT4);
+  const uint32_t head[] = {F_NSCALAR, PackedCore::kPackedScalarWords, PackedCore::kPackedWords, PackedCore::kPackedTimeoutHcbr,
+                           PackedCore::kPackedTcHcbr};
+  const uint32_t tail[] = {L.node_base, L.node_words, L.n_hasblk, L.rset_words, L.created_base, L.qcmade_base, L.chain_base,
+                           L.round_cap, L.pay_base, L.pay_words, L.payload_cap, L.total_words};
+  const size_t need = 5 + 3 * (F_NSCALAR + 3) + 12;
+  if (!out || cap < need) { g_err = "output too small"; return -1; }
+  size_t k = 0;
+  for (uint32_t v : head) out[k++] = v;
+  for (uint32_t f = 0; f < F_NSCALAR + 3; f++) {
+    const auto pf = PackedCore::packed_field(f);
+    out[k++] = pf.word;
+    out[k++] = pf.shift;
+    out[k++] = pf.mask;
+  }
+  for (uint32_t v : tail) out[k++] = v;
+  return (int)k;
+}
+
+// One node block through the compact encoding's writers and readers, in a tile of fixed_layout(FX_DEFAULT4).total_words x 32
+// words that the caller has filled (`tile`, updated in place).  vals: the F_NSCALAR scalars, vmask, tmask, tcmask, the
+// timeout hcbr of authors 0..3, the TC hcbr of authors 0..3.  Node `node` of lane `lane` is loaded (which leaves the bitset
+// words clean), given the scalars and masks and stored; the TC hcbr goes in through put_timeout_hcbr and
+// copy_timeout_hcbr_to_tc, then the timeout hcbr through put_timeout_hcbr.  out: the scalars and masks as load_node reads
+// them back, the same through node_ld, the timeout hcbr and the TC hcbr through hcbr_of (62 words).
+int hostcore_packed_roundtrip(const uint32_t* vals, uint32_t node, uint32_t lane, uint32_t* tile, uint32_t* out) {
+  if (!vals || !tile || !out) { g_err = "NULL argument"; return LBFT_ERR_INVALID; }
+  if (node >= 4 || lane >= 32) { g_err = "node or lane out of range"; return LBFT_ERR_INVALID; }
+  const Params P{};
+  PackedCore core(P, TileMem<32>{tile, lane}, nullptr, nullptr, nullptr);
+  PackedCore::NodeRegs d;
+  core.win = 0;  // (the bitset word load_node speculates on: any valid index)
+  core.load_node(node, d);
+  for (uint32_t f = 0; f < F_NSCALAR; f++) d.f[f] = vals[f];
+  d.vmask = vals[F_NSCALAR];
+  d.tmask = vals[F_NSCALAR + 1];
+  d.tcmask = vals[F_NSCALAR + 2];
+  core.store_node(d);
+  for (uint32_t a = 0; a < 4; a++) core.put_timeout_hcbr(d, a, vals[F_NSCALAR + 7 + a]);
+  core.copy_timeout_hcbr_to_tc(d);
+  for (uint32_t a = 0; a < 4; a++) core.put_timeout_hcbr(d, a, vals[F_NSCALAR + 3 + a]);
+  PackedCore::NodeRegs e;
+  core.load_node(node, e);
+  uint32_t k = 0;
+  for (uint32_t f = 0; f < F_NSCALAR; f++) out[k++] = e.f[f];
+  out[k++] = e.vmask;
+  out[k++] = e.tmask;
+  out[k++] = e.tcmask;
+  const uint32_t b = core.nbase(node);
+  for (uint32_t f = 0; f < F_NSCALAR + 3; f++) out[k++] = core.node_ld(b, f);
+  for (uint32_t a = 0; a < 4; a++) out[k++] = PackedCore::hcbr_of(core.m.at(b + PackedCore::kPackedTimeoutHcbr), a);
+  for (uint32_t a = 0; a < 4; a++) out[k++] = PackedCore::hcbr_of(core.m.at(b + PackedCore::kPackedTcHcbr), a);
+  return LBFT_OK;
+}
+
+// A configuration of the FX_DEFAULT4 layout run through the compact-encoding instantiation (generic == 0) or the generic one
+// on the same layout (generic == 1), in a state buffer filled with 0xdeadbeef.  The outputs are hostcore_run's; `decoded`
+// (optional) receives kDecodedWords words per (instance, node) as decode_node reads them, and `raw` (optional) the state
+// buffer: ceil(num_instances / 32) warp tiles of total_words x 32 words.
+int hostcore_final_state(const lbft_config* c, int generic, uint32_t* commit_counts, uint64_t* last_states, uint32_t* lc_round,
+                         uint32_t* counters, uint32_t* status, uint32_t* decoded, uint32_t* raw) {
+  HostSetup hs;
+  if (!hs.build(*c)) { g_err = hs.error; return LBFT_ERR_INVALID; }
+  if (fixed_shape_of(hs.params) != FX_DEFAULT4) { g_err = "not the FX_DEFAULT4 layout"; return LBFT_ERR_INVALID; }
+  if (!generic && getenv("HOSTCORE_NO_FIXED")) { g_err = "HOSTCORE_NO_FIXED is set: no compact-encoding run"; return LBFT_ERR_STATE; }
+  std::vector<uint32_t> state;
+  Params P;
+  int rc = run_impl(c, commit_counts, last_states, lc_round, counters, status, nullptr, state, P, nullptr, 0, generic != 0);
+  if (rc != LBFT_OK) return rc;
+  for (uint32_t inst = 0; decoded && inst < c->num_instances; inst++) {
+    const TileMem<32> mem{state.data() + (size_t)(inst / 32) * P.L.total_words * 32, inst % 32};
+    for (uint32_t n = 0; n < 4; n++) {
+      uint32_t* o = decoded + ((size_t)inst * 4 + n) * kDecodedWords;
+      if (generic) {
+        GenericCore core(P, mem, nullptr, nullptr, nullptr);
+        decode_node(core, n, o);
+      } else {
+        PackedCore core(P, mem, nullptr, nullptr, nullptr);
+        decode_node(core, n, o);
+      }
+    }
+  }
+  if (raw) memcpy(raw, state.data(), state.size() * sizeof(uint32_t));
+  return LBFT_OK;
+}
 }  // extern "C"
 
 static int run_impl(const lbft_config* c, uint32_t* commit_counts, uint64_t* last_states, uint32_t* lc_round,
                     uint32_t* counters, uint32_t* status, uint32_t* words_per_instance, std::vector<uint32_t>& state,
-                    Params& P, const int64_t* stops, size_t nstops) {
+                    Params& P, const int64_t* stops, size_t nstops, bool generic) {
   HostSetup hs;
   if (!hs.build(*c)) { g_err = hs.error; return LBFT_ERR_INVALID; }
   P = hs.params;
@@ -192,7 +314,7 @@ static int run_impl(const lbft_config* c, uint32_t* commit_counts, uint64_t* las
                               : run_all<NMAX, QS, false, true>(P, state, P.zig_x, P.zig_f))                          \
                : (P.record_rs ? run_all<NMAX, QS, true, false>(P, state, P.zig_x, P.zig_f)                          \
                               : run_all<NMAX, QS, false, false>(P, state, P.zig_x, P.zig_f)))
-  const int fx = getenv("HOSTCORE_NO_FIXED") ? (int)FX_NONE : fixed_shape_of(P);
+  const int fx = (generic || getenv("HOSTCORE_NO_FIXED")) ? (int)FX_NONE : fixed_shape_of(P);
   if (fx == FX_DEFAULT4) run_all_fx<16, 2, FX_DEFAULT4>(P, state, P.zig_x, P.zig_f);
   else if (fx == FX_PART7) run_all_fx<16, 3, FX_PART7>(P, state, P.zig_x, P.zig_f);
   else if (fx == FX_COMMITTEE64) run_all_fx<64, 3, FX_COMMITTEE64>(P, state, P.zig_x, P.zig_f);

@@ -253,6 +253,64 @@ class HostCore:
         return _round_switches(lambda c, i, out, cap, n: fn(c, i, P(st.ctypes.data), len(st), out, cap, n), self.lib.hostcore_last_error,
                                seeds, num_nodes, instance, max_clock, **kw)
 
+    # ---- the compact encoding of the four-author compile-time layout (sim_core.cuh Core::PACK, FX_DEFAULT4) ----
+    LAYOUT_KEYS = ("node_base", "node_words", "n_hasblk", "rset_words", "created_base", "qcmade_base", "chain_base", "round_cap",
+                   "pay_base", "pay_words", "payload_cap", "total_words")
+    DECODED_WORDS = 24 + 3 + 4 + 4  # per node: F_* scalars, vmask / tmask / tcmask, timeout hcbr[4], TC hcbr[4]
+
+    def packed_fields(self):
+        """The core's packed_field() table and constants, and the offsets of fixed_layout(FX_DEFAULT4): a dict with
+        'nscalar', 'scalar_words', 'packed_words', 'timeout_hcbr', 'tc_hcbr', 'fields' ([(word, shift, mask)] for F_* 0 ..
+        F_NSCALAR + 2, the last three the vote / timeout / TC author masks) and the layout keys of LAYOUT_KEYS."""
+        out = np.zeros(256, np.uint32)
+        fn = self.lib.hostcore_packed_fields
+        fn.argtypes = [P, ctypes.c_size_t]
+        k = fn(P(out.ctypes.data), len(out))
+        if k < 0:
+            raise RuntimeError(self.lib.hostcore_last_error().decode())
+        v = [int(x) for x in out[:k]]
+        info = dict(zip(("nscalar", "scalar_words", "packed_words", "timeout_hcbr", "tc_hcbr"), v[:5]))
+        nf = info["nscalar"] + 3
+        info["fields"] = [tuple(v[5 + 3 * f: 8 + 3 * f]) for f in range(nf)]
+        info.update(zip(self.LAYOUT_KEYS, v[5 + 3 * nf:]))
+        return info
+
+    def packed_roundtrip(self, vals, tile, node, lane):
+        """vals (24 scalars, 3 masks, 4 timeout hcbr, 4 TC hcbr) through store_node / put_timeout_hcbr /
+        copy_timeout_hcbr_to_tc into node `node` of lane `lane` of `tile` (uint32 [total_words * 32], updated in place), and
+        back: returns (load_node's 27 values, node_ld's 27 values, hcbr_of of the timeout vector, hcbr_of of the TC vector)."""
+        v = np.ascontiguousarray(vals, dtype=np.uint32)
+        assert v.shape == (35,) and tile.dtype == np.uint32 and tile.flags["C_CONTIGUOUS"]
+        out = np.zeros(62, np.uint32)
+        fn = self.lib.hostcore_packed_roundtrip
+        fn.argtypes = [P, ctypes.c_uint32, ctypes.c_uint32, P, P]
+        if fn(P(v.ctypes.data), node, lane, P(tile.ctypes.data), P(out.ctypes.data)) != 0:
+            raise RuntimeError(self.lib.hostcore_last_error().decode())
+        return out[:27], out[27:54], out[54:58], out[58:62]
+
+    def final_state(self, seeds, num_nodes, max_clock=1000, generic=False, **kw):
+        """One FX_DEFAULT4 configuration through the compact-encoding instantiation (or, generic=True, the generic one on
+        the same layout) in a state buffer filled with 0xdeadbeef.  Returns a Result with lc_round, plus `decoded`
+        [instance, node, DECODED_WORDS] (hcbr entries of authors outside tmask / tcmask read 0) and `raw` [instance,
+        total_words], the instance's words out of its warp tile; `raw_tiles` is the whole buffer [tile, word, lane]."""
+        cfg, keep = make_config(seeds, num_nodes, max_clock, **kw)
+        I = cfg.num_instances
+        words = self.setup_info(num_nodes, max_clock, **kw)["words"]
+        tiles = (I + 31) // 32
+        res = Result(I, num_nodes)
+        res.lc_round = np.zeros((I, num_nodes), np.uint32)
+        res.decoded = np.zeros((I, num_nodes, self.DECODED_WORDS), np.uint32)
+        res.raw_tiles = np.zeros((tiles, words, 32), np.uint32)
+        fn = self.lib.hostcore_final_state
+        fn.argtypes = [ctypes.POINTER(LbftConfig), ctypes.c_int, P, P, P, P, P, P, P]
+        rc = fn(ctypes.byref(cfg), 1 if generic else 0, P(res.commit_counts.ctypes.data), P(res.last_states.ctypes.data),
+                P(res.lc_round.ctypes.data), P(res.counters.ctypes.data), P(res.status.ctypes.data), P(res.decoded.ctypes.data),
+                P(res.raw_tiles.ctypes.data))
+        if rc != 0:
+            raise RuntimeError(self.lib.hostcore_last_error().decode())
+        res.raw = res.raw_tiles.transpose(0, 2, 1).reshape(tiles * 32, words)[:I]
+        return res
+
 
 def assert_same(a, b, what=""):
     """Bit-exact comparison of two Result objects on everything the reference exposes."""
