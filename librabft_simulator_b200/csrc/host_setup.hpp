@@ -126,6 +126,209 @@ inline int fixed_shape_of(const Params& P) {
   return FX_NONE;
 }
 
+// The delay model's mean: what the stamp-width and queue-mode tests are sized by.
+inline double mean_delay(const lbft_config& c) {
+  return c.delay_kind == LBFT_DELAY_UNIFORM ? 0.5 * (double)(c.delay_lo + c.delay_hi) : c.delay_mean;
+}
+
+// Round capacity per epoch: round_cap, or enough for the horizon, in whole bitset words.
+inline uint32_t round_cap_of(const lbft_config& c) {
+  uint32_t rcap = c.round_cap ? c.round_cap : (uint32_t)(c.max_clock / 12 + 40);
+  rcap = (rcap + 31) / 32 * 32;
+  return rcap < 32 ? 32 : rcap;
+}
+
+// Epochs (node.rs:329-348): a node commits at most one command per round, so commands_per_epoch >= round_cap can never be
+// reached and the layout stays single-epoch (every BASELINE configuration).  Otherwise the per-round tables get `epochs` spans
+// of round_cap rounds each (global round id = epoch * rspan + round).
+inline uint32_t epochs_of(const lbft_config& c, uint32_t rcap) {
+  if (c.commands_per_epoch >= rcap) return 1;
+  uint32_t epochs = (uint32_t)(rcap / c.commands_per_epoch) + 2;
+  if (epochs > MAX_EPOCHS) epochs = MAX_EPOCHS;
+  while (epochs > 2 && (uint64_t)epochs * rcap > 32768) epochs--;
+  return epochs;
+}
+
+// The delay model of a configuration (simulator.rs:101-102) into the fields a sweep keeps per set; the error text if it is
+// not valid.
+inline const char* delay_model(const lbft_config& c, SweepSet& s) {
+  s.delay_kind = c.delay_kind;
+  if (c.delay_kind == LBFT_DELAY_LOGNORMAL) {
+    if (!(c.delay_mean > 0.0) || !(c.delay_variance >= 0.0)) return "LogNormal delay needs mean > 0 and variance >= 0";
+    s.mu = std::log(c.delay_mean / std::sqrt(1.0 + c.delay_variance / (c.delay_mean * c.delay_mean)));
+    s.sigma = std::sqrt(std::log(1.0 + c.delay_variance / (c.delay_mean * c.delay_mean)));
+    s.delay_const = s.sigma == 0.0;
+    s.delay_const_value = s.delay_const ? (int64_t)std::exp(s.mu) : 0;
+    if (s.delay_const && (s.delay_const_value < 0 || s.delay_const_value > (1 << 29))) return "constant delay out of range";
+  } else if (c.delay_kind == LBFT_DELAY_UNIFORM) {
+    if (c.delay_lo < 0 || c.delay_hi < c.delay_lo || c.delay_hi > (1 << 29)) return "uniform delay needs 0 <= lo <= hi < 2^29";
+    s.uni_lo = (uint64_t)c.delay_lo;
+    s.uni_span = (uint64_t)(c.delay_hi - c.delay_lo + 1);
+  } else return "unknown delay_kind";
+  return nullptr;
+}
+
+// Why `c` cannot make a handle (the first failing check), or null.
+inline const char* config_error(const lbft_config& c) {
+  if (c.struct_size != sizeof(lbft_config)) return "lbft_config.struct_size does not match this library (ABI mismatch)";
+  if (c.num_instances == 0) return "num_instances must be > 0";
+  if (c.num_nodes < 1 || c.num_nodes > 64) return "num_nodes must be in 1..64";
+  if (!c.seeds) return "seeds must not be NULL";
+  if (c.max_clock < 0 || c.max_clock >= (1 << 29)) return "max_clock must be in [0, 2^29)";
+  if (c.flags & ~(uint32_t)(LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE | LBFT_FLAG_TRUE_DATA_SYNC)) return "unknown bits in flags";
+  const bool tds = (c.flags & LBFT_FLAG_TRUE_DATA_SYNC) != 0;
+  if (tds && (c.flags & (LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE)))
+    return "LBFT_FLAG_TRUE_DATA_SYNC cannot be combined with recording / resumable runs";
+  if (c.commands_per_epoch == 0) return "commands_per_epoch must be > 0";
+  if (c.delta < 0 || c.target_commit_interval < 0) return "delta and target_commit_interval must be >= 0";
+  // delta == 0 makes round durations 0: a node can then create a timeout and propose in the same update (SURVEY App.
+  // C.1b), which the round-id form does not represent (the device would flag every instance LBFT_ST_INVARIANT after
+  // running the whole batch).  Refuse it up front.
+  if (c.delta == 0) return "delta = 0 is not supported: a timeout and a proposal in the same update (SURVEY App. C.1b)";
+  SweepSet s{};
+  if (const char* e = delay_model(c, s)) return e;
+  uint64_t total = 0;
+  for (uint32_t i = 0; i < c.num_nodes; i++) {
+    if (c.voting_rights && c.voting_rights[i] > (1u << 24)) return "voting_rights entries must be <= 2^24";
+    total += c.voting_rights ? c.voting_rights[i] : 1;
+  }
+  if (total == 0) return "total voting rights must be > 0";
+  if (c.partition_windows > 64) return "partition_windows must be <= 64";
+  if (round_cap_of(c) > 32768) return "round_cap must be <= 32768";
+  if (c.queue_cap > (1u << 20)) return "queue_cap too large";
+  if (c.payload_cap > 0xfff0u) return "payload_cap must be < 65520";
+  if (tds && c.commands_per_epoch < round_cap_of(c))
+    return "LBFT_FLAG_TRUE_DATA_SYNC needs commands_per_epoch >= round_cap (single-epoch runs)";
+  return nullptr;
+}
+
+// Kernel family.  One thread per instance needs tens of thousands of instances to fill an H100 (65 536 x 4 authors is one wave
+// of warps) and serialises the 32 instances of a warp through every fan-out; one WARP per instance (lbft_wide_kernel) has no
+// cross-instance divergence, splits fan-outs, queue scans and per-author vectors over its lanes, and for committees of <= 16
+// keeps the whole instance in shared memory: committees of <= 5 switch below ~4 K instances, larger ones always profit (H100:
+// 1 024 x 4 takes 2.5 ms wide against 9.2 ms on the thread kernel, 65 536 x 4 49.5 ms on the thread kernel against 68.4 ms
+// wide).  Recording / resumable handles stay on the thread kernel (the wide one has no save area).
+// LBFT_FORCE_KERNEL=wide|thread is a test seam, read here only: it runs one configuration through both families (and any
+// value turns off the sparse tiles below).
+// Returns KernelSel::tile: 1 = the wide kernel, else the thread kernel's instances per warp tile.  (Decided before the queue: the
+// wide kernel has a shared-memory queue of its own.)
+inline int kernel_family(const lbft_config& c, uint32_t rcap) {
+  const uint32_t N = c.num_nodes, I = c.num_instances;
+  const char* force = std::getenv("LBFT_FORCE_KERNEL");
+  if (c.flags & (LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE | LBFT_FLAG_TRUE_DATA_SYNC)) return 32;
+  if (force && !strcmp(force, "thread")) return 32;
+  if (force && !strcmp(force, "wide")) return 1;
+  if (N < 6 && I > 4096) return 32;
+  // Sparse warp tiles of the thread kernel (kernels.cuh TILE: 8 or 16 instances per warp, the other lanes retire at once):
+  // the instances of a warp serialise through each other's code paths, so as long as the batch does not fill the machine
+  // with full warps (2 112 warps of <= 128 registers = one wave on 132 SMs), fewer instances per warp finish sooner.
+  // Measured on BASELINE configs[4] (16 384 x 7, H100): 8 per warp 42.0 ms, full tiles 77.7, the wide kernel (8 lanes per
+  // instance) 60.4.  So for committees of 6..16 (calendar queue, plain
+  // single-epoch handles): about one wave of 8-instance warps -> tile 8, of 16-instance warps -> tile 16, more -> full
+  // tiles; below that the wide kernel.
+  if (force || N < 6 || N > 16 || c.max_clock > 4095 || I <= 12288 || c.commands_per_epoch < rcap || c.queue_cap > 0xfff0u) return 1;
+  const uint32_t tile = I <= 24576 ? 8u : (I <= 49152 ? 16u : 32u);
+  // (these handles get the calendar queue: the sparse-tile kernels keep the occupancy words of their instances in shared
+  // memory, sim_core.cuh KS — ((max_clock + 8) / 8) x tile words per warp: horizons up to ~3 500 ms at 8 per warp, ~1 750
+  // at 16)
+  return (uint64_t)(((uint32_t)c.max_clock + 8) / 8) * tile > 3584 ? 32 : (int)tile;
+}
+
+// The layout, with the queue mode (queue_scan) and the queue / payload capacities decided here.
+inline Layout choose_layout(const lbft_config& c, uint32_t rcap, uint32_t epochs, int tile) {
+  const uint32_t N = c.num_nodes;
+  const bool wide = tile == 1, tds = (c.flags & LBFT_FLAG_TRUE_DATA_SYNC) != 0;
+  // (recording round switches queues the duplicate timers the normal path elides — measured high-water marks
+  // roughly double, 46 -> 64+ at N = 4 — so the smallest committees get 128 entries and the HBM scan queue)
+  // (resumable runs queue them too: the event dropped at a stop must be the one the reference drops)
+  const bool record = (c.flags & (LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE)) != 0;
+  uint32_t pcap = c.payload_cap ? c.payload_cap : (N <= 4 ? 32u : (N <= 8 ? 64u : pow2_ceil(8 * N)));
+  // (true data-sync keeps a snapshot per request and per response in flight as well)
+  if (tds && !c.payload_cap) pcap = N <= 4 ? 128u : (N <= 8 ? 192u : 4 * pcap);
+  // The shortest horizons run on the compact entries: 32-bit keys (time:14 | kind:2 | stamp:16) + 16-bit payload words.
+  // (16-bit stamps: ~0.14 N^2 events are created per simulated ms at the reference's 10 ms mean delay, and proportionally
+  // more with shorter delays; stay well inside 65 536 — an overflow would be flagged, not silent)
+  const double mean = mean_delay(c), events_per_ms = 0.14 * N * N * (10.0 / (mean < 1.0 ? 1.0 : mean));
+  const bool compact = c.max_clock < (1 << 14) - 64 && pcap <= 255 && events_per_ms * (double)c.max_clock < 32768.0;
+  // Small committees use the scan queue (64-bit entries: time:24 | 3-kind:2 | stamp:22 | slot:8 | sender:4 |
+  // receiver:4, O(1) append, linear min-scan); larger ones the binary heap with 3-word entries.
+  // (explicit capacities beyond what the scan queue can encode / scan efficiently select the heap.)
+  uint32_t scan = N <= 5 && c.max_clock < (1 << 24) - 64 && c.payload_cap <= 255 && c.queue_cap <= 512 ? 1u : 0u;
+  uint32_t cap = c.queue_cap ? c.queue_cap : (scan ? (N <= 4 ? (record ? 128u : 64u) : 8 * N * N) : pow2_ceil(6 * N * N + 32));
+  if (cap < readout_queue_floor(scan, rcap)) cap = readout_queue_floor(scan, rcap);
+  if (scan && compact && cap <= 64) scan = 2;  // queue in shared memory
+  // the HBM scan queue hands out 22-bit creation stamps: long horizons / very short delays go to the heap or calendar
+  // queue (30-bit / 32-bit stamps) instead of aborting with LBFT_ST_QUEUE_OVERFLOW half-way through
+  if (scan == 1 && events_per_ms * (double)c.max_clock > 2.0e6) scan = 0;
+  // The wide kernel scans its (single) shared-memory queue with all 32 lanes, so the same compact entries serve committees
+  // up to 16 (4-bit sender/receiver) and queues up to 1 024 entries.
+  if (wide && N <= 16 && compact) {
+    const uint32_t want = c.queue_cap ? c.queue_cap : (N <= 4 ? 64u : 8 * N * N);
+    if (want <= 1024) {
+      scan = 2;
+      cap = want < readout_queue_floor(2, rcap) ? readout_queue_floor(2, rcap) : want;
+    }
+  }
+  // everything else with a moderate horizon: calendar queue (O(1) push/pop, exact: FIFO order inside a (time, kind)
+  // list is creation-stamp order); the binary heap remains for long horizons
+  if (scan == 0 && c.max_clock <= 4095 && cap <= 0xfff0u) scan = 3;
+  // epochs: the read-out floor of the global round ids, for the mode as it stands; then a shared-memory queue that outgrew
+  // shared memory moves to the HBM scan, calendar or heap queue (keeping the floor it got)
+  if (epochs > 1) {
+    const uint32_t floor = readout_queue_floor(scan, epochs * rcap);
+    if (cap < floor) cap = scan ? floor : pow2_ceil(floor);
+    if (scan == 2 && cap > (wide ? 1024u : 64u)) scan = N <= 5 ? 1u : (c.max_clock <= 4095 ? 3u : 0u);
+  }
+  return make_layout(N, rcap, cap, pcap, c.partition_windows, scan, (uint32_t)c.max_clock, (c.flags & LBFT_FLAG_ROUND_SWITCHES) != 0,
+                     (c.flags & LBFT_FLAG_RESUMABLE) != 0, epochs, tds);
+}
+
+// The kernel a handle launches, once its layout is known.
+inline KernelSel select_kernel(const lbft_config& c, int tile, const Params& p, bool sweep) {
+  KernelSel k{};
+  const uint32_t N = c.num_nodes, qscan = p.L.queue_scan;
+  k.wide = tile == 1;
+  k.tile = tile;
+  // lanes per instance: enough for the committee's fan-out, few enough that a warp carries several instances
+  // (8 lanes per instance — four instances per warp — win once the batch fills the machine with warps, committees of 64
+  // included: on an H100 8 192 x 64 takes 0.86 s against 1.32 s with a warp per instance; below ~4 K instances a whole warp
+  // per instance has the lower latency)
+  k.group = c.num_instances > 4096 && p.L.epochs == 1 ? 8 : 32;
+  // wide kernel: the whole instance lives in shared memory when the instances of 16 resident warps (32 / group each) fit on
+  // an SM
+  const size_t smem_bytes = sizeof(uint32_t) * (size_t)p.L.total_words + 6u * (size_t)p.L.queue_cap + 1024u;
+  k.smem = k.wide && qscan == 2 && p.L.epochs == 1 && smem_bytes * (128u / k.group) <= 56u * 1024u;
+  k.qmode = (int)qscan;
+  k.nmax = (qscan == 1 || qscan == 2) ? 16 : (N <= 16 ? 16 : (N <= 32 ? 32 : 64));
+  k.epochs = p.L.epochs > 1;
+  k.tds = p.L.tds != 0;
+  k.rec = p.record_rs != 0;
+  k.res = p.resumable != 0;
+  // compile-time layouts: FX_DEFAULT4 on the thread kernel, FX_PART7 on its 8-instance warp tiles, FX_COMMITTEE64 on the wide
+  // kernel with 8 lanes per instance (sweep handles run the generic layout)
+  const int fx = fixed_shape_of(p);
+  k.fixed = !sweep && ((fx == FX_DEFAULT4 && !k.wide) || (fx == FX_PART7 && !k.wide && k.tile == 8) ||
+                       (fx == FX_COMMITTEE64 && k.wide && k.group == 8))
+                ? fx : FX_NONE;
+  k.sweep = sweep;
+  return k;
+}
+
+// `c` with the fields of one parameter set of a sweep substituted.
+inline lbft_config with_set(const lbft_config& c, const lbft_param_set& q) {
+  lbft_config cs = c;
+  cs.delay_kind = q.delay_kind;
+  cs.delay_mean = q.delay_mean;
+  cs.delay_variance = q.delay_variance;
+  cs.delay_lo = q.delay_lo;
+  cs.delay_hi = q.delay_hi;
+  cs.target_commit_interval = q.target_commit_interval;
+  cs.delta = q.delta;
+  cs.gamma = q.gamma;
+  cs.lambda = q.lambda;
+  return cs;
+}
+
 struct HostSetup {
   Params params{};  // pointer members are left null; the runtime fills in device addresses
   std::vector<double> zig_x, zig_f;
@@ -139,196 +342,14 @@ struct HostSetup {
   KernelSel sel{};
 
   bool build(const lbft_config& c) {
-    if (c.struct_size != sizeof(lbft_config)) return fail("lbft_config.struct_size does not match this library (ABI mismatch)");
-    if (c.num_instances == 0) return fail("num_instances must be > 0");
-    if (c.num_nodes < 1 || c.num_nodes > 64) return fail("num_nodes must be in 1..64");
-    if (!c.seeds) return fail("seeds must not be NULL");
-    if (c.max_clock < 0 || c.max_clock >= (1 << 29)) return fail("max_clock must be in [0, 2^29)");
-    if (c.flags & ~(uint32_t)(LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE | LBFT_FLAG_TRUE_DATA_SYNC)) return fail("unknown bits in flags");
-    const bool tds = (c.flags & LBFT_FLAG_TRUE_DATA_SYNC) != 0;
-    if (tds && (c.flags & (LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE)))
-      return fail("LBFT_FLAG_TRUE_DATA_SYNC cannot be combined with recording / resumable runs");
-    if (c.commands_per_epoch == 0) return fail("commands_per_epoch must be > 0");
-    if (c.delta < 0 || c.target_commit_interval < 0) return fail("delta and target_commit_interval must be >= 0");
-    // delta == 0 makes round durations 0: a node can then create a timeout and propose in the same update (SURVEY App.
-    // C.1b), which the round-id form does not represent (the device would flag every instance LBFT_ST_INVARIANT after
-    // running the whole batch).  Refuse it up front.
-    if (c.delta == 0) return fail("delta = 0 is not supported: a timeout and a proposal in the same update (SURVEY App. C.1b)");
-    const uint32_t N = c.num_nodes;
-    Params& p = params;
-    p.num_instances = c.num_instances;
-    p.max_clock = (int32_t)c.max_clock;
-    p.delay_kind = c.delay_kind;
-    if (c.delay_kind == LBFT_DELAY_LOGNORMAL) {
-      if (!(c.delay_mean > 0.0) || !(c.delay_variance >= 0.0)) return fail("LogNormal delay needs mean > 0 and variance >= 0");
-      // simulator.rs:101-102
-      p.mu = std::log(c.delay_mean / std::sqrt(1.0 + c.delay_variance / (c.delay_mean * c.delay_mean)));
-      p.sigma = std::sqrt(std::log(1.0 + c.delay_variance / (c.delay_mean * c.delay_mean)));
-      p.delay_const = p.sigma == 0.0;
-      p.delay_const_value = p.delay_const ? (int64_t)std::exp(p.mu) : 0;
-      if (p.delay_const && (p.delay_const_value < 0 || p.delay_const_value > (1 << 29))) return fail("constant delay out of range");
-    } else if (c.delay_kind == LBFT_DELAY_UNIFORM) {
-      if (c.delay_lo < 0 || c.delay_hi < c.delay_lo || c.delay_hi > (1 << 29)) return fail("uniform delay needs 0 <= lo <= hi < 2^29");
-      p.uni_lo = (uint64_t)c.delay_lo;
-      p.uni_span = (uint64_t)(c.delay_hi - c.delay_lo + 1);
-    } else return fail("unknown delay_kind");
-    p.tci = (int32_t)(c.target_commit_interval > (1 << 30) ? (1 << 30) : c.target_commit_interval);
-    p.commands_per_epoch = c.commands_per_epoch > 0xffffffffULL ? 0xffffffffu : (uint32_t)c.commands_per_epoch;
-    // voting rights / quorum (configuration.rs:29-56; simulated_context.rs:209-216 = all 1)
-    weights.assign(N, 1);
-    uint64_t total = 0;
-    for (uint32_t i = 0; i < N; i++) {
-      if (c.voting_rights) {
-        if (c.voting_rights[i] > (1u << 24)) return fail("voting_rights entries must be <= 2^24");
-        weights[i] = (uint32_t)c.voting_rights[i];
-      }
-      total += weights[i];
-    }
-    if (total == 0) return fail("total voting rights must be > 0");
-    p.quorum = (uint32_t)(2 * total / 3 + 1);
-    p.silent_mask = 0;
-    if (c.silent)
-      for (uint32_t i = 0; i < N; i++)
-        if (c.silent[i]) p.silent_mask |= 1ULL << i;
-    p.part_max_len = c.partition_max_len;
-    if (c.partition_windows > 64) return fail("partition_windows must be <= 64");
-    // capacities
-    uint32_t rcap = c.round_cap ? c.round_cap : (uint32_t)(c.max_clock / 12 + 40);
-    rcap = (rcap + 31) / 32 * 32;
-    if (rcap < 32) rcap = 32;
-    if (rcap > 32768) return fail("round_cap must be <= 32768");
-    // Small committees use the scan queue (64-bit entries: time:24 | 3-kind:2 | stamp:22 | slot:8 | sender:4 |
-    // receiver:4, O(1) append, linear min-scan); larger ones the binary heap with 3-word entries.
-    // (explicit capacities beyond what the scan queue can encode / scan efficiently select the heap.)
-    uint32_t qscan = (N <= 5 && c.max_clock < (1 << 24) - 64) ? 1u : 0u;
-    if (c.payload_cap > 255 || c.queue_cap > 512) qscan = 0;
-    // Kernel family.  One thread per instance needs tens of thousands of instances to fill an H100 (65 536 x 4 authors is
-    // one wave of warps) and serialises the 32 instances of a warp through every fan-out; one WARP per instance
-    // (lbft_wide_kernel) has no cross-instance divergence, splits fan-outs, queue scans and per-author vectors over its
-    // lanes, and for committees of <= 16 keeps the whole instance in shared memory: committees of <= 5 switch below ~4 K
-    // instances, larger ones always profit (H100: 1 024 x 4 takes 2.5 ms wide against 9.2 ms on the thread kernel, 65 536 x 4
-    // 49.5 ms on the thread kernel against 68.4 ms wide).  Recording / resumable handles
-    // stay on the thread kernel (the wide one has no save area).
-    // LBFT_FORCE_KERNEL=wide|thread is a test seam, read here only: it runs one configuration through both families (and any
-    // value turns off the sparse tiles below).
-    const bool modes = (c.flags & (LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE)) != 0;
-    const char* force = std::getenv("LBFT_FORCE_KERNEL");
-    bool wide = !modes && !tds && (N >= 6 || c.num_instances <= 4096);
-    if (force && !strcmp(force, "wide") && !modes && !tds) wide = true;
-    if (force && !strcmp(force, "thread")) wide = false;
-    // Sparse warp tiles of the thread kernel (kernels.cuh TILE: 8 or 16 instances per warp, the other lanes retire at once):
-    // the instances of a warp serialise through each other's code paths, so as long as the batch does not fill the machine
-    // with full warps (2 112 warps of <= 128 registers = one wave on 132 SMs), fewer instances per warp finish sooner.
-    // Measured on BASELINE configs[4] (16 384 x 7, H100): 8 per warp 42.0 ms, full tiles 77.7, the wide kernel (8 lanes per
-    // instance) 60.4.  So for committees of 6..16 (calendar queue, plain
-    // single-epoch handles): about one wave of 8-instance warps -> tile 8, of 16-instance warps -> tile 16, more -> full
-    // tiles; below that the wide kernel.
-    uint32_t tile = 32;
-    if (!force && wide && N >= 6 && N <= 16 && c.max_clock <= 4095 && c.num_instances > 12288 && c.commands_per_epoch >= rcap &&
-        c.queue_cap <= 0xfff0u) {
-      wide = false;
-      tile = c.num_instances <= 24576 ? 8u : (c.num_instances <= 49152 ? 16u : 32u);
-      // (these handles get the calendar queue: the sparse-tile kernels keep the occupancy words of their instances in shared
-      // memory, sim_core.cuh KS — ((max_clock + 8) / 8) x tile words per warp: horizons up to ~3 500 ms at 8 per warp, ~1 750
-      // at 16)
-      if ((uint64_t)(((uint32_t)c.max_clock + 8) / 8) * tile > 3584) tile = 32;
-    }
-    sel.wide = wide;
-    sel.tile = wide ? 1 : (int)tile;
-    // lanes per instance: enough for the committee's fan-out, few enough that a warp carries several instances
-    // (8 lanes per instance — four instances per warp — win once the batch fills the machine with warps, committees of 64
-    // included: on an H100 8 192 x 64 takes 0.86 s against 1.32 s with a warp per instance; below ~4 K instances a whole warp
-    // per instance has the lower latency)
-    sel.group = c.num_instances > 4096 ? 8 : 32;
-    // (recording round switches queues the duplicate timers the normal path elides — measured high-water marks
-    // roughly double, 46 -> 64+ at N = 4 — so the smallest committees get 128 entries and the HBM scan queue)
-    // (resumable runs queue them too: the event dropped at a stop must be the one the reference drops)
-    const bool record = (c.flags & (LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE)) != 0;
-    uint32_t qcap = c.queue_cap ? c.queue_cap : (qscan ? (N <= 4 ? (record ? 128u : 64u) : 8 * N * N) : pow2_ceil(6 * N * N + 32));
-    if (2 * qcap < rcap && qscan) qcap = (rcap + 1) / 2;  // the read-out reuses the queue area as chain scratch
-    if (qcap < rcap && !qscan) qcap = rcap;
-    if (qcap > (1u << 20)) return fail("queue_cap too large");
-    uint32_t pcap = c.payload_cap ? c.payload_cap : (N <= 4 ? 32u : (N <= 8 ? 64u : pow2_ceil(8 * N)));
-    // (true data-sync keeps a snapshot per request and per response in flight as well)
-    if (tds && !c.payload_cap) pcap = N <= 4 ? 128u : (N <= 8 ? 192u : 4 * pcap);
-    if (pcap > 0xfff0u) return fail("payload_cap must be < 65520");
-    // shortest horizons: 32-bit keys (time:14 | kind:2 | stamp:16) + 16-bit payload words, queue in shared memory
-    // (16-bit stamps: ~0.14 N^2 events are created per simulated ms at the reference's 10 ms mean delay, and
-    // proportionally more with shorter delays; stay well inside 65 536 — an overflow would be flagged, not silent)
-    const double mean_delay = c.delay_kind == LBFT_DELAY_UNIFORM ? 0.5 * (double)(c.delay_lo + c.delay_hi) : c.delay_mean;
-    const double events_per_ms = 0.14 * N * N * (10.0 / (mean_delay < 1.0 ? 1.0 : mean_delay));
-    if (qscan && c.max_clock < (1 << 14) - 64 && qcap <= 64 && pcap <= 255 && events_per_ms * (double)c.max_clock < 32768.0)
-      qscan = 2;
-    // the HBM scan queue hands out 22-bit creation stamps: long horizons / very short delays go to the heap or calendar
-    // queue (30-bit / 32-bit stamps) instead of aborting with LBFT_ST_QUEUE_OVERFLOW half-way through
-    if (qscan == 1 && events_per_ms * (double)c.max_clock > 2.0e6) qscan = 0;
-    // The wide kernel scans its (single) shared-memory queue with all 32 lanes, so the same compact entries serve committees
-    // up to 16 (4-bit sender/receiver) and queues up to 1 024 entries.
-    if (wide && N <= 16 && c.max_clock < (1 << 14) - 64 && pcap <= 255 && events_per_ms * (double)c.max_clock < 32768.0) {
-      const uint32_t want = c.queue_cap ? c.queue_cap : (N <= 4 ? 64u : 8 * N * N);
-      if (want <= 1024) {
-        qscan = 2;
-        qcap = want;
-        if (2 * qcap < rcap) qcap = (rcap + 1) / 2;
-      }
-    }
-    // everything else with a moderate horizon: calendar queue (O(1) push/pop, exact: FIFO order inside a (time, kind)
-    // list is creation-stamp order); the binary heap remains for long horizons
-    if (qscan == 0 && c.max_clock <= 4095 && qcap <= 0xfff0u) qscan = 3;
-    // loop_until(.., Some(csv_path)) simulator.rs:380-381: keep DataWriter's round-switch table (the compile-time-layout
-    // kernel never records: its layout has no table, so the generic instantiation is selected)
-    p.record_rs = (c.flags & LBFT_FLAG_ROUND_SWITCHES) ? 1u : 0u;
-    p.resumable = (c.flags & LBFT_FLAG_RESUMABLE) ? 1u : 0u;
-    p.stop_clock = p.max_clock;
-    p.run_flags = 0;
-    // Epochs (node.rs:329-348): a node commits at most one command per round, so commands_per_epoch >= round_cap can never
-    // be reached and the layout stays single-epoch (every BASELINE configuration).  Otherwise the per-round tables get
-    // `epochs` spans of round_cap rounds each (global round id = epoch * rspan + round).
-    uint32_t epochs = 1;
-    if (c.commands_per_epoch < rcap) {
-      if (tds) return fail("LBFT_FLAG_TRUE_DATA_SYNC needs commands_per_epoch >= round_cap (single-epoch runs)");
-      sel.group = 32;
-      epochs =(uint32_t)(rcap / c.commands_per_epoch) + 2;
-      if (epochs > MAX_EPOCHS) epochs = MAX_EPOCHS;
-      while (epochs > 2 && (uint64_t)epochs * rcap > 32768) epochs--;
-      if (qcap < (epochs * rcap + 1) / 2 && qscan) qcap = (epochs * rcap + 1) / 2;  // read-out scratch (see above)
-      if (qcap < epochs * rcap && !qscan) qcap = pow2_ceil(epochs * rcap);
-      if (qscan == 2 && qcap > (wide ? 1024u : 64u)) qscan = N <= 5 ? 1u : (c.max_clock <= 4095 ? 3u : 0u);
-    }
-    p.L = make_layout(N, rcap, qcap, pcap, c.partition_windows, qscan, (uint32_t)c.max_clock, p.record_rs != 0, p.resumable != 0, epochs, tds);
-    // wide kernel: the whole instance lives in shared memory when the instances of 16 resident warps (32 / group each) fit on
-    // an SM
-    const size_t smem_bytes = sizeof(uint32_t) * (size_t)p.L.total_words + 6u * (size_t)qcap + 1024u;
-    sel.smem = wide && qscan == 2 && epochs == 1 && smem_bytes * (128u / sel.group) <= 56u * 1024u;
-    // leader(round) for every representable round (+1: the pacemaker looks at active_round <= round_cap)
-    leader.resize(rcap + 1);
-    for (uint32_t r = 0; r <= rcap; r++) leader[r] = (uint8_t)pick_author(weights, total, siphash13_u64(r));
-    // duration(n) = (delta as f64 * (n as f64).powf(gamma)) as i64; period = (lambda * duration as f64) as i64
-    duration.resize(rcap + 1);
-    period.resize(rcap + 1);
-    for (uint32_t n = 0; n <= rcap; n++) {
-      double dv = (double)c.delta * std::pow((double)n, c.gamma);
-      int64_t dur = std::isnan(dv) ? 0 : (dv >= 9.2e18 ? INT64_MAX : (dv <= -9.2e18 ? INT64_MIN : (int64_t)dv));
-      double pv = c.lambda * (double)dur;
-      int64_t per = std::isnan(pv) ? 0 : (pv >= 9.2e18 ? INT64_MAX : (pv <= -9.2e18 ? INT64_MIN : (int64_t)pv));
-      const int64_t CL = 1 << 30;  // any deadline beyond max_clock (< 2^29) behaves identically
-      duration[n] = (int32_t)(dur > CL ? CL : (dur < -CL ? -CL : dur));
-      period[n] = (int32_t)(per > CL ? CL : (per < -CL ? -CL : per));
-    }
-    for (uint32_t i = 0; i < 64; i++) p.c_weights[i] = i < N ? weights[i] : 0;
-    build_ziggurat();
-    build_delay_table();
-    sel.qmode = (int)qscan;
-    sel.nmax = (qscan == 1 || qscan == 2) ? 16 : (N <= 16 ? 16 : (N <= 32 ? 32 : 64));
-    sel.epochs = epochs > 1;
-    sel.tds = tds;
-    sel.rec = p.record_rs != 0;
-    sel.res = p.resumable != 0;
-    // compile-time layouts: FX_DEFAULT4 on the thread kernel, FX_PART7 on its 8-instance warp tiles, FX_COMMITTEE64 on the wide
-    // kernel with 8 lanes per instance
-    const int fx = fixed_shape_of(p);
-    sel.fixed = (fx == FX_DEFAULT4 && !wide) || (fx == FX_PART7 && !wide && tile == 8) || (fx == FX_COMMITTEE64 && wide && sel.group == 8)
-                    ? fx : FX_NONE;
+    if (const char* e = config_error(c)) return fail(e);
+    const uint32_t rcap = round_cap_of(c);
+    const int tile = kernel_family(c, rcap);
+    build_shared(c, choose_layout(c, rcap, epochs_of(c, rcap), tile));
+    SweepSet s{};
+    add_set(c, rcap, s);
+    use_set(s);
+    sel = select_kernel(c, tile, params, false);
     return true;
   }
 
@@ -343,79 +364,106 @@ struct HostSetup {
     if (c.flags) return fail("sweep handles take no flags (recording, resumable and true data-sync runs are plain handles only)");
     for (uint32_t i = 0; i < c.num_instances; i++)
       if (set_of_instance[i] >= num_sets) return fail("set_of_instance has an index >= num_sets");
-    auto with_set = [&c](const lbft_param_set& q) {
-      lbft_config cs = c;
-      cs.delay_kind = q.delay_kind;
-      cs.delay_mean = q.delay_mean;
-      cs.delay_variance = q.delay_variance;
-      cs.delay_lo = q.delay_lo;
-      cs.delay_hi = q.delay_hi;
-      cs.target_commit_interval = q.target_commit_interval;
-      cs.delta = q.delta;
-      cs.gamma = q.gamma;
-      cs.lambda = q.lambda;
-      return cs;
-    };
-    const auto mean_delay = [](const lbft_param_set& q) {
-      return q.delay_kind == LBFT_DELAY_UNIFORM ? 0.5 * (double)(q.delay_lo + q.delay_hi) : q.delay_mean;
-    };
-    sets.resize(num_sets);
-    duration.clear();
-    period.clear();
-    std::vector<double> thr_all;
     uint32_t fastest = 0;
     for (uint32_t s = 0; s < num_sets; s++) {
-      HostSetup h;
-      if (!h.build(with_set(ps[s])) || ps[s].reserved) {
-        char buf[64];
-        snprintf(buf, sizeof buf, "parameter set %u: ", s);
-        return fail((buf + (ps[s].reserved ? std::string("reserved must be 0") : h.error)).c_str());
-      }
-      const Params& q = h.params;
-      SweepSet& w = sets[s];
-      w.delay_kind = q.delay_kind;
-      w.delay_const = q.delay_const;
-      w.delay_const_value = q.delay_const_value;
-      w.mu = q.mu;
-      w.sigma = q.sigma;
-      w.uni_lo = q.uni_lo;
-      w.uni_span = q.uni_span;
-      w.tci = q.tci;
-      w.delay_kmax = q.delay_kmax;
-      w.thr_off = (uint32_t)thr_all.size();
-      w.rt_off = (uint32_t)duration.size();
-      thr_all.insert(thr_all.end(), h.delay_thr.begin(), h.delay_thr.end());
-      duration.insert(duration.end(), h.duration.begin(), h.duration.end());
-      period.insert(period.end(), h.period.begin(), h.period.end());
-      if (mean_delay(ps[s]) < mean_delay(ps[fastest])) fastest = s;
+      const lbft_config cs = with_set(c, ps[s]);
+      const char* e = config_error(cs);
+      if (e || ps[s].reserved)
+        return fail(("parameter set " + std::to_string(s) + ": " + (ps[s].reserved ? "reserved must be 0" : e)).c_str());
+      if (mean_delay(cs) < mean_delay(with_set(c, ps[fastest]))) fastest = s;
     }
-    std::vector<int32_t> dur_all, per_all;
-    dur_all.swap(duration);
-    per_all.swap(period);
-    if (!build(with_set(ps[fastest]))) return false;
-    if (c.commands_per_epoch < params.L.round_cap)
+    const lbft_config cf = with_set(c, ps[fastest]);
+    const uint32_t rcap = round_cap_of(cf);
+    if (c.commands_per_epoch < rcap)
       return fail("sweep handles need commands_per_epoch >= round_cap (single-epoch runs: epochs are plain handles only)");
-    duration.swap(dur_all);
-    period.swap(per_all);
-    delay_thr.swap(thr_all);
+    const int tile = kernel_family(cf, rcap);
+    build_shared(cf, choose_layout(cf, rcap, 1, tile));
+    sets.resize(num_sets);
+    for (uint32_t s = 0; s < num_sets; s++) add_set(with_set(c, ps[s]), rcap, sets[s]);
+    use_set(sets[fastest]);
     set_of.assign(set_of_instance, set_of_instance + c.num_instances);
-    sel.fixed = FX_NONE;
-    sel.sweep = true;
+    sel = select_kernel(cf, tile, params, true);
     return true;
   }
 
+ private:
+  // Everything but the per-set part: the launch-uniform fields of Params, the voting rights, the leader table and the ziggurat.
+  void build_shared(const lbft_config& c, const Layout& L) {
+    const uint32_t N = c.num_nodes;
+    Params& p = params;
+    p.num_instances = c.num_instances;
+    p.max_clock = (int32_t)c.max_clock;
+    p.commands_per_epoch = c.commands_per_epoch > 0xffffffffULL ? 0xffffffffu : (uint32_t)c.commands_per_epoch;
+    // voting rights / quorum (configuration.rs:29-56; simulated_context.rs:209-216 = all 1)
+    weights.assign(N, 1);
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < N; i++) {
+      if (c.voting_rights) weights[i] = (uint32_t)c.voting_rights[i];
+      total += weights[i];
+    }
+    p.quorum = (uint32_t)(2 * total / 3 + 1);
+    for (uint32_t i = 0; i < 64; i++) p.c_weights[i] = i < N ? weights[i] : 0;
+    if (c.silent)
+      for (uint32_t i = 0; i < N; i++)
+        if (c.silent[i]) p.silent_mask |= 1ULL << i;
+    p.part_max_len = c.partition_max_len;
+    // loop_until(.., Some(csv_path)) simulator.rs:380-381: keep DataWriter's round-switch table (the compile-time-layout
+    // kernel never records: its layout has no table, so the generic instantiation is selected)
+    p.record_rs = (c.flags & LBFT_FLAG_ROUND_SWITCHES) ? 1u : 0u;
+    p.resumable = (c.flags & LBFT_FLAG_RESUMABLE) ? 1u : 0u;
+    p.stop_clock = p.max_clock;
+    p.L = L;
+    // leader(round) for every representable round (+1: the pacemaker looks at active_round <= round_cap)
+    leader.resize(L.rspan + 1);
+    for (uint32_t r = 0; r <= L.rspan; r++) leader[r] = (uint8_t)pick_author(weights, total, siphash13_u64(r));
+    build_ziggurat();
+  }
+
+  // The part of a configuration a sweep varies per parameter set (lbft_param_set): its delay model and tci into `s`, its delay
+  // thresholds and its duration / period tables appended to delay_thr / duration / period, where `s` records their offsets.
+  void add_set(const lbft_config& c, uint32_t rcap, SweepSet& s) {
+    delay_model(c, s);  // (valid: config_error() has checked it)
+    s.tci = (int32_t)(c.target_commit_interval > (1 << 30) ? (1 << 30) : c.target_commit_interval);
+    s.thr_off = (uint32_t)delay_thr.size();
+    build_delay_table(s);
+    // duration(n) = (delta as f64 * (n as f64).powf(gamma)) as i64; period = (lambda * duration as f64) as i64
+    s.rt_off = (uint32_t)duration.size();
+    for (uint32_t n = 0; n <= rcap; n++) {
+      double dv = (double)c.delta * std::pow((double)n, c.gamma);
+      int64_t dur = std::isnan(dv) ? 0 : (dv >= 9.2e18 ? INT64_MAX : (dv <= -9.2e18 ? INT64_MIN : (int64_t)dv));
+      double pv = c.lambda * (double)dur;
+      int64_t per = std::isnan(pv) ? 0 : (pv >= 9.2e18 ? INT64_MAX : (pv <= -9.2e18 ? INT64_MIN : (int64_t)pv));
+      const int64_t CL = 1 << 30;  // any deadline beyond max_clock (< 2^29) behaves identically
+      duration.push_back((int32_t)(dur > CL ? CL : (dur < -CL ? -CL : dur)));
+      period.push_back((int32_t)(per > CL ? CL : (per < -CL ? -CL : per)));
+    }
+  }
+
+  // The launch-uniform copy of a set's delay model and tci (a sweep's kernels read each instance's set instead).
+  void use_set(const SweepSet& s) {
+    Params& p = params;
+    p.delay_kind = s.delay_kind;
+    p.delay_const = s.delay_const;
+    p.delay_const_value = s.delay_const_value;
+    p.mu = s.mu;
+    p.sigma = s.sigma;
+    p.uni_lo = s.uni_lo;
+    p.uni_span = s.uni_span;
+    p.tci = s.tci;
+    p.delay_kmax = s.delay_kmax;
+  }
+
   // LogNormal delay without a device-side exp(): the reference truncates exp(mu + sigma*z) to an integer
-  // (simulator.rs:115-117), so only the integer part matters.  delay_thr[k] is the smallest double z with
+  // (simulator.rs:115-117), so only the integer part matters.  thr[k] is the smallest double z with
   // (exp(mu + sigma*z) as i64) >= k, found by bisection over the doubles with the HOST libm — the very
   // function the Rust reference calls — so the device result is bit-identical to the host's by
   // construction (no last-ulp dependence on the CUDA math library).  Table: thr[0] = -inf,
   // thr[1..kmax], thr[kmax+1] = +inf, where kmax = delay at the largest deviate the ziggurat can emit.
-  void build_delay_table() {
-    Params& p = params;
-    p.delay_kmax = 0;
-    delay_thr.clear();
-    if (p.delay_kind != LBFT_DELAY_LOGNORMAL || p.delay_const) return;
-    const double mu = p.mu, sigma = p.sigma;
+  // Appended to delay_thr; s.delay_kmax = 0 (and nothing appended) keeps the exp() path.
+  void build_delay_table(SweepSet& s) {
+    s.delay_kmax = 0;
+    if (s.delay_kind != LBFT_DELAY_LOGNORMAL || s.delay_const) return;
+    const double mu = s.mu, sigma = s.sigma;
     auto D = [mu, sigma](double z) -> int64_t {
       double v = std::exp(mu + sigma * z);
       return v >= 9.0e18 ? INT64_MAX : (int64_t)v;
@@ -425,22 +473,23 @@ struct HostSetup {
     if (kmax < 1 || kmax > 4096) return;  // too wide: keep the exp() path
     auto key = [](double d) { int64_t b; memcpy(&b, &d, 8); return b < 0 ? INT64_MIN - b : b; };  // monotone map
     auto unkey = [](int64_t k) { int64_t b = k < 0 ? INT64_MIN - k : k; double d; memcpy(&d, &b, 8); return d; };
-    delay_thr.assign((size_t)kmax + 2, 0.0);
-    delay_thr[0] = -INFINITY;
-    delay_thr[kmax + 1] = INFINITY;
+    std::vector<double> thr((size_t)kmax + 2, 0.0);
+    thr[0] = -INFINITY;
+    thr[kmax + 1] = INFINITY;
     for (int64_t k = 1; k <= kmax; k++) {
-      if (D(-ZMAX) >= k) { delay_thr[k] = -INFINITY; continue; }
+      if (D(-ZMAX) >= k) { thr[k] = -INFINITY; continue; }
       int64_t lo = key(-ZMAX), hi = key(ZMAX);  // D(lo) < k <= D(hi)
       while ((__int128)hi - lo > 1) {
         int64_t mid = (int64_t)(((__int128)lo + hi) >> 1);
         if (D(unkey(mid)) >= k) hi = mid; else lo = mid;
       }
-      delay_thr[k] = unkey(hi);
+      thr[k] = unkey(hi);
       // exp() must be monotone across the threshold for the table to be exact: check a few ulps either side
       for (int j = 1; j <= 4; j++)
-        if (D(unkey(hi + j)) < k || D(unkey(hi - j)) >= k) { delay_thr.clear(); return; }
+        if (D(unkey(hi + j)) < k || D(unkey(hi - j)) >= k) return;
     }
-    p.delay_kmax = (uint32_t)kmax;
+    delay_thr.insert(delay_thr.end(), thr.begin(), thr.end());
+    s.delay_kmax = (uint32_t)kmax;
   }
 
   // rand_distr 0.4.0 ziggurat_tables.rs (ZIG_NORM_X / ZIG_NORM_F / ZIG_NORM_R): regenerated with the
@@ -467,7 +516,6 @@ struct HostSetup {
     params.zig_r = lit(R);
   }
 
- private:
   bool fail(const char* msg) {
     error = msg;
     return false;

@@ -165,6 +165,13 @@ LBFT_LAYOUT_FN Layout make_layout(uint32_t N, uint32_t round_cap, uint32_t queue
   return L;
 }
 
+// The smallest queue_cap for a layout with `round_cap` global round ids: finalize() uses the queue area (from heap_time on, dead
+// by then in a one-shot run) as chain scratch, one word per committed block of a node.  A scan or calendar queue has at least
+// two words per entry; the binary heap is given one entry per round.
+LBFT_LAYOUT_FN uint32_t readout_queue_floor(uint32_t queue_scan, uint32_t round_cap) {
+  return queue_scan ? (round_cap + 1) / 2 : round_cap;
+}
+
 // Shapes with a kernel instantiation whose layout is a compile-time constant (sim_core.cuh FX): every field offset folds
 // into an immediate and the extension branches the shape cannot reach are compiled out.  The host selects one only when the
 // handle's layout is bit-identical to the constant and the delay model is the reference's (LogNormal served by the

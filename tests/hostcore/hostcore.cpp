@@ -107,6 +107,17 @@ static size_t read_round_switches(const Layout& L, const std::vector<uint32_t>& 
   return k;
 }
 
+// FNV-1a over a byte range; over a host table, its length and then its bytes (hostcore_setup_digest)
+static uint64_t fnv1a(uint64_t h, const void* p, size_t n) {
+  for (size_t i = 0; i < n; i++) h = (h ^ ((const uint8_t*)p)[i]) * 0x100000001b3ULL;
+  return h;
+}
+template <class T>
+static uint64_t fnv1a(uint64_t h, const std::vector<T>& v) {
+  const uint64_t n = v.size();
+  return fnv1a(fnv1a(h, &n, sizeof n), v.data(), n * sizeof(T));
+}
+
 extern "C" {
 const char* hostcore_last_error(void) { return g_err.c_str(); }
 
@@ -137,6 +148,18 @@ int hostcore_kernel_info(const lbft_config* c, char* buf, size_t cap) {
   if (!hs.build(*c)) { g_err = hs.error; return LBFT_ERR_INVALID; }
   if (!buf || cap == 0) { g_err = "NULL argument"; return LBFT_ERR_INVALID; }
   snprintf(buf, cap, "%s", kernel_name(hs.sel).c_str());
+  return LBFT_OK;
+}
+
+// One 64-bit digest (FNV-1a) of everything the host setup built for a configuration: the Params bytes before the device
+// pointers, padding included, then each host table with its length.  *epochs receives Layout::epochs.
+int hostcore_setup_digest(const lbft_config* c, uint64_t* digest, uint32_t* epochs) {
+  HostSetup hs;
+  if (!hs.build(*c)) { g_err = hs.error; return LBFT_ERR_INVALID; }
+  uint64_t h = fnv1a(0xcbf29ce484222325ULL, &hs.params, offsetof(Params, seeds));
+  h = fnv1a(fnv1a(fnv1a(fnv1a(h, hs.zig_x), hs.zig_f), hs.leader), hs.duration);
+  *digest = fnv1a(fnv1a(fnv1a(h, hs.period), hs.weights), hs.delay_thr);
+  *epochs = hs.params.L.epochs;
   return LBFT_OK;
 }
 

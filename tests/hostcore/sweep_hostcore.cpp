@@ -29,6 +29,17 @@ static void run_sweep_all(const Params& P, std::vector<uint32_t>& state, const u
   }
 }
 
+// FNV-1a over a byte range; over a host table, its length and then its bytes (hostcore_sweep_setup_digest)
+static uint64_t fnv1a(uint64_t h, const void* p, size_t n) {
+  for (size_t i = 0; i < n; i++) h = (h ^ ((const uint8_t*)p)[i]) * 0x100000001b3ULL;
+  return h;
+}
+template <class T>
+static uint64_t fnv1a(uint64_t h, const std::vector<T>& v) {
+  const uint64_t n = v.size();
+  return fnv1a(fnv1a(h, &n, sizeof n), v.data(), n * sizeof(T));
+}
+
 extern "C" {
 const char* hostcore_sweep_last_error(void) { return g_err.c_str(); }
 
@@ -39,6 +50,18 @@ int hostcore_kernel_info_sweep(const lbft_config* c, const lbft_param_set* sets,
   if (!hs.build_sweep(*c, sets, num_sets, set_of)) { g_err = hs.error; return LBFT_ERR_INVALID; }
   if (!buf || cap == 0) { g_err = "NULL argument"; return LBFT_ERR_INVALID; }
   snprintf(buf, cap, "%s", kernel_name(hs.sel).c_str());
+  return LBFT_OK;
+}
+
+// hostcore_setup_digest (hostcore.cpp) of a sweep handle's host setup, with the parameter sets and the set of each instance.
+int hostcore_sweep_setup_digest(const lbft_config* c, const lbft_param_set* sets, uint32_t num_sets, const uint32_t* set_of,
+                                uint64_t* digest) {
+  HostSetup hs;
+  if (!hs.build_sweep(*c, sets, num_sets, set_of)) { g_err = hs.error; return LBFT_ERR_INVALID; }
+  uint64_t h = fnv1a(0xcbf29ce484222325ULL, &hs.params, offsetof(Params, seeds));
+  h = fnv1a(fnv1a(fnv1a(fnv1a(h, hs.zig_x), hs.zig_f), hs.leader), hs.duration);
+  h = fnv1a(fnv1a(fnv1a(h, hs.period), hs.weights), hs.delay_thr);
+  *digest = fnv1a(fnv1a(h, hs.sets), hs.set_of);
   return LBFT_OK;
 }
 
