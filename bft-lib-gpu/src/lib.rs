@@ -105,6 +105,7 @@ pub mod ffi {
     pub const LBFT_FLAG_ROUND_SWITCHES: u32 = 1;
     pub const LBFT_FLAG_RESUMABLE: u32 = 2;
     pub const LBFT_FLAG_TRUE_DATA_SYNC: u32 = 4;
+    pub const LBFT_FLAG_COMMIT_TIMES: u32 = 16;
 
     pub enum LbftSim {}
 
@@ -128,6 +129,7 @@ pub mod ffi {
         pub fn lbft_counters(sim: *mut LbftSim, out: *mut LbftInstanceCounters) -> c_int;
         pub fn lbft_commit_log(sim: *mut LbftSim, instance: u32, node: u32, out: *mut LbftCommit, cap: usize, n: *mut usize) -> c_int;
         pub fn lbft_commit_logs(sim: *mut LbftSim, out: *mut LbftCommit, cap: usize, lens: *mut u32) -> c_int;
+        pub fn lbft_commit_times(sim: *mut LbftSim, committed: *mut i64, proposed: *mut i64, cap: usize) -> c_int;
         pub fn lbft_round_switches(sim: *mut LbftSim, instance: u32, out: *mut LbftRoundSwitch, cap: usize, n: *mut usize) -> c_int;
         pub fn lbft_snapshot_size(sim: *mut LbftSim, bytes: *mut usize) -> c_int;
         pub fn lbft_snapshot_save(sim: *mut LbftSim, buf: *mut u8, cap: usize) -> c_int;

@@ -82,6 +82,10 @@ typedef struct lbft_round_switch {
  * dispatches the request to the requester itself (bft-lib/src/simulator.rs:446), which makes every round trip a no-op; that
  * behaviour is the default here, as its golden tests pin it.  Plain runs only (no other flag, commands_per_epoch >= round_cap). */
 #define LBFT_FLAG_TRUE_DATA_SYNC 4u
+/* Record commit latency: the global clock (Simulator.clock) at which each block is proposed and at which each node commits it,
+ * read back with lbft_commit_times.  Plain and sweep handles; not with recording, resumable or true data-sync runs, nor with
+ * commands_per_epoch < round_cap (LBFT_ERR_INVALID).  (Bit 8 is unassigned.) */
+#define LBFT_FLAG_COMMIT_TIMES 16u
 
 /* Per-instance event counters (simulator.rs:31 event_count; data_writer.rs message counter). */
 typedef struct lbft_instance_counters {
@@ -162,8 +166,8 @@ typedef struct lbft_param_set {
  * Every output of instance i is what lbft_create + lbft_run give it with that set's fields substituted into `config`
  * (as long as neither run reports LBFT_ERR_CAPACITY: the sweep's layout is the one the set with the shortest mean delay
  * would get).  Each set is validated like lbft_create validates those fields.  Refused (LBFT_ERR_INVALID, before any device
- * work): num_sets == 0 or > min(num_instances, 65536), NULL sets / set_of_instance, an index >= num_sets, any flags bit,
- * and commands_per_epoch < round_cap (sweeps are plain single-epoch runs).  Every other entry point works on the handle
+ * work): num_sets == 0 or > min(num_instances, 65536), NULL sets / set_of_instance, an index >= num_sets, any flags bit
+ * but LBFT_FLAG_COMMIT_TIMES, and commands_per_epoch < round_cap (sweeps are plain single-epoch runs).  Every other entry point works on the handle
  * as on a plain one; lbft_set_seeds keeps the set assignment, and lbft_run_until / snapshots return LBFT_ERR_STATE. */
 int lbft_create_sweep(const lbft_config* config, const lbft_param_set* sets, uint32_t num_sets,
                       const uint32_t* set_of_instance, lbft_sim** out_sim);
@@ -206,6 +210,14 @@ int lbft_commit_log(lbft_sim* sim, uint32_t instance, uint32_t node, lbft_commit
  * lbft_commit_log).  Rows past a log's end are zero; logs longer than cap are truncated (lens tells).  lens may be
  * NULL. */
 int lbft_commit_logs(lbft_sim* sim, lbft_commit* out, size_t cap, uint32_t* lens);
+/* Commit latency of EVERY context of the batch (needs LBFT_FLAG_COMMIT_TIMES), aligned row for row with lbft_commit_logs and
+ * read the same way (one device pass, one copy).  committed[(instance * num_nodes + node) * cap + k] is the global clock of
+ * the event at which the node committed row k of its committed_history(); proposed[instance * cap + k] is the global clock
+ * of the event at which row k of the instance's longest log was proposed (= the row's NodeTime + the proposer's startup
+ * time).  Entries past a log's end (or past cap) are -1; proposed may be NULL.  LBFT_ERR_STATE without the flag, before a
+ * run has finished, while an lbft_run_async is in flight, or when the logs of an instance are not prefixes of one chain;
+ * LBFT_ERR_INVALID if cap is 0 or > 65535. */
+int lbft_commit_times(lbft_sim* sim, int64_t* committed, int64_t* proposed, size_t cap);
 /* Round switches of one instance (needs LBFT_FLAG_ROUND_SWITCHES, else LBFT_ERR_STATE): node-major,
  * rounds ascending within a node; writes min(*n, cap) rows, *n = full length.  Replaces the data behind
  * DataWriter::write_to_file's round_switches.txt (data_writer.rs:61-86); number_of_messages.txt is

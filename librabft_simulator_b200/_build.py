@@ -1,8 +1,8 @@
 """Build recipes for the native pieces (run by ``__graft_entry__.build()``).
 
 * ``csrc/liblbft_b200.so`` — the product: sm_90a (H100) CUDA kernels + the C ABI of ``include/lbft.h``.
-* ``oracle/liblbft_oracle.so``, ``tests/hostcore/libhostcore.so`` and ``tests/hostcore/libhostcore_sweep.so`` — test
-  infrastructure only.
+* ``oracle/liblbft_oracle.so``, ``tests/hostcore/libhostcore.so``, ``tests/hostcore/libhostcore_sweep.so`` and
+  ``tests/hostcore/libhostcore_ct.so`` — test infrastructure only.
 All artefacts are built in-tree and git-ignored.
 """
 import os
@@ -17,14 +17,15 @@ ORACLE_PATH = os.path.join(ORACLE_DIR, "liblbft_oracle.so")
 HOSTCORE_DIR = os.path.join(ROOT, "tests", "hostcore")
 HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore.so")
 SWEEP_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_sweep.so")
+CT_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_ct.so")
 
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 # Translation units of the product library: the host runtime (C ABI) and the kernel instantiations, one group per file so
 # that they compile in parallel and the bench kernel (k_fixed.cu) can be rebuilt alone; the sweep twins (lbft_create_sweep)
-# in units of their own.
+# and the commit-times twins (LBFT_FLAG_COMMIT_TIMES) in units of their own.
 PRODUCT_UNITS = ["lbft_api.cu", "k_fixed.cu", "k_scan.cu", "k_calendar.cu", "k_heap.cu", "k_wide.cu", "k_sweep_thread.cu",
-                 "k_sweep_wide.cu"]
+                 "k_sweep_wide.cu", "k_ct_thread.cu", "k_ct_wide.cu", "k_ct_sweep_thread.cu", "k_ct_sweep_wide.cu"]
 PRODUCT_HEADERS = ["kernels.cuh", "sim_core.cuh", "sim_params.h", "host_setup.hpp"]
 
 
@@ -134,5 +135,18 @@ def build_sweep_hostcore(force=False):
     return SWEEP_HOSTCORE_PATH
 
 
+def build_ct_hostcore(force=False):
+    """The host-compiled core of commit-times handles and the oracle observed per event (tests/hostcore/ct_hostcore.cpp):
+    test infrastructure."""
+    srcs = [os.path.join(HOSTCORE_DIR, "ct_hostcore.cpp"), os.path.join(ROOT, "include", "lbft.h")] + [
+        os.path.join(CSRC, f) for f in ("sim_core.cuh", "sim_params.h", "host_setup.hpp")] + [
+        os.path.join(ORACLE_DIR, f) for f in ("oracle_capi.cpp", "lbft_oracle.hpp")]
+    if not force and _newer(CT_HOSTCORE_PATH, srcs):
+        return CT_HOSTCORE_PATH
+    _run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-DLBFT_CHECK_C1",
+          "-o", CT_HOSTCORE_PATH, "ct_hostcore.cpp"], HOSTCORE_DIR)
+    return CT_HOSTCORE_PATH
+
+
 def build_all(force=False):
-    return build_product(force), build_oracle(force), build_hostcore(force), build_sweep_hostcore(force)
+    return build_product(force), build_oracle(force), build_hostcore(force), build_sweep_hostcore(force), build_ct_hostcore(force)

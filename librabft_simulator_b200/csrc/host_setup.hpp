@@ -88,12 +88,21 @@ struct KernelSel {
   int fixed;   // FX_* (sim_params.h): the instantiation with that compile-time layout; FX_NONE = generic
   bool rec, res;
   bool sweep;  // a sweep handle: lbft_sweep_event_loop_kernel / lbft_sweep_wide_kernel (per-instance parameter sets)
+  bool ct;     // LBFT_FLAG_COMMIT_TIMES: the commit-times twin (lbft_ct_*_kernel) of the kernel the other fields name
 };
 
 // The kernel's name, spelled like the symbol cuobjdump shows (lbft_kernel_info).
 inline std::string kernel_name(const KernelSel& k) {
   char buf[96];
-  if (k.sweep && k.wide)
+  if (k.ct && k.sweep && k.wide)
+    snprintf(buf, sizeof buf, "lbft_ct_sweep_wide_kernel<%d,%d,%s,%d>", k.nmax, k.qmode, k.smem ? "true" : "false", k.group);
+  else if (k.ct && k.sweep)
+    snprintf(buf, sizeof buf, "lbft_ct_sweep_event_loop_kernel<%d,%d,%d>", k.nmax, k.qmode, k.tile);
+  else if (k.ct && k.wide)
+    snprintf(buf, sizeof buf, "lbft_ct_wide_kernel<%d,%d,%s,%d,%d>", k.nmax, k.qmode, k.smem ? "true" : "false", k.group, k.fixed);
+  else if (k.ct)
+    snprintf(buf, sizeof buf, "lbft_ct_event_loop_kernel<%d,%d,%d,%d>", k.nmax, k.qmode, k.fixed, k.tile);
+  else if (k.sweep && k.wide)
     snprintf(buf, sizeof buf, "lbft_sweep_wide_kernel<%d,%d,%s,%d>", k.nmax, k.qmode, k.smem ? "true" : "false", k.group);
   else if (k.sweep)
     snprintf(buf, sizeof buf, "lbft_sweep_event_loop_kernel<%d,%d,%d>", k.nmax, k.qmode, k.tile);
@@ -106,7 +115,7 @@ inline std::string kernel_name(const KernelSel& k) {
 }
 // Whether two selections name the same kernel (the fields kernel_name prints).
 constexpr bool same_kernel(const KernelSel& a, const KernelSel& b) {
-  return a.sweep == b.sweep && a.wide == b.wide && a.nmax == b.nmax && a.qmode == b.qmode && a.epochs == b.epochs && a.fixed == b.fixed &&
+  return a.ct == b.ct && a.sweep == b.sweep && a.wide == b.wide && a.nmax == b.nmax && a.qmode == b.qmode && a.epochs == b.epochs && a.fixed == b.fixed &&
          (a.wide ? a.smem == b.smem && a.group == b.group
                  : a.rec == b.rec && a.res == b.res && a.tds == b.tds && a.tile == b.tile);
 }
@@ -175,7 +184,8 @@ inline const char* config_error(const lbft_config& c) {
   if (c.num_nodes < 1 || c.num_nodes > 64) return "num_nodes must be in 1..64";
   if (!c.seeds) return "seeds must not be NULL";
   if (c.max_clock < 0 || c.max_clock >= (1 << 29)) return "max_clock must be in [0, 2^29)";
-  if (c.flags & ~(uint32_t)(LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE | LBFT_FLAG_TRUE_DATA_SYNC)) return "unknown bits in flags";
+  if (c.flags & ~(uint32_t)(LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE | LBFT_FLAG_TRUE_DATA_SYNC | LBFT_FLAG_COMMIT_TIMES))
+    return "unknown bits in flags";
   const bool tds = (c.flags & LBFT_FLAG_TRUE_DATA_SYNC) != 0;
   if (tds && (c.flags & (LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE)))
     return "LBFT_FLAG_TRUE_DATA_SYNC cannot be combined with recording / resumable runs";
@@ -199,6 +209,11 @@ inline const char* config_error(const lbft_config& c) {
   if (c.payload_cap > 0xfff0u) return "payload_cap must be < 65520";
   if (tds && c.commands_per_epoch < round_cap_of(c))
     return "LBFT_FLAG_TRUE_DATA_SYNC needs commands_per_epoch >= round_cap (single-epoch runs)";
+  // commit times: the twins of the one-shot single-epoch kernels only (their table is indexed by round id)
+  if ((c.flags & LBFT_FLAG_COMMIT_TIMES) && (c.flags & (LBFT_FLAG_ROUND_SWITCHES | LBFT_FLAG_RESUMABLE | LBFT_FLAG_TRUE_DATA_SYNC)))
+    return "LBFT_FLAG_COMMIT_TIMES (commit times) cannot be combined with recording, resumable or true data-sync runs";
+  if ((c.flags & LBFT_FLAG_COMMIT_TIMES) && epochs_of(c, round_cap_of(c)) > 1)
+    return "LBFT_FLAG_COMMIT_TIMES (commit times) needs commands_per_epoch >= round_cap (single-epoch runs)";
   return nullptr;
 }
 
@@ -311,6 +326,7 @@ inline KernelSel select_kernel(const lbft_config& c, int tile, const Params& p, 
                        (fx == FX_COMMITTEE64 && k.wide && k.group == 8))
                 ? fx : FX_NONE;
   k.sweep = sweep;
+  k.ct = (c.flags & LBFT_FLAG_COMMIT_TIMES) != 0;  // (the flag changes nothing above: the twin of the flag-off kernel)
   return k;
 }
 
@@ -361,7 +377,7 @@ struct HostSetup {
     if (c.struct_size != sizeof(lbft_config)) return fail("lbft_config.struct_size does not match this library (ABI mismatch)");
     if (!ps || !set_of_instance) return fail("sets and set_of_instance must not be NULL");
     if (num_sets == 0 || num_sets > c.num_instances || num_sets > 65536u) return fail("num_sets must be in 1..min(num_instances, 65536)");
-    if (c.flags) return fail("sweep handles take no flags (recording, resumable and true data-sync runs are plain handles only)");
+    if (c.flags & ~(uint32_t)LBFT_FLAG_COMMIT_TIMES) return fail("sweep handles take no flags (recording, resumable and true data-sync runs are plain handles only)");
     for (uint32_t i = 0; i < c.num_instances; i++)
       if (set_of_instance[i] >= num_sets) return fail("set_of_instance has an index >= num_sets");
     uint32_t fastest = 0;

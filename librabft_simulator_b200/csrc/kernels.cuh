@@ -4,10 +4,12 @@
 //   lbft_wide_kernel<NMAX, QMODE>                          one WARP per instance (small batches, large committees)
 //   lbft_sweep_event_loop_kernel / lbft_sweep_wide_kernel  the same bodies for sweep handles (lbft_create_sweep: per-instance
 //                                                          delay model and NodeConfig)
+//   lbft_ct_*_kernel                                       the same bodies with the commit-time stores (LBFT_FLAG_COMMIT_TIMES),
+//                                                          a twin of every one-shot single-epoch plain and sweep kernel
 //
 // All do init -> event loop -> read-out in a single launch.  The instantiations are spread over several .cu files
-// (k_fixed.cu, k_scan.cu, k_calendar.cu, k_heap.cu, k_wide.cu, k_sweep_thread.cu, k_sweep_wide.cu) so that they compile in
-// parallel and the bench kernel can be rebuilt alone; lbft_api.cu only sees the launch_* functions declared at the end.
+// (k_fixed.cu, k_scan.cu, k_calendar.cu, k_heap.cu, k_wide.cu, k_sweep_thread.cu, k_sweep_wide.cu, k_ct_*.cu) so that they
+// compile in parallel and the bench kernel can be rebuilt alone; lbft_api.cu only sees the launch_* functions declared at the end.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -39,9 +41,10 @@ struct LaunchShape {
 // The body of both thread kernels (lbft_event_loop_kernel, lbft_sweep_event_loop_kernel), given the kernel's shared memory.
 // SW (sweep handles): the instance's parameter set supplies the delay model and NodeConfig; its thresholds are read through
 // L1 from the concatenated table, as the instances of one warp may belong to different sets.
-template <int NMAX, int QMODE, int FX, bool REC, bool RES, bool EP, bool TDS, int TILE, bool SW>
+// CT: the commit-time stores (sim_core.cuh Core CT) into `times`, [num_instances][N + 1][round_cap].
+template <int NMAX, int QMODE, int FX, bool REC, bool RES, bool EP, bool TDS, int TILE, bool SW, bool CT = false>
 __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, double* s_zf, double* s_thr, uint32_t* s_queue,
-                                                const uint32_t* set_of, const SweepSet* sets) {
+                                                const uint32_t* set_of, const SweepSet* sets, int32_t* times = nullptr) {
   static_assert(TILE == 32 || ((QMODE == 3 || QMODE == 2) && !REC && !RES && !EP && !TDS), "sparse tiles: plain kernels over the calendar / shared-memory queue");
   for (int i = threadIdx.x; i < 257; i += blockDim.x) {
     s_zx[i] = P.zig_x[i];
@@ -68,8 +71,9 @@ __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, d
   // sparse tiles over the calendar queue: the kind-occupancy words of the tile's instances in shared memory, a column per
   // lane (sim_core.cuh KS; the host only selects sparse tiles when 14 warps' worth fits, host_setup.hpp)
   constexpr bool KS = QMODE == 3 && TILE < 32;
-  Core<TileMem<TILE>, NMAX, QMODE, FX, REC, RES, 1, EP, TDS, KS, SW> core(P, mem, s_zx, s_zf, thr_fits ? s_thr : P.delay_thr, sk, sd);
+  Core<TileMem<TILE>, NMAX, QMODE, FX, REC, RES, 1, EP, TDS, KS, SW, CT> core(P, mem, s_zx, s_zf, thr_fits ? s_thr : P.delay_thr, sk, sd);
   if (KS) core.km = s_queue + (size_t)(threadIdx.x >> 5) * calendar_kmask_words(FX ? fixed_layout(FX) : P.L) * TILE + lane;
+  if constexpr (CT) core.ct = times + (size_t)inst * (core.L.num_nodes + 1) * core.L.round_cap;
   if constexpr (SW) core.bind_set(sets + set_of[inst]);
   if (RES && (P.run_flags & 1u)) core.restore_regs();  // a later lbft_run_until: continue where the last launch stopped
   else core.init(P.seeds[inst]);
@@ -124,8 +128,9 @@ LBFT_LAYOUT_FN uint32_t wide_smem_words_per_group(const Layout& L, int qmode, bo
 // SMEM: the instance's state words live in shared memory for the whole run; only the chain table (and the epoch table) is
 // copied to the instance's global extent at the end, for lbft_commit_log / lbft_commit_logs.
 // The body of both wide kernels (lbft_wide_kernel, lbft_sweep_wide_kernel).  SW: as event_loop_body.
-template <int NMAX, int QMODE, bool SMEM, int G, bool EP, int FX, bool SW>
-__device__ __forceinline__ void wide_body(const Params& P, uint32_t* s_wide, const uint32_t* set_of, const SweepSet* sets) {
+template <int NMAX, int QMODE, bool SMEM, int G, bool EP, int FX, bool SW, bool CT = false>
+__device__ __forceinline__ void wide_body(const Params& P, uint32_t* s_wide, const uint32_t* set_of, const SweepSet* sets,
+                                          int32_t* times = nullptr) {
   constexpr uint32_t kPerBlock = wide_warps(G) * 32 / G;
   const uint32_t grp = threadIdx.x / G, wl = threadIdx.x % G;
   const uint32_t inst = blockIdx.x * kPerBlock + grp;
@@ -138,8 +143,9 @@ __device__ __forceinline__ void wide_body(const Params& P, uint32_t* s_wide, con
   uint32_t* gstate = P.state + (size_t)inst * KL.total_words;
   uint32_t* state = SMEM ? sk + wide_queue_words(KL.queue_cap, QMODE) : gstate;
   TileMem<1> mem{state, 0};
-  Core<TileMem<1>, NMAX, QMODE, FX, false, false, G, EP, false, false, SW> core(P, mem, P.zig_x, P.zig_f, P.delay_thr, sk, sd);
+  Core<TileMem<1>, NMAX, QMODE, FX, false, false, G, EP, false, false, SW, CT> core(P, mem, P.zig_x, P.zig_f, P.delay_thr, sk, sd);
   core.wl = wl;
+  if constexpr (CT) core.ct = times + (size_t)inst * (KL.num_nodes + 1) * KL.round_cap;
   core.gm = G == 32 ? 0xffffffffu : (((1u << (G & 31)) - 1u) << ((threadIdx.x & 31u) & ~(uint32_t)(G - 1)));
   core.ws = ws;
   if constexpr (SW) core.bind_set(sets + set_of[inst]);
@@ -167,6 +173,43 @@ __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbf
   wide_body<NMAX, QMODE, SMEM, G, false, FX_NONE, true>(S.P, s_wide, S.set_of, S.sets);
 }
 
+// The parameter block of a commit-times kernel (LBFT_FLAG_COMMIT_TIMES): the plain (Params) or sweep (SweepParams) block and
+// the commit-time table, [num_instances][N + 1][round_cap] int32.  (A block of its own, so that no other kernel's parameters
+// move.)
+template <class KP>
+struct CtParams {
+  KP base;
+  int32_t* times;
+};
+
+// The commit-times twins of the one-shot single-epoch kernels: the same bodies with CT set.
+template <int NMAX, int QMODE, int FX, int TILE>
+__global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMODE>::kBlocksPerSm) lbft_ct_event_loop_kernel(const __grid_constant__ CtParams<Params> C) {
+  __shared__ double s_zx[257];
+  __shared__ double s_zf[257];
+  __shared__ double s_thr[kThrSmem];
+  extern __shared__ uint32_t s_queue[];
+  event_loop_body<NMAX, QMODE, FX, false, false, false, false, TILE, false, true>(C.base, s_zx, s_zf, s_thr, s_queue, nullptr, nullptr, C.times);
+}
+template <int NMAX, int QMODE, int TILE>
+__global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMODE>::kBlocksPerSm) lbft_ct_sweep_event_loop_kernel(const __grid_constant__ CtParams<SweepParams> C) {
+  __shared__ double s_zx[257];
+  __shared__ double s_zf[257];
+  extern __shared__ uint32_t s_queue[];
+  event_loop_body<NMAX, QMODE, FX_NONE, false, false, false, false, TILE, true, true>(C.base.P, s_zx, s_zf, nullptr, s_queue, C.base.set_of,
+                                                                                     C.base.sets, C.times);
+}
+template <int NMAX, int QMODE, bool SMEM, int G, int FX>
+__global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbft_ct_wide_kernel(const __grid_constant__ CtParams<Params> C) {
+  extern __shared__ __align__(8) uint32_t s_wide[];
+  wide_body<NMAX, QMODE, SMEM, G, false, FX, false, true>(C.base, s_wide, nullptr, nullptr, C.times);
+}
+template <int NMAX, int QMODE, bool SMEM, int G>
+__global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbft_ct_sweep_wide_kernel(const __grid_constant__ CtParams<SweepParams> C) {
+  extern __shared__ __align__(8) uint32_t s_wide[];
+  wide_body<NMAX, QMODE, SMEM, G, false, FX_NONE, true, true>(C.base.P, s_wide, C.base.set_of, C.base.sets, C.times);
+}
+
 // One per translation unit: launches the instantiation the selection names, or returns cudaErrorInvalidValue if the unit
 // has none (lbft_api.cu reports that with the kernel's name).
 cudaError_t launch_fixed(const KernelSel& k, const Params& P, cudaStream_t stream);
@@ -176,6 +219,10 @@ cudaError_t launch_heap(const KernelSel& k, const Params& P, cudaStream_t stream
 cudaError_t launch_wide(const KernelSel& k, const Params& P, cudaStream_t stream);
 cudaError_t launch_sweep_thread(const KernelSel& k, const SweepParams& S, cudaStream_t stream);
 cudaError_t launch_sweep_wide(const KernelSel& k, const SweepParams& S, cudaStream_t stream);
+cudaError_t launch_ct_thread(const KernelSel& k, const CtParams<Params>& C, cudaStream_t stream);
+cudaError_t launch_ct_wide(const KernelSel& k, const CtParams<Params>& C, cudaStream_t stream);
+cudaError_t launch_ct_sweep_thread(const KernelSel& k, const CtParams<SweepParams>& C, cudaStream_t stream);
+cudaError_t launch_ct_sweep_wide(const KernelSel& k, const CtParams<SweepParams>& C, cudaStream_t stream);
 
 // Lets `kernel` take up to the device's opt-in limit of shared memory per block, beyond the 48 KB default (the QMODE 2
 // queues of four warps, the wide kernel's shared-memory instance state); `whole_carveout` also asks for the largest
@@ -197,15 +244,20 @@ inline cudaError_t allow_optin_smem(Kernel kernel, bool whole_carveout) {
 
 inline const Params& params_of(const Params& P) { return P; }
 inline const Params& params_of(const SweepParams& S) { return S.P; }
+template <class KP>
+inline const Params& params_of(const CtParams<KP>& C) { return params_of(C.base); }
 
 // One instantiation of a kernel template: the selection that names it, and its launch.  try_launch launches it if `k` names
-// it and reports whether it did.  SW: the sweep twin of the generic plain instantiation (lbft_sweep_*_kernel).
+// it and reports whether it did.  SW: the sweep twin of the generic plain instantiation (lbft_sweep_*_kernel).  CT: the
+// commit-times twin (lbft_ct_*_kernel) of the instantiation the other arguments name.
 template <int NMAX, int QM, int FX = FX_NONE, bool REC = false, bool RES = false, bool EP = false, bool TDS = false, int TILE = 32,
-          bool SW = false>
+          bool SW = false, bool CT = false>
 struct ThreadKernel {
   static_assert(!SW || (FX == FX_NONE && !REC && !RES && !EP && !TDS), "sweeps: plain single-epoch generic kernels only");
-  static constexpr KernelSel sel{/*wide*/ false, /*smem*/ false, /*group*/ 0, EP, TDS, TILE, NMAX, QM, FX, REC, RES, SW};
-  using KParams = typename std::conditional<SW, SweepParams, Params>::type;  // the kernel's parameter block
+  static_assert(!CT || (!REC && !RES && !EP && !TDS), "commit times: one-shot single-epoch kernels only");
+  static constexpr KernelSel sel{/*wide*/ false, /*smem*/ false, /*group*/ 0, EP, TDS, TILE, NMAX, QM, FX, REC, RES, SW, CT};
+  using Base = typename std::conditional<SW, SweepParams, Params>::type;
+  using KParams = typename std::conditional<CT, CtParams<Base>, Base>::type;  // the kernel's parameter block
   static bool try_launch(const KernelSel& k, const KParams& KP, cudaStream_t stream, cudaError_t& e) {
     if (!same_kernel(k, sel)) return false;
     const Params& P = params_of(KP);
@@ -216,7 +268,9 @@ struct ThreadKernel {
     const size_t dyn = QM == 2 ? (size_t)(T / 32) * P.L.queue_cap * (32 * 4 + 32 * 2)
                                : (QM == 3 && TILE < 32 ? (size_t)calendar_kmask_words(P.L) * TILE * sizeof(uint32_t) : 0);
     void (*kernel)(KParams);
-    if constexpr (SW) kernel = lbft_sweep_event_loop_kernel<NMAX, QM, TILE>;
+    if constexpr (CT && SW) kernel = lbft_ct_sweep_event_loop_kernel<NMAX, QM, TILE>;
+    else if constexpr (CT) kernel = lbft_ct_event_loop_kernel<NMAX, QM, FX, TILE>;
+    else if constexpr (SW) kernel = lbft_sweep_event_loop_kernel<NMAX, QM, TILE>;
     else kernel = lbft_event_loop_kernel<NMAX, QM, FX, REC, RES, EP, TDS, TILE>;
     e = dyn > 0 ? allow_optin_smem(kernel, QM == 2) : cudaSuccess;
     if (e == cudaSuccess) {
@@ -226,11 +280,13 @@ struct ThreadKernel {
     return true;
   }
 };
-template <int NMAX, int QM, bool SMEM, int G, bool EP = false, int FX = FX_NONE, bool SW = false>
+template <int NMAX, int QM, bool SMEM, int G, bool EP = false, int FX = FX_NONE, bool SW = false, bool CT = false>
 struct WideKernel {
   static_assert(!SW || (FX == FX_NONE && !EP), "sweeps: plain single-epoch generic kernels only");
-  static constexpr KernelSel sel{/*wide*/ true, SMEM, G, EP, /*tds*/ false, /*tile*/ 1, NMAX, QM, FX, /*rec*/ false, /*res*/ false, SW};
-  using KParams = typename std::conditional<SW, SweepParams, Params>::type;
+  static_assert(!CT || !EP, "commit times: single-epoch kernels only");
+  static constexpr KernelSel sel{/*wide*/ true, SMEM, G, EP, /*tds*/ false, /*tile*/ 1, NMAX, QM, FX, /*rec*/ false, /*res*/ false, SW, CT};
+  using Base = typename std::conditional<SW, SweepParams, Params>::type;
+  using KParams = typename std::conditional<CT, CtParams<Base>, Base>::type;
   static bool try_launch(const KernelSel& k, const KParams& KP, cudaStream_t stream, cudaError_t& e) {
     if (!same_kernel(k, sel)) return false;
     const Params& P = params_of(KP);
@@ -238,7 +294,9 @@ struct WideKernel {
     const uint32_t blocks = (P.num_instances + kPerBlock - 1) / kPerBlock;
     const size_t dyn = (size_t)kPerBlock * wide_smem_words_per_group(P.L, QM, SMEM) * sizeof(uint32_t);
     void (*kernel)(KParams);
-    if constexpr (SW) kernel = lbft_sweep_wide_kernel<NMAX, QM, SMEM, G>;
+    if constexpr (CT && SW) kernel = lbft_ct_sweep_wide_kernel<NMAX, QM, SMEM, G>;
+    else if constexpr (CT) kernel = lbft_ct_wide_kernel<NMAX, QM, SMEM, G, FX>;
+    else if constexpr (SW) kernel = lbft_sweep_wide_kernel<NMAX, QM, SMEM, G>;
     else kernel = lbft_wide_kernel<NMAX, QM, SMEM, G, EP, FX>;
     e = dyn > 48 * 1024 ? allow_optin_smem(kernel, false) : cudaSuccess;  // (the wide kernel has no static shared memory)
     if (e == cudaSuccess) {
@@ -277,5 +335,11 @@ template <int NMAX, int QM>
 using SweepThread = ThreadKernel<NMAX, QM, FX_NONE, false, false, false, false, 32, true>;
 template <int NMAX, int QM>
 using SweepWideVariants = Kernels<WideKernel<NMAX, QM, false, 8, false, FX_NONE, true>, WideKernel<NMAX, QM, false, 32, false, FX_NONE, true>>;
+// The commit-times twins (k_ct_*.cu): of a full-tile generic thread kernel and of the two HBM lane groups of a generic wide
+// kernel, plain (SW = false) or sweep.
+template <int NMAX, int QM, bool SW>
+using CtThread = ThreadKernel<NMAX, QM, FX_NONE, false, false, false, false, 32, SW, true>;
+template <int NMAX, int QM, bool SW>
+using CtWideVariants = Kernels<WideKernel<NMAX, QM, false, 8, false, FX_NONE, SW, true>, WideKernel<NMAX, QM, false, 32, false, FX_NONE, SW, true>>;
 
 }  // namespace lbft

@@ -90,6 +90,9 @@ struct lbft_sim {
   size_t summary_bytes = 0;
   lbft_commit* d_logs = nullptr;  // lbft_commit_logs: [I][logs_cap], allocated on first use
   size_t logs_cap = 0;
+  int32_t* d_times = nullptr;    // LBFT_FLAG_COMMIT_TIMES: the commit-time table [I][N + 1][round_cap] (sim_core.cuh Core CT)
+  int64_t* d_times_out = nullptr;  // lbft_commit_times: [I][N][times_cap] committed, then [I][times_cap] proposed; on first use
+  size_t times_cap = 0;
   uint64_t device_bytes = 0;
   // pinned host staging: two seed buffers (lbft_set_seeds never writes the one an in-flight upload reads) and two
   // result sets (see HostResults)
@@ -122,6 +125,7 @@ static void free_all(lbft_sim* s) {
   cudaFree(s->d_period); cudaFree(s->d_weights); cudaFree(s->d_delay_thr); cudaFree(s->d_state); cudaFree(s->d_summary);
   cudaFree(s->d_lc_round); cudaFree(s->d_counters); cudaFree(s->d_status);
   cudaFree(s->d_error); cudaFree(s->d_logs); cudaFree(s->d_sets); cudaFree(s->d_set_of);
+  cudaFree(s->d_times); cudaFree(s->d_times_out);
   for (int b = 0; b < 2; b++) {
     cudaFreeHost(s->h_seeds[b]);
     HostResults& r = s->res[b];
@@ -297,6 +301,7 @@ static int create_on_device(lbft_sim* s, const lbft_config* config, lbft_sim** o
   CREATE_TRY(dev_alloc(s, &s->d_counters, I * 12));
   CREATE_TRY(dev_alloc(s, &s->d_status, I));
   CREATE_TRY(dev_alloc(s, &s->d_error, 1));
+  if (s->hs.sel.ct) CREATE_TRY(dev_alloc(s, &s->d_times, I * (N + 1) * L.round_cap));  // (never cleared: see Core CT)
   for (int b = 0; b < 2; b++) {
     HostResults& r = s->res[b];
     CREATE_TRY(cudaMallocHost((void**)&s->h_seeds[b], I * sizeof(uint64_t)));
@@ -458,7 +463,11 @@ static int enqueue_kernel(lbft_sim* s) {
   CUDA_TRY(cudaEventRecord(s->ev[2], s->stream));
   const KernelSel& k = s->hs.sel;
   const SweepParams sp{s->P, s->d_set_of, s->d_sets};
-  cudaError_t e = k.sweep ? (k.wide ? launch_sweep_wide(k, sp, s->stream) : launch_sweep_thread(k, sp, s->stream))
+  const CtParams<Params> cp{s->P, s->d_times};
+  const CtParams<SweepParams> csp{sp, s->d_times};
+  cudaError_t e = k.ct ? (k.sweep ? (k.wide ? launch_ct_sweep_wide(k, csp, s->stream) : launch_ct_sweep_thread(k, csp, s->stream))
+                                  : (k.wide ? launch_ct_wide(k, cp, s->stream) : launch_ct_thread(k, cp, s->stream)))
+                  : k.sweep ? (k.wide ? launch_sweep_wide(k, sp, s->stream) : launch_sweep_thread(k, sp, s->stream))
                   : k.wide ? launch_wide(k, s->P, s->stream)
                   : k.fixed == FX_DEFAULT4 ? launch_fixed(k, s->P, s->stream)
                   : (k.qmode == 1 || k.qmode == 2) ? launch_scan(k, s->P, s->stream)
@@ -639,6 +648,8 @@ int lbft_commit_log(lbft_sim* s, uint32_t instance, uint32_t node, lbft_commit* 
 // ancestor chain of its last committed block; the kernel lays out the LONGEST log of each instance in commit order
 // and verifies that every other node's last committed block lies on it at depth == its commit count (SURVEY App.
 // C.3).  Instances where that does not hold are counted in *bad.
+// The same walk, written once for the host and the device, is sim_core.cuh walk_commit_chain (lbft_commit_times); this kernel
+// keeps its own copy so that its code stays what it was before that function existed.  The two must walk alike.
 // ---------------------------------------------------------------------------------------------
 __global__ void lbft_commit_logs_kernel(const __grid_constant__ Params P, uint32_t stride, lbft_commit* out, uint32_t cap, uint32_t* bad) {
   const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
@@ -705,7 +716,56 @@ int lbft_commit_logs(lbft_sim* s, lbft_commit* out, size_t cap, uint32_t* lens) 
   return LBFT_OK;
 }
 
+// Bulk read-out of the commit-time table (LBFT_FLAG_COMMIT_TIMES), aligned with lbft_commit_logs: one thread per instance
+// walks its chain (sim_core.cuh commit_times_of).  Instances whose logs are not prefixes of one chain are counted in *bad.
+__global__ void lbft_commit_times_kernel(const __grid_constant__ Params P, uint32_t stride, const int32_t* times, uint32_t cap,
+                                         int64_t* committed, int64_t* proposed, uint32_t* bad) {
+  const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
+  if (inst >= P.num_instances) return;
+  const Layout& L = P.L;
+  const uint32_t N = L.num_nodes, tile = inst / stride, lane = inst % stride;
+  if (!commit_times_of(L, P.state + (size_t)tile * L.total_words * stride + lane, stride, P.out_commit_counts + (size_t)inst * N,
+                       P.out_lc_round + (size_t)inst * N, times + (size_t)inst * (N + 1) * L.round_cap, cap,
+                       committed + (size_t)inst * N * cap, proposed + (size_t)inst * cap))
+    atomicAdd(bad, 1u);
+}
+
 extern "C" {
+
+int lbft_commit_times(lbft_sim* s, int64_t* committed, int64_t* proposed, size_t cap) {
+  if (!s || !committed) return set_error(LBFT_ERR_INVALID, "sim and committed must not be NULL");
+  if (!s->hs.sel.ct) return set_error(LBFT_ERR_STATE, "commit times were not recorded: set LBFT_FLAG_COMMIT_TIMES in lbft_config.flags");
+  if (!s->downloaded) return set_error(LBFT_ERR_STATE, "results are not available: call lbft_run first");
+  if (cap == 0 || cap > 0xffffu) return set_error(LBFT_ERR_INVALID, "cap must be in 1..65535 rows per instance");
+  if (int r = need_idle(s)) return r;
+  CUDA_TRY(cudaSetDevice(s->device));
+  const size_t I = s->I, N = s->N;
+  if (cap > s->times_cap) {
+    cudaFree(s->d_times_out);
+    s->d_times_out = nullptr;
+    s->times_cap = 0;
+    cudaError_t e = cudaMalloc((void**)&s->d_times_out, I * (N + 1) * cap * sizeof(int64_t));
+    if (e != cudaSuccess) return set_error(LBFT_ERR_NOMEM, std::string("commit-time buffer: ") + cudaGetErrorString(e));
+    s->times_cap = cap;
+  }
+  int64_t* d_committed = s->d_times_out;
+  int64_t* d_proposed = s->d_times_out + I * N * cap;
+  CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
+  lbft_commit_times_kernel<<<(s->I + 127) / 128, 128, 0, s->stream>>>(s->P, s->stride, s->d_times, (uint32_t)cap, d_committed,
+                                                                        d_proposed, s->d_error);
+  CUDA_TRY(cudaGetLastError());
+  uint32_t bad = 0;
+  CUDA_TRY(cudaMemcpyAsync(committed, d_committed, I * N * cap * sizeof(int64_t), cudaMemcpyDeviceToHost, s->stream));
+  if (proposed) CUDA_TRY(cudaMemcpyAsync(proposed, d_proposed, I * cap * sizeof(int64_t), cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(&bad, s->d_error, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  if (bad) {
+    char buf[160];
+    snprintf(buf, sizeof buf, "%u instance(s) have node logs that are not prefixes of one chain: read them with lbft_commit_log", bad);
+    return set_error(LBFT_ERR_STATE, buf);
+  }
+  return LBFT_OK;
+}
 
 int lbft_round_switches(lbft_sim* s, uint32_t instance, lbft_round_switch* out, size_t cap, size_t* n) {
   if (!s || !n) return set_error(LBFT_ERR_INVALID, "NULL argument");

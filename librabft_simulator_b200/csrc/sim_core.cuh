@@ -124,6 +124,15 @@ LBFT_HD double bits_to_f64(uint64_t b) {
 #endif
 }
 LBFT_HD uint64_t rotl64(uint64_t x, int k) { return (x << k) | (x >> (64 - k)); }
+// A store that the kernel never reads back (the commit-time table, Core CT): evict-first, so that those lines do not push the
+// live instance state out of L2.
+LBFT_HD void st_evict_first(int32_t* p, int32_t v) {
+#if defined(__CUDA_ARCH__)
+  __stcs(p, v);
+#else
+  *p = v;
+#endif
+}
 
 // SipHash-1-3 with a zero key over a stream of u64 words (Rust DefaultHasher; the state key of
 // simulated_context.rs:51-55 only ever feeds whole 8-byte integers).
@@ -574,11 +583,16 @@ using QueueFor = typename std::conditional<QMODE == 0, HeapQueue<Mem, G>, typena
 // KS: (QMODE 3) the calendar's kind-occupancy words live in shared memory (CalendarQueue).
 // SW: a sweep handle (lbft_create_sweep) — the delay model and NodeConfig come from the instance's parameter set (bind_set)
 // instead of Params; every read of them goes through the accessors below.
+// CT: LBFT_FLAG_COMMIT_TIMES — propose_block and process_commits store the global clock into the instance's commit-time table
+// (ct, outside the instance state: [N + 1][round_cap] int32, row n = node n's commit of round r, row N = the proposal of
+// round r).  Nothing in the kernel reads the table back, and it is not cleared at init: the read-out (commit_times_of) only
+// reads rounds on a committed chain, which were proposed and committed in the same run.
 template <class Mem, int NMAX, int QMODE, int FX = 0, bool REC = false, bool RES = false, int G = 1, bool EP = false,
-          bool TDS = false, bool KS = false, bool SW = false>
+          bool TDS = false, bool KS = false, bool SW = false, bool CT = false>
 struct Core {
   static_assert(!KS || (QMODE == 3 && !RES && G == 1), "shared-memory occupancy words: calendar queue, one-shot thread kernels");
   static_assert(!SW || (FX == FX_NONE && !REC && !RES && !EP && !TDS), "sweeps: plain single-epoch generic kernels only");
+  static_assert(!CT || (!REC && !RES && !EP && !TDS), "commit times: one-shot single-epoch runs");
   static constexpr bool FIXED = FX != FX_NONE;                               // compile-time layout, reference delay model
   static constexpr bool MAY_SILENT = FX == FX_NONE || FX == FX_COMMITTEE64;  // silent nodes (extension D.2) reachable
   static_assert(!(FIXED && EP), "the compile-time layout is single-epoch");
@@ -609,6 +623,7 @@ struct Core {
   using Queue = QueueFor<QMODE, Mem, G, KS>;
   Queue q;                 // given its shared memory by the constructor (QMODE 2: sk / sd, or the host harness's stand-in) and init (km)
   uint32_t* km = nullptr;  // KS: the calendar's occupancy words in shared memory, a column per lane, set by the kernel
+  int32_t* ct = nullptr;   // CT: the instance's commit-time table, set by the kernel
   // ---- per-instance registers ----
   uint64_t s0, s1, s2, s3;  // Xoshiro256** (simulator.rs:32)
   uint32_t draws;
@@ -1110,6 +1125,11 @@ struct Core {
     m.st(L.chain_base + 2 * (d.gb + r) + 1, (uint32_t)clk);
     chain_cache_put(d.gb + r, prev_round);
     insert_block(d, r);
+    if constexpr (CT) stamp_commit_time(L.num_nodes, d.gb + r);
+  }
+  // CT: the global clock into row `row`, round `r` of the commit-time table (one lane per wide group)
+  LBFT_HD void stamp_commit_time(uint32_t row, uint32_t r) {
+    if (wl == 0) st_evict_first(ct + (size_t)row * L.round_cap + r, clock);
   }
   // create_vote :676-700
   LBFT_HD bool create_vote(NodeRegs& d, uint32_t n, uint32_t r, uint32_t prev) {
@@ -1120,7 +1140,7 @@ struct Core {
   }
   // process_commits node.rs:313-350 over committed_states_after record_store.rs:557-574 and
   // StateFinalizer::commit simulated_context.rs:161-185
-  LBFT_HD void process_commits(NodeRegs& d) {
+  LBFT_HD void process_commits(NodeRegs& d, uint32_t n) {
     uint32_t after = d.f[F_TRK_HCR];
     uint32_t top = d.f[F_HCC] ? d.f[F_HCR] : 0;
     while (top > after) {
@@ -1135,6 +1155,7 @@ struct Core {
       if (chain_parent(d.gb + q) != d.f[F_LC_ROUND]) status |= ST_INVARIANT;  // happened_just_before
       d.f[F_LC_ROUND] = d.gb + q;
       d.f[F_COMMITS]++;
+      if constexpr (CT) stamp_commit_time(n, d.gb + q);
       after = q;
       // "check if the current epoch just ended" (node.rs:327-347): read_epoch_id = executed commands / commands_per_epoch
       // (simulated_context.rs:199-207)
@@ -1268,7 +1289,7 @@ struct Core {
         a.next = clk;
       }
     }
-    process_commits(d);
+    process_commits(d, n);
     // ---- CommitTracker::update_tracker, node.rs:364-396
     bool trk_new_epoch = false;
     if (multi()) {  // "if current_epoch_id > self.epoch_id", node.rs:372-376
@@ -1864,5 +1885,52 @@ struct Core {
     }
   }
 };
+
+// The chain walk of the bulk read-outs (lbft_commit_logs, lbft_commit_times) over one instance.  A node's committed_history() is
+// the ancestor chain of its last committed block (every commit extends the previous one by exactly one block,
+// simulated_context.rs:172-174), so the walk starts from the last committed block of the instance's LONGEST log and calls
+// visit(k, r, c0) for row k = depth - 1, ..., 0 of that log, round r (a global round id) and r's chain word c0 (prev | cmd << 16).
+// tb: the instance's state word 0, its words `stride` apart; cc / lc: the instance's commit counts and last committed rounds.
+// Returns false unless every node's last committed block lies on that chain at depth == its commit count (SURVEY App. C.3):
+// the logs of the instance are then not prefixes of one chain.  (lbft_api.cu lbft_commit_logs_kernel keeps its own copy of this
+// walk; the two must stay alike.)
+template <class Visit>
+LBFT_HD bool walk_commit_chain(const Layout& L, const uint32_t* tb, uint32_t stride, const uint32_t* cc, const uint32_t* lc, Visit visit) {
+  const uint32_t N = L.num_nodes;
+  uint32_t best = 0;
+  for (uint32_t n = 1; n < N; n++)
+    if (cc[n] > cc[best]) best = n;
+  uint32_t k = cc[best], r = lc[best], matched = 0;
+  while (r != 0 && k > 0) {
+    for (uint32_t n = 0; n < N; n++)
+      if (cc[n] == k) matched += lc[n] == r ? 1u : 0x10000u;
+    --k;
+    const uint32_t c0 = tb[(size_t)(L.chain_base + 2 * r) * stride];
+    visit(k, r, c0);
+    // the parent; epochs > 1: the parent of an epoch's first block is the block whose state is the epoch's initial state
+    const uint32_t p = c0 & 0xffffu, ep = r / L.rspan;
+    r = p ? ep * L.rspan + p : (L.epochs > 1 ? tb[(size_t)(L.einit_base + ep) * stride] : 0u);
+  }
+  uint32_t empty = 0;
+  for (uint32_t n = 0; n < N; n++) empty += cc[n] == 0 ? (lc[n] == 0 ? 1u : 0x10000u) : 0u;
+  return r == 0 && k == 0 && matched + empty == N;
+}
+
+// lbft_commit_times for one instance: for row k of the logs (walk_commit_chain), round r's entries of the commit-time table
+// `times` (Core CT; single-epoch layouts, so r < round_cap).  committed: the instance's [N][cap] block, proposed: its [cap] row
+// or null — -1 wherever there is no entry.  Returns false when the logs of the instance are not prefixes of one chain.
+LBFT_HD bool commit_times_of(const Layout& L, const uint32_t* tb, uint32_t stride, const uint32_t* cc, const uint32_t* lc,
+                             const int32_t* times, uint32_t cap, int64_t* committed, int64_t* proposed) {
+  const uint32_t N = L.num_nodes;
+  for (size_t w = 0; w < (size_t)N * cap; w++) committed[w] = -1;
+  if (proposed)
+    for (uint32_t k = 0; k < cap; k++) proposed[k] = -1;
+  return walk_commit_chain(L, tb, stride, cc, lc, [&](uint32_t k, uint32_t r, uint32_t) {
+    if (k >= cap) return;
+    if (proposed) proposed[k] = times[(size_t)N * L.round_cap + r];
+    for (uint32_t n = 0; n < N; n++)
+      if (cc[n] > k) committed[(size_t)n * cap + k] = times[(size_t)n * L.round_cap + r];
+  });
+}
 
 }  // namespace lbft

@@ -85,6 +85,13 @@ class SimulatedContextView:
     def num_commits(self):
         return int(self._batch.commit_counts[self._instance, self.author])
 
+    def commit_times(self):
+        """Aligned with ``committed_history()``: ``(proposed, committed)`` global clocks per row — when the block was proposed
+        and when this node committed it (needs ``commit_times=True``; include/lbft.h lbft_commit_times)."""
+        n = self.num_commits()
+        committed, proposed = self._batch.commit_times()  # (the whole batch once per result, shared by its contexts)
+        return [(int(proposed[self._instance, k]), int(committed[self._instance, self.author, k])) for k in range(n)]
+
 
 class BatchResult:
     """Results of ``BatchSimulator.loop_until``: what the reference's callers read from ``Vec<&Context>``.
@@ -106,6 +113,7 @@ class BatchResult:
         self.active_rounds = sim._fetch("lbft_active_rounds", np.uint32, (I,))
         self.status = sim._fetch("lbft_status", np.uint32, (I,))
         self._counters = None
+        self._commit_times = {}  # cap -> (committed, proposed), read on first use
 
     @property
     def counters(self):
@@ -135,6 +143,23 @@ class BatchResult:
         self._check_current("commit logs")
         return self._sim.commit_logs(cap)
 
+    def commit_times(self, cap=None):
+        """Commit latency of the whole batch in one device pass (``lbft_commit_times``; needs ``commit_times=True``):
+        ``(committed[instance, node, cap], proposed[instance, cap])`` as int64 global clocks, aligned row for row with
+        ``commit_logs(cap)`` — ``committed[i, n, k]`` is when node n committed row k of its ``committed_history()``,
+        ``proposed[i, k]`` when row k of the instance's longest log was proposed; -1 past each log's end.  ``cap`` defaults to
+        the longest log of the batch.  Read from the handle once per ``cap``; the arrays are shared, do not modify them."""
+        cap = max(1, int(self.commit_counts.max())) if cap is None else int(cap)
+        if cap not in self._commit_times:
+            self._check_current("commit times")
+            self._commit_times[cap] = self._sim.commit_times(cap)
+        return self._commit_times[cap]
+
+    def commit_latencies(self, cap=None):
+        """``committed - proposed`` per ``[instance, node, row]`` (int64), -1 where the node committed nothing."""
+        committed, proposed = self.commit_times(cap)
+        return np.where(committed >= 0, committed - proposed[:, None, :], -1)
+
     def contexts(self, instance=0):
         """The ``Vec<&Context>`` that ``loop_until`` returns for one instance."""
         return [SimulatedContextView(self, instance, a) for a in range(self._sim.num_nodes)]
@@ -146,13 +171,15 @@ class BatchSimulator:
     def __init__(self, seeds, num_nodes, network_delay=RandomDelay(), node_config=NodeConfig(),
                  commands_per_epoch=30000, voting_rights=None, silent=None, partition_windows=0,
                  partition_max_len=0, device=0, round_cap=0, queue_cap=0, payload_cap=0, record_round_switches=False, resumable=False,
-                 true_data_sync=False):
+                 true_data_sync=False, commit_times=False):
         self._lib = _lib.load()
         self.record_round_switches = bool(record_round_switches)  # LBFT_FLAG_ROUND_SWITCHES (DataWriter, data_writer.rs)
         self.resumable = bool(resumable)  # LBFT_FLAG_RESUMABLE: run_until / snapshot / restore
         # LBFT_FLAG_TRUE_DATA_SYNC: NON-PARITY variant — requests are answered by the node they were sent to (the reference
         # simulator dispatches them to the requester itself, simulator.rs:446)
         self.true_data_sync = bool(true_data_sync)
+        # LBFT_FLAG_COMMIT_TIMES: record when each block is proposed and when each node commits it (commit_times())
+        self.commit_times_enabled = bool(commit_times)
         self.seeds = np.ascontiguousarray(np.asarray(seeds, dtype=np.uint64).reshape(-1))
         self.num_instances = int(self.seeds.shape[0])
         self.num_nodes = int(num_nodes)
@@ -184,7 +211,7 @@ class BatchSimulator:
         c.partition_windows, c.partition_max_len = self.partition_windows, self.partition_max_len
         c.device, c.round_cap, c.queue_cap, c.payload_cap = self.device, self.round_cap, self.queue_cap, self.payload_cap
         c.flags = ((_lib.FLAG_ROUND_SWITCHES if self.record_round_switches else 0) | (_lib.FLAG_RESUMABLE if self.resumable else 0) |
-                   (_lib.FLAG_TRUE_DATA_SYNC if self.true_data_sync else 0))
+                   (_lib.FLAG_TRUE_DATA_SYNC if self.true_data_sync else 0) | (_lib.FLAG_COMMIT_TIMES if self.commit_times_enabled else 0))
         return c
 
     def create(self, max_clock):
@@ -384,6 +411,17 @@ class BatchSimulator:
         rows = np.empty((self.num_instances, int(cap)), dtype=COMMIT_DTYPE)
         _lib.check(self._lib.lbft_commit_logs(self._handle, ctypes.c_void_p(rows.ctypes.data), int(cap), ctypes.c_void_p(lens.ctypes.data)))
         return rows, lens
+
+    def commit_times(self, cap=None):
+        """``lbft_commit_times``: ``(committed[instance, node, cap], proposed[instance, cap])``, int64 global clocks with -1
+        padding (see ``BatchResult.commit_times``); ``cap`` defaults to the longest log of the batch."""
+        if cap is None:
+            cap = max(1, int(self._fetch("lbft_commit_counts", np.uint32, (self.num_instances, self.num_nodes)).max()))
+        committed = np.empty((self.num_instances, self.num_nodes, int(cap)), dtype=np.int64)
+        proposed = np.empty((self.num_instances, int(cap)), dtype=np.int64)
+        _lib.check(self._lib.lbft_commit_times(self._handle, ctypes.c_void_p(committed.ctypes.data), ctypes.c_void_p(proposed.ctypes.data),
+                                               int(cap)))
+        return committed, proposed
 
     def round_switches(self, instance):
         """``DataWriter::nodes_round_switch`` of one instance as ``[(node, round, time)]``, node-major
