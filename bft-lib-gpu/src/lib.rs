@@ -100,6 +100,35 @@ pub mod ffi {
         pub timers_elided: u32,
     }
 
+    /// include/lbft.h `lbft_latency_spec`: the histogram and proposal-time window of `lbft_latency_stats`
+    #[repr(C)]
+    #[derive(Clone, Copy, Debug, PartialEq)]
+    pub struct LbftLatencySpec {
+        pub struct_size: u32,
+        pub num_bins: u32,
+        pub bin_width: i64,
+        pub proposed_from: i64,
+        pub proposed_until: i64,
+    }
+    /// The header's spelling of `LbftLatencySpec`, as the `extern "C"` block names it.
+    #[allow(non_camel_case_types)]
+    pub type lbft_latency_spec = LbftLatencySpec;
+
+    /// include/lbft.h `lbft_latency_summary`: one group's commit-latency statistics (`min` / `max` are -1 when `samples == 0`)
+    #[repr(C)]
+    #[derive(Clone, Copy, Default, Debug, PartialEq)]
+    pub struct LbftLatencySummary {
+        pub instances: u64,
+        pub excluded: u64,
+        pub samples: u64,
+        pub sum: u64,
+        pub min: i64,
+        pub max: i64,
+    }
+    /// The header's spelling of `LbftLatencySummary`, as the `extern "C"` block names it.
+    #[allow(non_camel_case_types)]
+    pub type lbft_latency_summary = LbftLatencySummary;
+
     pub const LBFT_OK: c_int = 0;
     pub const LBFT_ERR_CAPACITY: c_int = -4;
     pub const LBFT_FLAG_ROUND_SWITCHES: u32 = 1;
@@ -130,6 +159,7 @@ pub mod ffi {
         pub fn lbft_commit_log(sim: *mut LbftSim, instance: u32, node: u32, out: *mut LbftCommit, cap: usize, n: *mut usize) -> c_int;
         pub fn lbft_commit_logs(sim: *mut LbftSim, out: *mut LbftCommit, cap: usize, lens: *mut u32) -> c_int;
         pub fn lbft_commit_times(sim: *mut LbftSim, committed: *mut i64, proposed: *mut i64, cap: usize) -> c_int;
+        pub fn lbft_latency_stats(sim: *mut LbftSim, spec: *const lbft_latency_spec, out: *mut lbft_latency_summary, hist: *mut u64) -> c_int;
         pub fn lbft_round_switches(sim: *mut LbftSim, instance: u32, out: *mut LbftRoundSwitch, cap: usize, n: *mut usize) -> c_int;
         pub fn lbft_snapshot_size(sim: *mut LbftSim, bytes: *mut usize) -> c_int;
         pub fn lbft_snapshot_save(sim: *mut LbftSim, buf: *mut u8, cap: usize) -> c_int;
@@ -182,6 +212,7 @@ pub struct GpuSimulator {
     horizon: Option<i64>,
     devices: Vec<i32>,
     record_round_switches: bool,
+    commit_times: bool,
     shards: Vec<Shard>,
 }
 
@@ -204,8 +235,15 @@ impl GpuSimulator {
             horizon: None,
             devices: vec![0],
             record_round_switches: false,
+            commit_times: false,
             shards: Vec::new(),
         }
+    }
+
+    /// Record when each block is proposed and when each node commits it (`LBFT_FLAG_COMMIT_TIMES`), for `latency_stats`.
+    pub fn with_commit_times(mut self) -> Self {
+        self.commit_times = true;
+        self
     }
 
     /// Shard the batch over these CUDA devices (contiguous instance ranges, no data-path communication); one host
@@ -233,6 +271,9 @@ impl GpuSimulator {
             }
             if self.record_round_switches {
                 flags |= ffi::LBFT_FLAG_ROUND_SWITCHES;
+            }
+            if self.commit_times {
+                flags |= ffi::LBFT_FLAG_COMMIT_TIMES;
             }
             let c = ffi::LbftConfig {
                 struct_size: std::mem::size_of::<ffi::LbftConfig>() as u32,
@@ -352,6 +393,42 @@ impl GpuSimulator {
             }
         }
         (rows, lens)
+    }
+
+    /// Commit-latency statistics of the whole batch (`lbft_latency_stats`; build the simulator `with_commit_times()`), reduced
+    /// on each GPU and merged over them: the summary and `num_bins` histogram counts, bin b holding latencies in
+    /// `[b * bin_width, (b + 1) * bin_width)` and the last bin everything above.  Only rows proposed in
+    /// `[proposed_from, proposed_until)` count.
+    pub fn latency_stats(&self, num_bins: u32, bin_width: i64, proposed_from: i64, proposed_until: i64) -> (ffi::LbftLatencySummary, Vec<u64>) {
+        let spec = ffi::LbftLatencySpec {
+            struct_size: std::mem::size_of::<ffi::LbftLatencySpec>() as u32,
+            num_bins,
+            bin_width,
+            proposed_from,
+            proposed_until,
+        };
+        let mut total = ffi::LbftLatencySummary { min: i64::MAX, max: -1, ..Default::default() };
+        let mut hist = vec![0u64; num_bins as usize];
+        for s in &self.shards {
+            let mut part = ffi::LbftLatencySummary::default();
+            let mut h = vec![0u64; num_bins as usize];
+            check(unsafe { ffi::lbft_latency_stats(s.sim, &spec, &mut part, h.as_mut_ptr()) }, "lbft_latency_stats");
+            total.instances += part.instances;
+            total.excluded += part.excluded;
+            total.samples += part.samples;
+            total.sum += part.sum;
+            if part.samples > 0 {
+                total.min = total.min.min(part.min);
+                total.max = total.max.max(part.max);
+            }
+            for (a, b) in hist.iter_mut().zip(h) {
+                *a += b;
+            }
+        }
+        if total.samples == 0 {
+            total.min = -1;
+        }
+        (total, hist)
     }
 }
 

@@ -263,6 +263,35 @@ void lbft_destroy(lbft_sim* sim);
 const char* lbft_last_error(void);
 uint32_t lbft_abi_version(void);
 
+/* Commit-latency statistics (lbft_latency_stats).  A sample is one latency committed - proposed of row k of node n's
+ * committed_history(), with the times of lbft_commit_times; it counts when the row's proposed time p lies in
+ * [proposed_from, proposed_until).  Bin b of a histogram counts latencies in [b * bin_width, (b + 1) * bin_width); the last
+ * bin also counts every latency above it. */
+typedef struct lbft_latency_spec {
+  uint32_t struct_size;           /* = sizeof(lbft_latency_spec)                                       */
+  uint32_t num_bins;              /* 1..65536                                                          */
+  int64_t bin_width;              /* >= 1 (ms of global clock)                                         */
+  int64_t proposed_from, proposed_until;  /* window on the proposed time, from <= until                */
+} lbft_latency_spec;
+
+/* One group's statistics: instances without an error bit, instances with one (LBFT_ST_ERROR_MASK: they add nothing), the
+ * number of samples, their sum, and their minimum and maximum (-1 when samples == 0). */
+typedef struct lbft_latency_summary {
+  uint64_t instances, excluded, samples, sum;
+  int64_t min, max;
+} lbft_latency_summary;
+
+/* Commit-latency statistics of the last run (needs LBFT_FLAG_COMMIT_TIMES), reduced on the device per group: a parameter set
+ * of a sweep handle (num_sets groups, instance i in group set_of_instance[i]) or the whole batch of a plain handle (one
+ * group).  out[num_groups]; hist[group * num_bins + b], or NULL (then not copied).  Every row of every log counts (there is no
+ * cap), and every value is an exact integer that does not depend on launch shape.  The chain of an instance with an error
+ * bit is not walked.  LBFT_ERR_STATE without the flag, before a run has finished, while an lbft_run_async is in flight, or
+ * when the logs of an instance without an error bit are not prefixes of one chain; LBFT_ERR_INVALID for NULL sim / spec /
+ * out, a wrong struct_size, num_bins outside 1..65536, bin_width < 1, proposed_from > proposed_until,
+ * num_groups * num_bins > 2^24, or a handle whose num_instances * num_nodes * round_cap * max_clock does not fit in 64 bits
+ * (the bound on sum). */
+int lbft_latency_stats(lbft_sim* sim, const lbft_latency_spec* spec, lbft_latency_summary* out, uint64_t* hist);
+
 #ifdef __cplusplus
 }
 #endif

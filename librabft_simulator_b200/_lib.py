@@ -41,6 +41,17 @@ class LbftRoundSwitch(ctypes.Structure):
     _fields_ = [("node", c_u32), ("round", c_u32), ("time", c_i64)]
 
 
+class LbftLatencySpec(ctypes.Structure):
+    """include/lbft.h lbft_latency_spec: the histogram and window of ``lbft_latency_stats``."""
+    _fields_ = [("struct_size", c_u32), ("num_bins", c_u32), ("bin_width", c_i64), ("proposed_from", c_i64),
+                ("proposed_until", c_i64)]
+
+
+class LbftLatencySummary(ctypes.Structure):
+    """include/lbft.h lbft_latency_summary: one group's statistics."""
+    _fields_ = [("instances", c_u64), ("excluded", c_u64), ("samples", c_u64), ("sum", c_u64), ("min", c_i64), ("max", c_i64)]
+
+
 FLAG_ROUND_SWITCHES = 1  # LBFT_FLAG_ROUND_SWITCHES
 FLAG_RESUMABLE = 2  # LBFT_FLAG_RESUMABLE
 FLAG_TRUE_DATA_SYNC = 4  # LBFT_FLAG_TRUE_DATA_SYNC (non-parity variant)
@@ -59,7 +70,7 @@ ST_INVARIANT, ST_EPOCH_CHANGE, ST_DELAY_NEAR_INT, ST_TIME_OVERFLOW = 16, 32, 64,
 ST_ERROR_MASK = ST_ROUND_OVERFLOW | ST_QUEUE_OVERFLOW | ST_PAYLOAD_OVERFLOW | ST_INVARIANT | ST_TIME_OVERFLOW
 
 EXPORTS = [
-    "lbft_create", "lbft_create_sweep", "lbft_run", "lbft_run_async", "lbft_wait", "lbft_commit_logs", "lbft_commit_times", "lbft_upload", "lbft_run_device", "lbft_download", "lbft_commit_counts",
+    "lbft_create", "lbft_create_sweep", "lbft_run", "lbft_run_async", "lbft_wait", "lbft_commit_logs", "lbft_commit_times", "lbft_latency_stats", "lbft_upload", "lbft_run_device", "lbft_download", "lbft_commit_counts",
     "lbft_last_states", "lbft_commit_log", "lbft_round_switches", "lbft_active_rounds", "lbft_counters", "lbft_status", "lbft_timing_info",
     "lbft_memory_info", "lbft_kernel_info", "lbft_run_until", "lbft_snapshot_size", "lbft_snapshot_save", "lbft_snapshot_load", "lbft_set_seeds", "lbft_device_buffer", "lbft_destroy", "lbft_last_error", "lbft_abi_version",
 ]
@@ -93,6 +104,7 @@ def load():
     lib.lbft_commit_log.argtypes = [P, c_u32, c_u32, ctypes.POINTER(LbftCommit), ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)]
     lib.lbft_commit_logs.argtypes = [P, P, ctypes.c_size_t, P]
     lib.lbft_commit_times.argtypes = [P, P, P, ctypes.c_size_t]
+    lib.lbft_latency_stats.argtypes = [P, ctypes.POINTER(LbftLatencySpec), P, P]
     lib.lbft_round_switches.argtypes = [P, c_u32, ctypes.POINTER(LbftRoundSwitch), ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)]
     lib.lbft_timing_info.argtypes = [P, ctypes.POINTER(LbftTiming)]
     lib.lbft_run_until.argtypes = [P, c_i64]

@@ -538,4 +538,19 @@ struct HostSetup {
   }
 };
 
+// lbft_latency_stats: the groups of a handle (its parameter sets, or one), and the checks on its spec (null when it is valid).
+inline uint32_t latency_groups(const HostSetup& hs) { return hs.sets.empty() ? 1u : (uint32_t)hs.sets.size(); }
+inline const char* latency_spec_error(const HostSetup& hs, const lbft_latency_spec& spec) {
+  if (spec.struct_size != sizeof(lbft_latency_spec)) return "lbft_latency_spec.struct_size does not match this library (ABI mismatch)";
+  if (spec.num_bins < 1 || spec.num_bins > 65536u) return "num_bins must be in 1..65536";
+  if (spec.bin_width < 1) return "bin_width must be >= 1";
+  if (spec.proposed_from > spec.proposed_until) return "proposed_from must be <= proposed_until";
+  if ((uint64_t)latency_groups(hs) * spec.num_bins > (1u << 24)) return "num_groups * num_bins must be <= 2^24";
+  // every sample is at most max_clock and an instance has fewer than round_cap rows per node: this bounds sum
+  const Params& p = hs.params;
+  const unsigned __int128 bound = (unsigned __int128)p.num_instances * p.L.num_nodes * p.L.round_cap * (uint64_t)p.max_clock;
+  if (bound >> 64) return "num_instances * num_nodes * round_cap * max_clock must fit in 64 bits (the bound on sum)";
+  return nullptr;
+}
+
 }  // namespace lbft

@@ -27,6 +27,7 @@ static_assert(LBFT_SAME(ST_DONE, LBFT_ST_DONE) && LBFT_SAME(ST_ROUND_OVERFLOW, L
                   LBFT_SAME(ST_DELAY_NEAR_INT, LBFT_ST_DELAY_NEAR_INT) && LBFT_SAME(ST_TIME_OVERFLOW, LBFT_ST_TIME_OVERFLOW),
               "status bits out of sync with include/lbft.h");
 static_assert(sizeof(lbft_instance_counters) == 12 * sizeof(uint32_t), "counter layout");
+static_assert(sizeof(lbft_latency_summary) == 6 * sizeof(uint64_t), "latency summary layout (64-bit atomics on every field)");
 static_assert(LBFT_SAME(ST_ERROR_BITS, LBFT_ST_ERROR_MASK), "error mask out of sync with include/lbft.h");
 
 // ---------------------------------------------------------------------------------------------
@@ -93,6 +94,8 @@ struct lbft_sim {
   int32_t* d_times = nullptr;    // LBFT_FLAG_COMMIT_TIMES: the commit-time table [I][N + 1][round_cap] (sim_core.cuh Core CT)
   int64_t* d_times_out = nullptr;  // lbft_commit_times: [I][N][times_cap] committed, then [I][times_cap] proposed; on first use
   size_t times_cap = 0;
+  unsigned char* d_lat = nullptr;  // lbft_latency_stats: [groups] summaries, then [groups][num_bins] u64 bins; on first use
+  size_t lat_bytes = 0;
   uint64_t device_bytes = 0;
   // pinned host staging: two seed buffers (lbft_set_seeds never writes the one an in-flight upload reads) and two
   // result sets (see HostResults)
@@ -125,7 +128,7 @@ static void free_all(lbft_sim* s) {
   cudaFree(s->d_period); cudaFree(s->d_weights); cudaFree(s->d_delay_thr); cudaFree(s->d_state); cudaFree(s->d_summary);
   cudaFree(s->d_lc_round); cudaFree(s->d_counters); cudaFree(s->d_status);
   cudaFree(s->d_error); cudaFree(s->d_logs); cudaFree(s->d_sets); cudaFree(s->d_set_of);
-  cudaFree(s->d_times); cudaFree(s->d_times_out);
+  cudaFree(s->d_times); cudaFree(s->d_times_out); cudaFree(s->d_lat);
   for (int b = 0; b < 2; b++) {
     cudaFreeHost(s->h_seeds[b]);
     HostResults& r = s->res[b];
@@ -730,6 +733,93 @@ __global__ void lbft_commit_times_kernel(const __grid_constant__ Params P, uint3
     atomicAdd(bad, 1u);
 }
 
+// lbft_latency_stats: the accumulators before the reduction — every field 0, min INT64_MAX (turned into -1 for an empty group on
+// the host), max -1.
+__global__ void lbft_latency_init_kernel(lbft_latency_summary* sum, uint32_t groups, unsigned long long* hist, size_t hist_len) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < hist_len || i < groups; i += (size_t)gridDim.x * blockDim.x) {
+    if (i < groups) sum[i] = lbft_latency_summary{0, 0, 0, 0, INT64_MAX, -1};
+    if (i < hist_len) hist[i] = 0;
+  }
+}
+
+// Per-group commit-latency statistics: one thread per instance walks its chain (sim_core.cuh latency_samples_of) unless its
+// status has an error bit.  Integer atomics only, so every value is exact and independent of launch shape and atomic order.
+// The kernel picks its path from what it sees:
+//  * all instances of the block in one group (a plain handle, or a sweep laid out set by set as SweepSimulator.grid does) and
+//    num_bins <= kLatSharedBins: the histogram is built in shared memory (u32: a block holds at most 128 instances x 64 nodes x
+//    32 768 rows = 2^28 samples) and added to the group's with one atomic per non-zero bin;
+//  * otherwise every sample adds to its group's histogram in global memory.
+// The summary fields are summed over each warp whose lanes share a group (shuffles, then one atomic per field), else per thread.
+constexpr uint32_t kLatSharedBins = 8192;
+constexpr uint32_t kLatBlock = 128;
+__global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __grid_constant__ Params P, uint32_t stride,
+                                                                       const int32_t* times, const uint32_t* set_of, int64_t width,
+                                                                       uint32_t bins, int64_t from, int64_t until,
+                                                                       lbft_latency_summary* sum, unsigned long long* hist,
+                                                                       uint32_t* bad) {
+  extern __shared__ uint32_t sh_bins[];
+  const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool live = inst < P.num_instances;
+  const uint32_t g0 = set_of ? set_of[blockIdx.x * blockDim.x] : 0u;
+  const uint32_t g = live && set_of ? set_of[inst] : g0;
+  const bool shared_hist = __syncthreads_and(g == g0) && bins <= kLatSharedBins;
+  if (shared_hist) {
+    for (uint32_t b = threadIdx.x; b < bins; b += blockDim.x) sh_bins[b] = 0;
+    __syncthreads();
+  }
+  unsigned long long clean = 0, excluded = 0, samples = 0, total = 0;
+  long long lo = INT64_MAX, hi = -1;
+  if (live) {
+    if (P.out_status[inst] & ST_ERROR_BITS) {
+      excluded = 1;
+    } else {
+      clean = 1;
+      const Layout& L = P.L;
+      const uint32_t N = L.num_nodes, tile = inst / stride, lane = inst % stride;
+      unsigned long long* gh = hist + (size_t)g * bins;
+      const bool ok = latency_samples_of(L, P.state + (size_t)tile * L.total_words * stride + lane, stride,
+                                         P.out_commit_counts + (size_t)inst * N, P.out_lc_round + (size_t)inst * N,
+                                         times + (size_t)inst * (N + 1) * L.round_cap, from, until, [&](int64_t lat) {
+                                           samples++;
+                                           total += (unsigned long long)lat;
+                                           lo = lat < lo ? lat : lo;
+                                           hi = lat > hi ? lat : hi;
+                                           const uint32_t b = latency_bin(lat, width, bins);
+                                           if (shared_hist) atomicAdd(&sh_bins[b], 1u);
+                                           else atomicAdd(&gh[b], 1ull);
+                                         });
+      if (!ok) atomicAdd(bad, 1u);
+    }
+  }
+  lbft_latency_summary* gs = sum + g;
+  const uint32_t full = 0xffffffffu;
+  if (__all_sync(full, g == __shfl_sync(full, g, 0))) {
+    for (int o = 16; o > 0; o >>= 1) {
+      clean += __shfl_down_sync(full, clean, o);
+      excluded += __shfl_down_sync(full, excluded, o);
+      samples += __shfl_down_sync(full, samples, o);
+      total += __shfl_down_sync(full, total, o);
+      lo = min(lo, __shfl_down_sync(full, lo, o));
+      hi = max(hi, __shfl_down_sync(full, hi, o));
+    }
+    if ((threadIdx.x & 31) != 0) clean = excluded = samples = 0;  // (lane 0 holds the warp's totals)
+  }
+  if (clean) atomicAdd((unsigned long long*)&gs->instances, clean);
+  if (excluded) atomicAdd((unsigned long long*)&gs->excluded, excluded);
+  if (samples) {
+    atomicAdd((unsigned long long*)&gs->samples, samples);
+    atomicAdd((unsigned long long*)&gs->sum, total);
+    atomicMin((long long*)&gs->min, lo);
+    atomicMax((long long*)&gs->max, hi);
+  }
+  if (shared_hist) {
+    __syncthreads();
+    unsigned long long* gh = hist + (size_t)g0 * bins;
+    for (uint32_t b = threadIdx.x; b < bins; b += blockDim.x)
+      if (sh_bins[b]) atomicAdd(&gh[b], (unsigned long long)sh_bins[b]);
+  }
+}
+
 extern "C" {
 
 int lbft_commit_times(lbft_sim* s, int64_t* committed, int64_t* proposed, size_t cap) {
@@ -764,6 +854,50 @@ int lbft_commit_times(lbft_sim* s, int64_t* committed, int64_t* proposed, size_t
     snprintf(buf, sizeof buf, "%u instance(s) have node logs that are not prefixes of one chain: read them with lbft_commit_log", bad);
     return set_error(LBFT_ERR_STATE, buf);
   }
+  return LBFT_OK;
+}
+
+int lbft_latency_stats(lbft_sim* s, const lbft_latency_spec* spec, lbft_latency_summary* out, uint64_t* hist) {
+  if (!s || !spec || !out) return set_error(LBFT_ERR_INVALID, "sim, spec and out must not be NULL");
+  if (!s->hs.sel.ct) return set_error(LBFT_ERR_STATE, "commit times were not recorded: set LBFT_FLAG_COMMIT_TIMES in lbft_config.flags");
+  if (!s->downloaded) return set_error(LBFT_ERR_STATE, "results are not available: call lbft_run first");
+  if (const char* e = latency_spec_error(s->hs, *spec)) return set_error(LBFT_ERR_INVALID, e);
+  if (int r = need_idle(s)) return r;
+  CUDA_TRY(cudaSetDevice(s->device));
+  const uint32_t groups = latency_groups(s->hs), bins = spec->num_bins;
+  const size_t hist_len = (size_t)groups * bins;
+  const size_t bytes = groups * sizeof(lbft_latency_summary) + hist_len * sizeof(uint64_t);
+  if (bytes > s->lat_bytes) {
+    cudaFree(s->d_lat);
+    s->d_lat = nullptr;
+    s->lat_bytes = 0;
+    cudaError_t e = cudaMalloc((void**)&s->d_lat, bytes);
+    if (e != cudaSuccess) return set_error(LBFT_ERR_NOMEM, std::string("latency-statistics buffer: ") + cudaGetErrorString(e));
+    s->lat_bytes = bytes;
+  }
+  lbft_latency_summary* d_sum = reinterpret_cast<lbft_latency_summary*>(s->d_lat);
+  unsigned long long* d_hist = reinterpret_cast<unsigned long long*>(s->d_lat + groups * sizeof(lbft_latency_summary));
+  const size_t init_blocks = ((hist_len > groups ? hist_len : groups) + 255) / 256;
+  lbft_latency_init_kernel<<<(unsigned)(init_blocks < 4096 ? init_blocks : 4096), 256, 0, s->stream>>>(d_sum, groups, d_hist, hist_len);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
+  const size_t smem = bins <= kLatSharedBins ? bins * sizeof(uint32_t) : 0;
+  lbft_latency_stats_kernel<<<(s->I + kLatBlock - 1) / kLatBlock, kLatBlock, smem, s->stream>>>(
+      s->P, s->stride, s->d_times, s->hs.sel.sweep ? s->d_set_of : nullptr, spec->bin_width, bins, spec->proposed_from,
+      spec->proposed_until, d_sum, d_hist, s->d_error);
+  CUDA_TRY(cudaGetLastError());
+  uint32_t bad = 0;
+  CUDA_TRY(cudaMemcpyAsync(out, d_sum, groups * sizeof(lbft_latency_summary), cudaMemcpyDeviceToHost, s->stream));
+  if (hist) CUDA_TRY(cudaMemcpyAsync(hist, d_hist, hist_len * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(&bad, s->d_error, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  if (bad) {
+    char buf[160];
+    snprintf(buf, sizeof buf, "%u instance(s) have node logs that are not prefixes of one chain: read them with lbft_commit_log", bad);
+    return set_error(LBFT_ERR_STATE, buf);
+  }
+  for (uint32_t g = 0; g < groups; g++)
+    if (out[g].samples == 0) out[g].min = -1;
   return LBFT_OK;
 }
 

@@ -1933,4 +1933,28 @@ LBFT_HD bool commit_times_of(const Layout& L, const uint32_t* tb, uint32_t strid
   });
 }
 
+// lbft_latency_stats for one instance: visit(latency) for every sample, i.e. committed - proposed of row k of every node that
+// committed it (every row: there is no cap), for the rows whose proposed time p has from <= p < until.  The arguments are those
+// of commit_times_of.  Returns false when the logs of the instance are not prefixes of one chain.
+template <class Visit>
+LBFT_HD bool latency_samples_of(const Layout& L, const uint32_t* tb, uint32_t stride, const uint32_t* cc, const uint32_t* lc,
+                                const int32_t* times, int64_t from, int64_t until, Visit visit) {
+  const uint32_t N = L.num_nodes;
+  return walk_commit_chain(L, tb, stride, cc, lc, [&](uint32_t k, uint32_t r, uint32_t) {
+    const int64_t p = times[(size_t)N * L.round_cap + r];
+    if (p < from || p >= until) return;
+    for (uint32_t n = 0; n < N; n++)
+      if (cc[n] > k) visit((int64_t)times[(size_t)n * L.round_cap + r] - p);
+  });
+}
+
+// The histogram bin of a latency: [b * w, (b + 1) * w) for b < bins - 1, the last bin also counting everything above.  (A
+// commit is never earlier than its proposal; the clamp at 0 only keeps the index inside the histogram.)
+LBFT_HD uint32_t latency_bin(int64_t lat, int64_t w, uint32_t bins) {
+  if (lat < w) return 0;
+  // a latency is the difference of two int32 clocks, so w <= lat < 2^32 here and a 32-bit division is exact
+  const uint32_t b = (uint32_t)lat / (uint32_t)w;
+  return b >= bins - 1 ? bins - 1 : b;
+}
+
 }  // namespace lbft

@@ -15,6 +15,7 @@ simulation work happens in the CUDA library; this module only marshals arguments
 import ctypes
 import os
 from dataclasses import dataclass
+from fractions import Fraction
 
 import numpy as np
 
@@ -23,6 +24,44 @@ from . import _lib
 DELAY_LOGNORMAL, DELAY_UNIFORM = 0, 1
 # one row of committed_history(): include/lbft.h lbft_commit
 COMMIT_DTYPE = np.dtype([("proposer", np.uint32), ("index", np.uint32), ("time", np.int64)])
+# one group's commit-latency statistics: include/lbft.h lbft_latency_summary
+LATENCY_SUMMARY_DTYPE = np.dtype([("instances", np.uint64), ("excluded", np.uint64), ("samples", np.uint64), ("sum", np.uint64),
+                                  ("min", np.int64), ("max", np.int64)])
+
+
+class LatencyStats:
+    """Commit-latency statistics per group (``BatchResult.latency_stats``), every value an exact integer: arrays
+    ``instances`` (clean instances), ``excluded`` (instances with an error bit), ``samples``, ``sum``, ``min`` and ``max``
+    (-1 for an empty group) of shape ``[groups]``, and ``hist[groups, num_bins]``, where bin b counts the latencies in
+    ``[b * bin_width, (b + 1) * bin_width)`` and the last bin also every latency above it."""
+
+    def __init__(self, summary, hist, bin_width):
+        for f in LATENCY_SUMMARY_DTYPE.names:
+            setattr(self, f, np.ascontiguousarray(summary[f]))
+        self.hist = hist
+        self.bin_width = int(bin_width)
+        self.num_bins = hist.shape[1]
+
+    def mean(self):
+        """Mean latency per group (float64), nan where a group has no samples."""
+        with np.errstate(invalid="ignore", divide="ignore"):
+            return np.where(self.samples > 0, self.sum.astype(np.float64) / self.samples, np.nan)
+
+    def percentile(self, q):
+        """The q-th percentile (0 <= q <= 100) per group: the lower edge ``b * bin_width`` of the first bin whose cumulative
+        count reaches rank ``max(1, ceil(q * samples / 100))``, with the rank computed exactly; +inf when that bin is the
+        last (it holds every latency above), nan for an empty group.  With ``bin_width = 1`` and an empty last bin this is
+        ``np.percentile(latencies, q, method="inverted_cdf")``."""
+        qf = Fraction(q)
+        if not 0 <= qf <= 100:
+            raise ValueError("q must be in [0, 100]")
+        n = self.samples.astype(object)
+        rank = np.maximum(1, -((-(n * qf.numerator)) // (100 * qf.denominator))).astype(np.uint64)  # ceil, in Python ints
+        b = (np.cumsum(self.hist, axis=1) < rank[:, None]).sum(axis=1)
+        out = b.astype(np.float64) * self.bin_width
+        out[b >= self.num_bins - 1] = np.inf
+        out[self.samples == 0] = np.nan
+        return out
 
 
 @dataclass(frozen=True)
@@ -159,6 +198,15 @@ class BatchResult:
         """``committed - proposed`` per ``[instance, node, row]`` (int64), -1 where the node committed nothing."""
         committed, proposed = self.commit_times(cap)
         return np.where(committed >= 0, committed - proposed[:, None, :], -1)
+
+    def latency_stats(self, num_bins=1024, bin_width=1, proposed_from=0, proposed_until=None):
+        """Commit-latency statistics per group, reduced on the device (``lbft_latency_stats``; needs ``commit_times=True``): a
+        group is a parameter set of a sweep (``param_sets`` order) or the whole batch of a plain simulator.  The samples are
+        the non-negative entries of ``commit_latencies()`` at full cap whose row was proposed in ``[proposed_from,
+        proposed_until)`` (``None``: no upper bound); instances with an error bit in ``status`` add nothing and are counted
+        in ``excluded``.  Returns a ``LatencyStats``."""
+        self._check_current("latency statistics")
+        return self._sim.latency_stats(num_bins, bin_width, proposed_from, proposed_until)
 
     def contexts(self, instance=0):
         """The ``Vec<&Context>`` that ``loop_until`` returns for one instance."""
@@ -422,6 +470,20 @@ class BatchSimulator:
         _lib.check(self._lib.lbft_commit_times(self._handle, ctypes.c_void_p(committed.ctypes.data), ctypes.c_void_p(proposed.ctypes.data),
                                                int(cap)))
         return committed, proposed
+
+    def latency_stats(self, num_bins=1024, bin_width=1, proposed_from=0, proposed_until=None):
+        """``lbft_latency_stats``: per-group commit-latency statistics as a ``LatencyStats`` (see
+        ``BatchResult.latency_stats``)."""
+        spec = _lib.LbftLatencySpec(struct_size=ctypes.sizeof(_lib.LbftLatencySpec), num_bins=int(num_bins), bin_width=int(bin_width),
+                                    proposed_from=int(proposed_from),
+                                    proposed_until=np.iinfo(np.int64).max if proposed_until is None else int(proposed_until))
+        groups = len(self.param_sets) if isinstance(self, SweepSimulator) else 1
+        summary = np.zeros(groups, dtype=LATENCY_SUMMARY_DTYPE)
+        # (a histogram the library refuses, num_bins out of range or num_groups * num_bins > 2^24, is not allocated here)
+        hist = np.zeros((groups, spec.num_bins if 1 <= spec.num_bins and groups * spec.num_bins <= 1 << 24 else 0), dtype=np.uint64)
+        _lib.check(self._lib.lbft_latency_stats(self._handle, ctypes.byref(spec), ctypes.c_void_p(summary.ctypes.data),
+                                                ctypes.c_void_p(hist.ctypes.data) if hist.size else None))
+        return LatencyStats(summary, hist, spec.bin_width)
 
     def round_switches(self, instance):
         """``DataWriter::nodes_round_switch`` of one instance as ``[(node, round, time)]``, node-major
