@@ -67,6 +67,19 @@ pub mod ffi {
     #[allow(non_camel_case_types)]
     pub type lbft_param_set = LbftParamSet;
 
+    /// include/lbft.h `lbft_fault_set`: the fault model of one parameter set of a fault sweep (`lbft_create_sweep_faults`) —
+    /// bit n of `silent_mask` makes node n silent; the partition plan as `LbftConfig::partition_windows` / `partition_max_len`
+    #[repr(C)]
+    #[derive(Clone, Copy, Default, Debug, PartialEq)]
+    pub struct LbftFaultSet {
+        pub silent_mask: u64,
+        pub partition_windows: u32,
+        pub partition_max_len: u32,
+    }
+    /// The header's spelling of `LbftFaultSet`, as the `extern "C"` block names it.
+    #[allow(non_camel_case_types)]
+    pub type lbft_fault_set = LbftFaultSet;
+
     /// include/lbft.h `lbft_commit`: one row of `committed_history()`
     #[repr(C)]
     #[derive(Clone, Copy, Default, Debug, PartialEq)]
@@ -145,6 +158,8 @@ pub mod ffi {
         pub fn lbft_create(config: *const LbftConfig, out_sim: *mut *mut LbftSim) -> c_int;
         pub fn lbft_create_sweep(config: *const LbftConfig, sets: *const lbft_param_set, num_sets: u32, set_of_instance: *const u32,
                                  out_sim: *mut *mut LbftSim) -> c_int;
+        pub fn lbft_create_sweep_faults(config: *const LbftConfig, sets: *const lbft_param_set, faults: *const lbft_fault_set, num_sets: u32,
+                                        set_of_instance: *const u32, out_sim: *mut *mut LbftSim) -> c_int;
         pub fn lbft_destroy(sim: *mut LbftSim);
         pub fn lbft_set_seeds(sim: *mut LbftSim, seeds: *const u64) -> c_int;
         pub fn lbft_run(sim: *mut LbftSim) -> c_int;

@@ -172,6 +172,25 @@ typedef struct lbft_param_set {
 int lbft_create_sweep(const lbft_config* config, const lbft_param_set* sets, uint32_t num_sets,
                       const uint32_t* set_of_instance, lbft_sim** out_sim);
 
+/* The fault model of one parameter set of a fault sweep: what lbft_config.silent / partition_windows / partition_max_len
+ * give a plain handle. */
+typedef struct lbft_fault_set {
+  uint64_t silent_mask;           /* bit n: node n is silent (lbft_config.silent[n] != 0); bits >= num_nodes must be 0 */
+  uint32_t partition_windows;     /* 0..64, as lbft_config.partition_windows                                        */
+  uint32_t partition_max_len;     /* as lbft_config.partition_max_len                                               */
+} lbft_fault_set;
+
+/* A fault sweep: lbft_create_sweep with the fault model per parameter set as well.  Every output of instance i (but the
+ * implementation counters max_queue / max_payloads / timers_elided, and runs with a capacity error) is what lbft_create +
+ * lbft_run give it with sets[s] and faults[s] substituted into `config`, s = set_of_instance[i].  The layout and kernel are
+ * what lbft_create_sweep picks with partition_windows set to the largest window count of any set.  Refused (LBFT_ERR_INVALID,
+ * before any device work): whatever lbft_create_sweep refuses, NULL faults, a silent_mask bit >= num_nodes, a set whose
+ * substituted configuration lbft_create refuses (the error names the set), and config->silent != NULL or non-zero
+ * config->partition_windows / partition_max_len (a fault sweep takes its faults per set only).  Flags, and every other entry
+ * point, as for lbft_create_sweep. */
+int lbft_create_sweep_faults(const lbft_config* config, const lbft_param_set* sets, const lbft_fault_set* faults,
+                             uint32_t num_sets, const uint32_t* set_of_instance, lbft_sim** out_sim);
+
 /* Simulator::new for every instance followed by loop_until(max_clock) (simulator.rs:200-250,
  * 380-475): copies the seeds host->device, runs the event-loop kernel to completion, copies the
  * per-node summaries (commit counts, last-committed-state keys, counters, status) device->host.

@@ -32,6 +32,12 @@ class LbftParamSet(ctypes.Structure):
     ]
 
 
+class LbftFaultSet(ctypes.Structure):
+    """``lbft_fault_set`` of include/lbft.h: the fault model of one parameter set of a fault sweep
+    (``lbft_create_sweep_faults``)."""
+    _fields_ = [("silent_mask", c_u64), ("partition_windows", c_u32), ("partition_max_len", c_u32)]
+
+
 class LbftCommit(ctypes.Structure):
     _fields_ = [("proposer", c_u32), ("index", c_u32), ("time", c_i64)]
 
@@ -70,7 +76,7 @@ ST_INVARIANT, ST_EPOCH_CHANGE, ST_DELAY_NEAR_INT, ST_TIME_OVERFLOW = 16, 32, 64,
 ST_ERROR_MASK = ST_ROUND_OVERFLOW | ST_QUEUE_OVERFLOW | ST_PAYLOAD_OVERFLOW | ST_INVARIANT | ST_TIME_OVERFLOW
 
 EXPORTS = [
-    "lbft_create", "lbft_create_sweep", "lbft_run", "lbft_run_async", "lbft_wait", "lbft_commit_logs", "lbft_commit_times", "lbft_latency_stats", "lbft_upload", "lbft_run_device", "lbft_download", "lbft_commit_counts",
+    "lbft_create", "lbft_create_sweep", "lbft_create_sweep_faults", "lbft_run", "lbft_run_async", "lbft_wait", "lbft_commit_logs", "lbft_commit_times", "lbft_latency_stats", "lbft_upload", "lbft_run_device", "lbft_download", "lbft_commit_counts",
     "lbft_last_states", "lbft_commit_log", "lbft_round_switches", "lbft_active_rounds", "lbft_counters", "lbft_status", "lbft_timing_info",
     "lbft_memory_info", "lbft_kernel_info", "lbft_run_until", "lbft_snapshot_size", "lbft_snapshot_save", "lbft_snapshot_load", "lbft_set_seeds", "lbft_device_buffer", "lbft_destroy", "lbft_last_error", "lbft_abi_version",
 ]
@@ -97,6 +103,8 @@ def load():
     P = ctypes.c_void_p
     lib.lbft_create.argtypes = [ctypes.POINTER(LbftConfig), ctypes.POINTER(P)]
     lib.lbft_create_sweep.argtypes = [ctypes.POINTER(LbftConfig), ctypes.POINTER(LbftParamSet), c_u32, P, ctypes.POINTER(P)]
+    lib.lbft_create_sweep_faults.argtypes = [ctypes.POINTER(LbftConfig), ctypes.POINTER(LbftParamSet), ctypes.POINTER(LbftFaultSet), c_u32, P,
+                                             ctypes.POINTER(P)]
     for name in ("lbft_run", "lbft_run_async", "lbft_wait", "lbft_upload", "lbft_run_device", "lbft_download"):
         getattr(lib, name).argtypes = [P]
     for name in ("lbft_commit_counts", "lbft_last_states", "lbft_active_rounds", "lbft_counters", "lbft_status"):

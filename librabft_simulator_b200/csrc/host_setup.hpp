@@ -345,6 +345,17 @@ inline lbft_config with_set(const lbft_config& c, const lbft_param_set& q) {
   return cs;
 }
 
+// `c` with the fault model of one parameter set of a fault sweep substituted: `silent` (num_nodes entries) receives the
+// mask's nodes and must outlive the result.
+inline lbft_config with_faults(const lbft_config& c, const lbft_fault_set& f, uint8_t (&silent)[64]) {
+  lbft_config cs = c;
+  for (uint32_t n = 0; n < 64; n++) silent[n] = (uint8_t)((f.silent_mask >> n) & 1);
+  cs.silent = f.silent_mask ? silent : nullptr;
+  cs.partition_windows = f.partition_windows;
+  cs.partition_max_len = f.partition_max_len;
+  return cs;
+}
+
 struct HostSetup {
   Params params{};  // pointer members are left null; the runtime fills in device addresses
   std::vector<double> zig_x, zig_f;
@@ -354,6 +365,7 @@ struct HostSetup {
   std::vector<double> delay_thr;  // see build_delay_table()
   std::vector<SweepSet> sets;     // sweep handles: one record per parameter set (build_sweep); empty otherwise
   std::vector<uint32_t> set_of;   // sweep handles: [num_instances] the set of each instance
+  std::vector<SweepFaults> faults;  // fault sweeps: one record per parameter set (build_sweep_faults); empty otherwise
   std::string error;
   KernelSel sel{};
 
@@ -373,22 +385,35 @@ struct HostSetup {
   // configuration.  Layout and kernel are what build() picks for the set with the highest event rate (the shortest mean
   // delay: the one the stamp-width and queue-mode tests are sized by), on the sweep kernels; per set, the delay model, the
   // threshold table and the duration / period tables are built as build() builds them and concatenated.
-  bool build_sweep(const lbft_config& c, const lbft_param_set* ps, uint32_t num_sets, const uint32_t* set_of_instance) {
+  //
+  // A fault sweep (lbft_create_sweep_faults, `fs` not null): each set's fault model is substituted as well, the shared
+  // configuration carries none, and the layout and kernel are what a sweep picks with the largest window count of any set in
+  // the configuration; `faults` gets each set's record, and Params::silent_mask the union of the sets' silent nodes (the
+  // kernels' launch-uniform test for whether any node can be silent: sim_core.cuh Core::any_silent).
+  bool build_sweep(const lbft_config& c, const lbft_param_set* ps, uint32_t num_sets, const uint32_t* set_of_instance,
+                   const lbft_fault_set* fs = nullptr) {
     if (c.struct_size != sizeof(lbft_config)) return fail("lbft_config.struct_size does not match this library (ABI mismatch)");
     if (!ps || !set_of_instance) return fail("sets and set_of_instance must not be NULL");
     if (num_sets == 0 || num_sets > c.num_instances || num_sets > 65536u) return fail("num_sets must be in 1..min(num_instances, 65536)");
     if (c.flags & ~(uint32_t)LBFT_FLAG_COMMIT_TIMES) return fail("sweep handles take no flags (recording, resumable and true data-sync runs are plain handles only)");
     for (uint32_t i = 0; i < c.num_instances; i++)
       if (set_of_instance[i] >= num_sets) return fail("set_of_instance has an index >= num_sets");
-    uint32_t fastest = 0;
+    if (fs && (c.silent || c.partition_windows || c.partition_max_len))
+      return fail("a fault sweep takes its silent nodes and partitions per set only: lbft_config.silent must be NULL and "
+                  "partition_windows / partition_max_len 0");
+    uint32_t fastest = 0, windows = 0;
     for (uint32_t s = 0; s < num_sets; s++) {
-      const lbft_config cs = with_set(c, ps[s]);
+      uint8_t silent[64];
+      const lbft_config cs = fs ? with_faults(with_set(c, ps[s]), fs[s], silent) : with_set(c, ps[s]);
       const char* e = config_error(cs);
+      if (!e && fs && c.num_nodes < 64 && (fs[s].silent_mask >> c.num_nodes)) e = "silent_mask has a bit at or above num_nodes";
       if (e || ps[s].reserved)
         return fail(("parameter set " + std::to_string(s) + ": " + (ps[s].reserved ? "reserved must be 0" : e)).c_str());
       if (mean_delay(cs) < mean_delay(with_set(c, ps[fastest]))) fastest = s;
+      if (fs && fs[s].partition_windows > windows) windows = fs[s].partition_windows;
     }
-    const lbft_config cf = with_set(c, ps[fastest]);
+    lbft_config cf = with_set(c, ps[fastest]);
+    if (fs) cf.partition_windows = windows;
     const uint32_t rcap = round_cap_of(cf);
     if (c.commands_per_epoch < rcap)
       return fail("sweep handles need commands_per_epoch >= round_cap (single-epoch runs: epochs are plain handles only)");
@@ -398,8 +423,22 @@ struct HostSetup {
     for (uint32_t s = 0; s < num_sets; s++) add_set(with_set(c, ps[s]), rcap, sets[s]);
     use_set(sets[fastest]);
     set_of.assign(set_of_instance, set_of_instance + c.num_instances);
+    if (fs) {
+      faults.resize(num_sets);
+      for (uint32_t s = 0; s < num_sets; s++) {
+        faults[s] = SweepFaults{fs[s].silent_mask, fs[s].partition_windows, fs[s].partition_max_len};
+        params.silent_mask |= fs[s].silent_mask;  // the union: the kernels' launch-uniform "any silent node" test
+      }
+    }
     sel = select_kernel(cf, tile, params, true);
     return true;
+  }
+
+  // A fault sweep (lbft_create_sweep_faults): build_sweep with each set's fault model.
+  bool build_sweep_faults(const lbft_config& c, const lbft_param_set* ps, const lbft_fault_set* fs, uint32_t num_sets,
+                          const uint32_t* set_of_instance) {
+    if (!fs) return fail("faults must not be NULL");
+    return build_sweep(c, ps, num_sets, set_of_instance, fs);
   }
 
  private:

@@ -3,7 +3,7 @@
 //   lbft_event_loop_kernel<NMAX, QMODE, FIXED, REC, RES>   one THREAD per instance, 32 instances per warp tile (large batches)
 //   lbft_wide_kernel<NMAX, QMODE>                          one WARP per instance (small batches, large committees)
 //   lbft_sweep_event_loop_kernel / lbft_sweep_wide_kernel  the same bodies for sweep handles (lbft_create_sweep: per-instance
-//                                                          delay model and NodeConfig)
+//                                                          delay model and NodeConfig; lbft_create_sweep_faults: and faults)
 //   lbft_ct_*_kernel                                       the same bodies with the commit-time stores (LBFT_FLAG_COMMIT_TIMES),
 //                                                          a twin of every one-shot single-epoch plain and sweep kernel
 //
@@ -39,12 +39,14 @@ struct LaunchShape {
 // each other's latency.  Plain kernels over the calendar queue and the shared-memory queue (whose columns keep their
 // 32-entry pitch); the state layout interleaves TILE instances.
 // The body of both thread kernels (lbft_event_loop_kernel, lbft_sweep_event_loop_kernel), given the kernel's shared memory.
-// SW (sweep handles): the instance's parameter set supplies the delay model and NodeConfig; its thresholds are read through
-// L1 from the concatenated table, as the instances of one warp may belong to different sets.
+// SW (sweep handles): the instance's parameter set supplies the delay model and NodeConfig, and on a fault sweep (`faults`:
+// `sets` heads a SweepSetFaults table) the silent nodes and partition plan; its thresholds are read through L1 from the
+// concatenated table, as the instances of one warp may belong to different sets.
 // CT: the commit-time stores (sim_core.cuh Core CT) into `times`, [num_instances][N + 1][round_cap].
 template <int NMAX, int QMODE, int FX, bool REC, bool RES, bool EP, bool TDS, int TILE, bool SW, bool CT = false>
 __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, double* s_zf, double* s_thr, uint32_t* s_queue,
-                                                const uint32_t* set_of, const SweepSet* sets, int32_t* times = nullptr) {
+                                                const uint32_t* set_of, const SweepSet* sets, int32_t* times = nullptr,
+                                                bool faults = false) {
   static_assert(TILE == 32 || ((QMODE == 3 || QMODE == 2) && !REC && !RES && !EP && !TDS), "sparse tiles: plain kernels over the calendar / shared-memory queue");
   for (int i = threadIdx.x; i < 257; i += blockDim.x) {
     s_zx[i] = P.zig_x[i];
@@ -74,7 +76,10 @@ __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, d
   Core<TileMem<TILE>, NMAX, QMODE, FX, REC, RES, 1, EP, TDS, KS, SW, CT> core(P, mem, s_zx, s_zf, thr_fits ? s_thr : P.delay_thr, sk, sd);
   if (KS) core.km = s_queue + (size_t)(threadIdx.x >> 5) * calendar_kmask_words(FX ? fixed_layout(FX) : P.L) * TILE + lane;
   if constexpr (CT) core.ct = times + (size_t)inst * (core.L.num_nodes + 1) * core.L.round_cap;
-  if constexpr (SW) core.bind_set(sets + set_of[inst]);
+  if constexpr (SW) {
+    core.bind_set(faults ? &reinterpret_cast<const SweepSetFaults*>(sets)[set_of[inst]].set : sets + set_of[inst]);
+    core.bind_faults(faults);
+  }
   if (RES && (P.run_flags & 1u)) core.restore_regs();  // a later lbft_run_until: continue where the last launch stopped
   else core.init(P.seeds[inst]);
   core.run();
@@ -101,7 +106,8 @@ __global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMOD
   __shared__ double s_zx[257];
   __shared__ double s_zf[257];
   extern __shared__ uint32_t s_queue[];
-  event_loop_body<NMAX, QMODE, FX_NONE, false, false, false, false, TILE, true>(S.P, s_zx, s_zf, nullptr, s_queue, S.set_of, S.sets);
+  event_loop_body<NMAX, QMODE, FX_NONE, false, false, false, false, TILE, true>(S.P, s_zx, s_zf, nullptr, s_queue, S.set_of, S.sets, nullptr,
+                                                                               S.faults != 0);
 }
 
 // ---- a group of G lanes per instance ("wide") ---------------------------------------------------------------------
@@ -130,7 +136,7 @@ LBFT_LAYOUT_FN uint32_t wide_smem_words_per_group(const Layout& L, int qmode, bo
 // The body of both wide kernels (lbft_wide_kernel, lbft_sweep_wide_kernel).  SW: as event_loop_body.
 template <int NMAX, int QMODE, bool SMEM, int G, bool EP, int FX, bool SW, bool CT = false>
 __device__ __forceinline__ void wide_body(const Params& P, uint32_t* s_wide, const uint32_t* set_of, const SweepSet* sets,
-                                          int32_t* times = nullptr) {
+                                          int32_t* times = nullptr, bool faults = false) {
   constexpr uint32_t kPerBlock = wide_warps(G) * 32 / G;
   const uint32_t grp = threadIdx.x / G, wl = threadIdx.x % G;
   const uint32_t inst = blockIdx.x * kPerBlock + grp;
@@ -148,7 +154,10 @@ __device__ __forceinline__ void wide_body(const Params& P, uint32_t* s_wide, con
   if constexpr (CT) core.ct = times + (size_t)inst * (KL.num_nodes + 1) * KL.round_cap;
   core.gm = G == 32 ? 0xffffffffu : (((1u << (G & 31)) - 1u) << ((threadIdx.x & 31u) & ~(uint32_t)(G - 1)));
   core.ws = ws;
-  if constexpr (SW) core.bind_set(sets + set_of[inst]);
+  if constexpr (SW) {
+    core.bind_set(faults ? &reinterpret_cast<const SweepSetFaults*>(sets)[set_of[inst]].set : sets + set_of[inst]);
+    core.bind_faults(faults);
+  }
   core.init(P.seeds[inst]);
   core.run();
   core.finalize(inst);
@@ -170,7 +179,7 @@ __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbf
 template <int NMAX, int QMODE, bool SMEM, int G>
 __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbft_sweep_wide_kernel(const __grid_constant__ SweepParams S) {
   extern __shared__ __align__(8) uint32_t s_wide[];
-  wide_body<NMAX, QMODE, SMEM, G, false, FX_NONE, true>(S.P, s_wide, S.set_of, S.sets);
+  wide_body<NMAX, QMODE, SMEM, G, false, FX_NONE, true>(S.P, s_wide, S.set_of, S.sets, nullptr, S.faults != 0);
 }
 
 // The parameter block of a commit-times kernel (LBFT_FLAG_COMMIT_TIMES): the plain (Params) or sweep (SweepParams) block and
@@ -197,7 +206,7 @@ __global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMOD
   __shared__ double s_zf[257];
   extern __shared__ uint32_t s_queue[];
   event_loop_body<NMAX, QMODE, FX_NONE, false, false, false, false, TILE, true, true>(C.base.P, s_zx, s_zf, nullptr, s_queue, C.base.set_of,
-                                                                                     C.base.sets, C.times);
+                                                                                     C.base.sets, C.times, C.base.faults != 0);
 }
 template <int NMAX, int QMODE, bool SMEM, int G, int FX>
 __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbft_ct_wide_kernel(const __grid_constant__ CtParams<Params> C) {
@@ -207,7 +216,7 @@ __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbf
 template <int NMAX, int QMODE, bool SMEM, int G>
 __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbft_ct_sweep_wide_kernel(const __grid_constant__ CtParams<SweepParams> C) {
   extern __shared__ __align__(8) uint32_t s_wide[];
-  wide_body<NMAX, QMODE, SMEM, G, false, FX_NONE, true, true>(C.base.P, s_wide, C.base.set_of, C.base.sets, C.times);
+  wide_body<NMAX, QMODE, SMEM, G, false, FX_NONE, true, true>(C.base.P, s_wide, C.base.set_of, C.base.sets, C.times, C.base.faults != 0);
 }
 
 // One per translation unit: launches the instantiation the selection names, or returns cudaErrorInvalidValue if the unit

@@ -77,6 +77,7 @@ struct lbft_sim {
   double* d_delay_thr = nullptr;
   SweepSet* d_sets = nullptr;    // sweep handles only
   uint32_t* d_set_of = nullptr;  // sweep handles only
+  SweepSetFaults* d_set_faults = nullptr;  // fault sweeps only: each set with its fault record (instead of d_sets)
   uint32_t* d_state = nullptr;
   uint32_t* d_commit_counts = nullptr;
   uint32_t* d_lc_round = nullptr;
@@ -127,7 +128,7 @@ static void free_all(lbft_sim* s) {
   cudaFree(s->d_seeds); cudaFree(s->d_zx); cudaFree(s->d_zf); cudaFree(s->d_leader); cudaFree(s->d_duration);
   cudaFree(s->d_period); cudaFree(s->d_weights); cudaFree(s->d_delay_thr); cudaFree(s->d_state); cudaFree(s->d_summary);
   cudaFree(s->d_lc_round); cudaFree(s->d_counters); cudaFree(s->d_status);
-  cudaFree(s->d_error); cudaFree(s->d_logs); cudaFree(s->d_sets); cudaFree(s->d_set_of);
+  cudaFree(s->d_error); cudaFree(s->d_logs); cudaFree(s->d_sets); cudaFree(s->d_set_of); cudaFree(s->d_set_faults);
   cudaFree(s->d_times); cudaFree(s->d_times_out); cudaFree(s->d_lat);
   for (int b = 0; b < 2; b++) {
     cudaFreeHost(s->h_seeds[b]);
@@ -253,9 +254,24 @@ int lbft_create_sweep(const lbft_config* config, const lbft_param_set* sets, uin
   return create_on_device(s, config, out_sim);
 }
 
+int lbft_create_sweep_faults(const lbft_config* config, const lbft_param_set* sets, const lbft_fault_set* faults, uint32_t num_sets,
+                             const uint32_t* set_of_instance, lbft_sim** out_sim) {
+  if (!config || !out_sim) return set_error(LBFT_ERR_INVALID, "config and out_sim must not be NULL");
+  *out_sim = nullptr;
+  lbft_sim* s = new (std::nothrow) lbft_sim();
+  if (!s) return set_error(LBFT_ERR_NOMEM, "out of host memory");
+  if (!s->hs.build_sweep_faults(*config, sets, faults, num_sets, set_of_instance)) {
+    std::string e = s->hs.error;
+    delete s;
+    return set_error(LBFT_ERR_INVALID, e);
+  }
+  return create_on_device(s, config, out_sim);
+}
+
 }  // extern "C"
 
-// The device half of lbft_create / lbft_create_sweep, once the host setup `s->hs` is built: takes ownership of `s`.
+// The device half of lbft_create / lbft_create_sweep / lbft_create_sweep_faults, once the host setup `s->hs` is built: takes
+// ownership of `s`.
 static int create_on_device(lbft_sim* s, const lbft_config* config, lbft_sim** out_sim) {
   s->I = config->num_instances;
   s->N = config->num_nodes;
@@ -326,10 +342,18 @@ static int create_on_device(lbft_sim* s, const lbft_config* config, lbft_sim** o
   CREATE_TRY(cudaMemcpy(s->d_weights, s->hs.weights.data(), N * sizeof(uint32_t), cudaMemcpyHostToDevice));
   if (s->d_delay_thr)
     CREATE_TRY(cudaMemcpy(s->d_delay_thr, s->hs.delay_thr.data(), s->hs.delay_thr.size() * sizeof(double), cudaMemcpyHostToDevice));
-  if (!s->hs.sets.empty()) {
+  if (!s->hs.sets.empty() && s->hs.faults.empty()) {
     CREATE_TRY(dev_alloc(s, &s->d_sets, s->hs.sets.size()));
-    CREATE_TRY(dev_alloc(s, &s->d_set_of, I));
     CREATE_TRY(cudaMemcpy(s->d_sets, s->hs.sets.data(), s->hs.sets.size() * sizeof(SweepSet), cudaMemcpyHostToDevice));
+  }
+  if (!s->hs.faults.empty()) {
+    std::vector<SweepSetFaults> table(s->hs.sets.size());
+    for (size_t k = 0; k < table.size(); k++) table[k] = SweepSetFaults{s->hs.sets[k], s->hs.faults[k]};
+    CREATE_TRY(dev_alloc(s, &s->d_set_faults, table.size()));
+    CREATE_TRY(cudaMemcpy(s->d_set_faults, table.data(), table.size() * sizeof(SweepSetFaults), cudaMemcpyHostToDevice));
+  }
+  if (!s->hs.sets.empty()) {
+    CREATE_TRY(dev_alloc(s, &s->d_set_of, I));
     CREATE_TRY(cudaMemcpy(s->d_set_of, s->hs.set_of.data(), I * sizeof(uint32_t), cudaMemcpyHostToDevice));
   }
 #undef CREATE_TRY
@@ -465,7 +489,8 @@ static int enqueue_kernel(lbft_sim* s) {
   CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
   CUDA_TRY(cudaEventRecord(s->ev[2], s->stream));
   const KernelSel& k = s->hs.sel;
-  const SweepParams sp{s->P, s->d_set_of, s->d_sets};
+  const SweepParams sp{s->P, s->d_set_of, s->d_set_faults ? reinterpret_cast<const SweepSet*>(s->d_set_faults) : s->d_sets,
+                       s->d_set_faults ? 1u : 0u, 0u};
   const CtParams<Params> cp{s->P, s->d_times};
   const CtParams<SweepParams> csp{sp, s->d_times};
   cudaError_t e = k.ct ? (k.sweep ? (k.wide ? launch_ct_sweep_wide(k, csp, s->stream) : launch_ct_sweep_thread(k, csp, s->stream))

@@ -29,6 +29,7 @@
 // written back once; every network send of the iteration goes through ONE copy of the delay-sampling +
 // enqueue code; the rare ziggurat wedge/tail and the exp() fallback live out of line.
 #pragma once
+#include <stddef.h>
 #include <stdint.h>
 
 #include <type_traits>
@@ -285,6 +286,20 @@ LBFT_COLD int64_t delay_via_exp(double mu, double sigma, double z) {  // bit 62 
   int64_t flag = fabs(v - r) < 1e-9 * (r > 1.0 ? r : 1.0) ? (1LL << 62) : 0;
   if (!(v < 1.0e9)) return (1LL << 61) | 1000000000LL;
   return flag | (int64_t)v;
+}
+
+// The silent mask of the fault record behind parameter set `set` in a fault sweep's table (SweepSetFaults; Core::is_silent),
+// loaded where it is used.  On the device the load is an asm block with the offset as its immediate, so that the compiler
+// can neither hoist the mask, nor the record's address, out of the event loop: either would hold two registers through it.
+static_assert(offsetof(SweepSetFaults, faults) == 64 && offsetof(SweepFaults, silent_mask) == 0, "the immediate below");
+LBFT_HD uint64_t silent_mask_behind(const SweepSet* set) {
+#if defined(__CUDA_ARCH__)
+  uint64_t v;
+  asm volatile("ld.global.nc.u64 %0, [%1+64];" : "=l"(v) : "l"(set));
+  return v;
+#else
+  return reinterpret_cast<const SweepSetFaults*>(set)->faults.silent_mask;
+#endif
 }
 
 // Partition plan (EXTENSION, SURVEY App. D.3): the windows open at `clock` and the next clock at which that set changes.
@@ -583,6 +598,8 @@ using QueueFor = typename std::conditional<QMODE == 0, HeapQueue<Mem, G>, typena
 // KS: (QMODE 3) the calendar's kind-occupancy words live in shared memory (CalendarQueue).
 // SW: a sweep handle (lbft_create_sweep) — the delay model and NodeConfig come from the instance's parameter set (bind_set)
 // instead of Params; every read of them goes through the accessors below.
+//     On a fault sweep (lbft_create_sweep_faults) the silent nodes and the partition plan come from the fault record of the
+//     instance's set (bind_faults), through the accessors below as well.
 // CT: LBFT_FLAG_COMMIT_TIMES — propose_block and process_commits store the global clock into the instance's commit-time table
 // (ct, outside the instance state: [N + 1][round_cap] int32, row n = node n's commit of round r, row N = the proposal of
 // round r).  Nothing in the kernel reads the table back, and it is not cleared at init: the read-out (commit_times_of) only
@@ -620,6 +637,7 @@ struct Core {
   const double* zf;
   const double* thr;  // delay thresholds (shared-memory copy on the device when it fits; SW: the instance's set's, bind_set)
   const SweepSet* sw = nullptr;  // SW: the instance's parameter set
+  bool faults = false;           // SW: a fault sweep: `sw` points into a SweepSetFaults table (bind_faults)
   using Queue = QueueFor<QMODE, Mem, G, KS>;
   Queue q;                 // given its shared memory by the constructor (QMODE 2: sk / sd, or the host harness's stand-in) and init (km)
   uint32_t* km = nullptr;  // KS: the calendar's occupancy words in shared memory, a column per lane, set by the kernel
@@ -662,6 +680,38 @@ struct Core {
   LBFT_HD int32_t tci() const { if constexpr (SW) return sw->tci; else return P.tci; }
   LBFT_HD int32_t duration(uint32_t n) const { if constexpr (SW) return P.duration[sw->rt_off + n]; else return P.duration[n]; }
   LBFT_HD int32_t period(uint32_t n) const { if constexpr (SW) return P.period[sw->rt_off + n]; else return P.period[n]; }
+  // The fault model: the launch's (Params, Layout), or on a fault sweep the record of the instance's set (bind_faults).
+  // SW: on a fault sweep (SweepParams::faults), the set bound by bind_set is the head of a SweepSetFaults entry whose fault
+  // record follows it; before init.  The sweep kernels sit at their register bound: a record pointer, or a silent mask, held
+  // through the event loop spills there and slows every sweep.  So nothing is held but this flag (uniform over the launch):
+  // the record is read at a fixed offset from `sw`, the silent mask where a node is tested (is_silent), and the window count
+  // only enters the plan drawn at init.
+  LBFT_HD void bind_faults(bool fault_sweep) { faults = fault_sweep; }
+  LBFT_HD const SweepFaults& fault_record() const { return reinterpret_cast<const SweepSetFaults*>(sw)->faults; }
+  // Whether the instance may have silent nodes, and whether node n is one.  On a fault sweep P.silent_mask is the union of
+  // the sets' silent nodes (HostSetup::build_sweep), so the launch-uniform test skips the record wherever no set has any.
+  LBFT_HD bool any_silent() const { return P.silent_mask; }
+  LBFT_HD bool is_silent(uint32_t n) const {
+    if constexpr (SW) return ((P.silent_mask >> n) & 1) && (!faults || ((silent_mask_behind(sw) >> n) & 1));
+    else return (P.silent_mask >> n) & 1;
+  }
+  // SW: whether run() drops an event of `kind` for `receiver` from `sender` unhandled (a silent receiver handles nothing, and a
+  // silent sender's request is not answered), with one load of the mask.
+  LBFT_HD bool sweep_silent_drop(uint32_t kind, uint32_t receiver, uint32_t sender) const {
+    const uint64_t mask = faults ? silent_mask_behind(sw) : P.silent_mask;
+    return ((mask >> receiver) | (kind == EV_REQUEST ? mask >> sender : 0)) & 1;
+  }
+  // The plan's window count and length, read when init() draws the plan.  A set never has more windows than the layout;
+  // init() leaves the layout's windows past the set's count empty ([0, 0): never open), so partitioned() and the send path stay
+  // keyed on L.part_windows, as packed_plan() is.
+  LBFT_HD uint32_t part_windows() const {
+    if constexpr (SW) return faults ? fault_record().part_windows : L.part_windows;
+    else return L.part_windows;
+  }
+  LBFT_HD uint32_t part_max_len() const {
+    if constexpr (SW) return faults ? fault_record().part_max_len : P.part_max_len;
+    else return P.part_max_len;
+  }
 
   // ------------------------------------------------------------------------------------------
   // RNG (rand_xoshiro 0.6.0 / rand 0.8.3 / rand_distr 0.4.0)
@@ -1535,8 +1585,7 @@ struct Core {
     // event up to max_clock is popped before a one-shot run ends — and keep the event, a third of the 64-author
     // configuration's traffic, out of the queue and out of the snapshot's reference count.  It still takes its creation
     // stamp and its delay draw.  Not while recording / resumable / true-data-sync (every pop is observable there).
-    if (ELIDE && !TDS && MAY_SILENT && P.silent_mask && kind != EV_RESPONSE &&
-        ((P.silent_mask >> (kind == EV_NOTIFY ? receiver : sender)) & 1)) {
+    if (ELIDE && !TDS && MAY_SILENT && any_silent() && kind != EV_RESPONSE && is_silent(kind == EV_NOTIFY ? receiver : sender)) {
       stamp++;
       if (stamp >= Queue::kStampLimit) status |= ST_QUEUE_OVERFLOW;
       if (t <= P.max_clock) {
@@ -1604,15 +1653,18 @@ struct Core {
       uint32_t kd = draws;
       seed_rng(seed ^ 0xD1B54A32D192ED03ULL, s0, s1, s2, s3);
       uint64_t nsub = N >= 64 ? 0xfffffffffffffffeULL : ((1ULL << N) - 2);
-      for (uint32_t k = 0; k < L.part_windows; k++) {
+      for (uint32_t k = 0; k < part_windows(); k++) {
         int64_t t0 = (int64_t)gen_range_u64((uint64_t)P.max_clock + 1);
-        int64_t len = 1 + (int64_t)gen_range_u64(P.part_max_len ? P.part_max_len : 1);
+        int64_t len = 1 + (int64_t)gen_range_u64(part_max_len() ? part_max_len() : 1);
         uint64_t mask = N >= 2 ? 1 + gen_range_u64(nsub) : 0;
         m.st(L.part_base + 4 * k, (uint32_t)t0);
         m.st(L.part_base + 4 * k + 1, (uint32_t)(t0 + len));
         m.st(L.part_base + 4 * k + 2, (uint32_t)mask);
         m.st(L.part_base + 4 * k + 3, (uint32_t)(mask >> 32));
       }
+      if constexpr (SW)  // a fault sweep's set with fewer windows than the layout: the rest stay empty
+        for (uint32_t k = part_windows(); k < L.part_windows; k++)
+          for (uint32_t w = 0; w < 4; w++) m.st(L.part_base + 4 * k + w, 0);
       s0 = k0; s1 = k1; s2 = k2; s3 = k3;
       draws = kd;
     }
@@ -1668,9 +1720,13 @@ struct Core {
       proc2 += kind == EV_RESPONSE;
       proc3 += kind == EV_TIMER;
       // EXTENSION D.2: silent nodes handle nothing and answer no request
-      if (MAY_SILENT && P.silent_mask) {
-        bool drop = (P.silent_mask >> receiver) & 1;
-        if (kind == EV_REQUEST && ((P.silent_mask >> sender) & 1)) drop = true;
+      if (MAY_SILENT && any_silent()) {
+        bool drop;
+        if constexpr (SW) drop = sweep_silent_drop(kind, receiver, sender);
+        else {
+          drop = (P.silent_mask >> receiver) & 1;
+          if (kind == EV_REQUEST && ((P.silent_mask >> sender) & 1)) drop = true;
+        }
         if (drop) {
           if (kind == EV_NOTIFY || (TDS && slot != PAY_NONE)) pay_unref(slot, pay_refs(slot));
           continue;

@@ -256,13 +256,30 @@ struct Params {
                          //     word instead of scanning I statuses
 };
 
+// The fault model of one parameter set of a fault sweep (lbft_create_sweep_faults): what Params::silent_mask, Layout::part_windows
+// and Params::part_max_len give every instance of a plain handle.  part_windows is at most the layout's (the partition region
+// is sized for the largest count of any set).
+struct SweepFaults {
+  uint64_t silent_mask;
+  uint32_t part_windows;
+  uint32_t part_max_len;
+};
+// One entry of a fault sweep's device table of parameter sets: the set, and its fault record right behind it, so that an
+// instance reaches the record at a fixed offset from the set pointer it holds anyway (sim_core.cuh Core::bind_faults).
+struct SweepSetFaults {
+  SweepSet set;
+  SweepFaults faults;
+};
+
 // The parameter block of a sweep handle's kernels (lbft_create_sweep): instance i runs with sets[set_of[i]], and
 // P.delay_thr / P.duration / P.period are the concatenated tables of all sets.  (A block of its own rather than fields
 // appended to Params, so that no other kernel's parameters move.)
 struct SweepParams {
   Params P;
   const uint32_t* set_of;  // [num_instances]
-  const SweepSet* sets;    // [num_sets]
+  const SweepSet* sets;    // [num_sets]; a fault sweep (lbft_create_sweep_faults): the sets of a SweepSetFaults [num_sets] table
+  uint32_t faults;         // 1: a fault sweep, whose instances take their silent nodes and partition plan from their set's record
+  uint32_t pad;
 };
 
 }  // namespace lbft

@@ -502,11 +502,33 @@ class BatchSimulator:
 
 
 @dataclass(frozen=True)
+class FaultSet:
+    """The fault model of one point of a sweep: the silent (crashed) nodes, by index, and the random partition plan — what
+    ``BatchSimulator``'s ``silent`` / ``partition_windows`` / ``partition_max_len`` give a whole batch."""
+    silent: tuple = ()
+    partition_windows: int = 0
+    partition_max_len: int = 0
+
+    def __post_init__(self):
+        object.__setattr__(self, "silent", tuple(int(n) for n in self.silent))  # (a list or array compares, and hashes, as a tuple)
+
+    def to_c(self):
+        mask = 0
+        for n in self.silent:
+            if not 0 <= int(n) < 64:
+                raise ValueError("silent node index %r is not in 0..63" % (n,))
+            mask |= 1 << int(n)
+        return _lib.LbftFaultSet(silent_mask=mask, partition_windows=int(self.partition_windows),
+                                 partition_max_len=int(self.partition_max_len))
+
+
+@dataclass(frozen=True)
 class ParamSet:
     """One point of a parameter sweep: the network delay and ``NodeConfig`` of the instances assigned to it
-    (main.rs --mean / --variance and --delta / --gamma / --lambda / --target_commit_interval)."""
+    (main.rs --mean / --variance and --delta / --gamma / --lambda / --target_commit_interval), and its fault model."""
     network_delay: RandomDelay = RandomDelay()
     node_config: NodeConfig = NodeConfig()
+    faults: FaultSet = FaultSet()
 
     def to_c(self):
         d, n = self.network_delay, self.node_config
@@ -517,10 +539,12 @@ class ParamSet:
 
 class SweepSimulator(BatchSimulator):
     """A parameter sweep as ONE batch (``lbft_create_sweep``): instance i runs ``Simulator::new(seeds[i], ..)`` under
-    ``param_sets[set_of_instance[i]]``; everything else (committee, voting rights, silent nodes, partitions,
-    ``commands_per_epoch``, capacities, device) is shared and passed as for ``BatchSimulator``.  Every result of instance i
-    is what a ``BatchSimulator`` with that set's delay and node config computes for it.  Running, re-seeding (the set
-    assignment stays), streaming and reading results work as on a ``BatchSimulator``."""
+    ``param_sets[set_of_instance[i]]``; everything else (committee, voting rights, ``commands_per_epoch``, capacities,
+    device) is shared and passed as for ``BatchSimulator``.  Silent nodes and partitions are shared too, unless a set carries
+    a ``FaultSet`` of its own: then every set has its own (``lbft_create_sweep_faults``) and the shared ``silent`` /
+    ``partition_*`` arguments must be left unset.  Every result of instance i is what a ``BatchSimulator`` with that set's
+    delay, node config and faults computes for it.  Running, re-seeding (the set assignment stays), streaming and reading
+    results work as on a ``BatchSimulator``."""
 
     def __init__(self, seeds, num_nodes, param_sets, set_of_instance, **shared):
         super().__init__(seeds, num_nodes, **shared)
@@ -530,24 +554,36 @@ class SweepSimulator(BatchSimulator):
             raise ValueError("set_of_instance needs one entry per seed (%d)" % self.num_instances)
 
     @classmethod
-    def grid(cls, seeds_per_point, delays, node_configs, num_nodes=4, **shared):
+    def grid(cls, seeds_per_point, delays, node_configs, num_nodes=4, faults=None, **shared):
         """The Cartesian product ``delays x node_configs`` (point p = i * len(node_configs) + j), each point run over the
         same seeds (``seeds_per_point``: a sequence of seeds, or a count k for seeds 0..k-1) in a contiguous block of
-        instances: point p holds instances [p * k, (p + 1) * k).  ``set_of_instance`` and ``param_sets`` say which is which."""
+        instances: point p holds instances [p * k, (p + 1) * k).  ``set_of_instance`` and ``param_sets`` say which is which.
+        ``faults``, a list of ``FaultSet``, adds a third, fastest-varying axis: point p = (i * len(node_configs) + j) *
+        len(faults) + f, so ``latency_stats().mean().reshape(len(delays), len(node_configs), len(faults))`` is the cube."""
         seeds = np.arange(seeds_per_point, dtype=np.uint64) if np.isscalar(seeds_per_point) else \
             np.asarray(seeds_per_point, dtype=np.uint64).reshape(-1)
-        sets = [ParamSet(d, n) for d in delays for n in node_configs]
+        sets = [ParamSet(d, n) for d in delays for n in node_configs] if faults is None else \
+            [ParamSet(d, n, f) for d in delays for n in node_configs for f in faults]
         k = seeds.shape[0]
         return cls(np.tile(seeds, len(sets)), num_nodes, sets, np.repeat(np.arange(len(sets), dtype=np.uint32), k), **shared)
 
     def create(self, max_clock):
-        """``lbft_create_sweep``: validate every set, build the per-set host tables, allocate device state."""
+        """``lbft_create_sweep``, or ``lbft_create_sweep_faults`` when some set has faults: validate every set, build the
+        per-set host tables, allocate device state."""
+        per_set = any(p.faults != FaultSet() for p in self.param_sets)
+        if per_set and (self.silent is not None or self.partition_windows or self.partition_max_len):
+            raise ValueError("a sweep takes silent nodes and partitions either per set (ParamSet.faults) or shared (silent / "
+                             "partition_windows / partition_max_len), not both")
         self.close()
         handle = ctypes.c_void_p()
         cfg = self.make_config(max_clock)
         sets = (_lib.LbftParamSet * max(1, len(self.param_sets)))(*[p.to_c() for p in self.param_sets])
-        _lib.check(self._lib.lbft_create_sweep(ctypes.byref(cfg), sets, len(self.param_sets),
-                                               ctypes.c_void_p(self.set_of_instance.ctypes.data), ctypes.byref(handle)))
+        so = ctypes.c_void_p(self.set_of_instance.ctypes.data)
+        if per_set:
+            faults = (_lib.LbftFaultSet * len(self.param_sets))(*[p.faults.to_c() for p in self.param_sets])
+            _lib.check(self._lib.lbft_create_sweep_faults(ctypes.byref(cfg), sets, faults, len(self.param_sets), so, ctypes.byref(handle)))
+        else:
+            _lib.check(self._lib.lbft_create_sweep(ctypes.byref(cfg), sets, len(self.param_sets), so, ctypes.byref(handle)))
         self._handle = handle
         return self
 
