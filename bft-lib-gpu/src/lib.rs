@@ -175,6 +175,8 @@ pub mod ffi {
         pub fn lbft_commit_logs(sim: *mut LbftSim, out: *mut LbftCommit, cap: usize, lens: *mut u32) -> c_int;
         pub fn lbft_commit_times(sim: *mut LbftSim, committed: *mut i64, proposed: *mut i64, cap: usize) -> c_int;
         pub fn lbft_latency_stats(sim: *mut LbftSim, spec: *const lbft_latency_spec, out: *mut lbft_latency_summary, hist: *mut u64) -> c_int;
+        pub fn lbft_block_latency_stats(sim: *mut LbftSim, spec: *const lbft_latency_spec, threshold: u64,
+                                        out: *mut lbft_latency_summary, unreached: *mut u64, hist: *mut u64) -> c_int;
         pub fn lbft_round_switches(sim: *mut LbftSim, instance: u32, out: *mut LbftRoundSwitch, cap: usize, n: *mut usize) -> c_int;
         pub fn lbft_snapshot_size(sim: *mut LbftSim, bytes: *mut usize) -> c_int;
         pub fn lbft_snapshot_save(sim: *mut LbftSim, buf: *mut u8, cap: usize) -> c_int;
@@ -444,6 +446,48 @@ impl GpuSimulator {
             total.min = -1;
         }
         (total, hist)
+    }
+
+    /// Block-latency statistics of the whole batch at a voting-rights threshold (`lbft_block_latency_stats`; build the
+    /// simulator `with_commit_times()`), reduced on each GPU and merged over them: one sample per block of each instance's
+    /// chain proposed in `[proposed_from, proposed_until)`, the time from its proposal until the nodes that committed it hold
+    /// `threshold` voting rights (1 ..= the total; e.g. `2 * total / 3 + 1` for a quorum).  Returns the summary, the number
+    /// of blocks that never reached the threshold, and the `num_bins` histogram counts.
+    pub fn block_latency_stats(&self, threshold: u64, num_bins: u32, bin_width: i64, proposed_from: i64, proposed_until: i64)
+                               -> (ffi::LbftLatencySummary, u64, Vec<u64>) {
+        let spec = ffi::LbftLatencySpec {
+            struct_size: std::mem::size_of::<ffi::LbftLatencySpec>() as u32,
+            num_bins,
+            bin_width,
+            proposed_from,
+            proposed_until,
+        };
+        let mut total = ffi::LbftLatencySummary { min: i64::MAX, max: -1, ..Default::default() };
+        let mut unreached = 0u64;
+        let mut hist = vec![0u64; num_bins as usize];
+        for s in &self.shards {
+            let mut part = ffi::LbftLatencySummary::default();
+            let mut part_unreached = 0u64;
+            let mut h = vec![0u64; num_bins as usize];
+            check(unsafe { ffi::lbft_block_latency_stats(s.sim, &spec, threshold, &mut part, &mut part_unreached, h.as_mut_ptr()) },
+                  "lbft_block_latency_stats");
+            total.instances += part.instances;
+            total.excluded += part.excluded;
+            total.samples += part.samples;
+            total.sum += part.sum;
+            if part.samples > 0 {
+                total.min = total.min.min(part.min);
+                total.max = total.max.max(part.max);
+            }
+            unreached += part_unreached;
+            for (a, b) in hist.iter_mut().zip(h) {
+                *a += b;
+            }
+        }
+        if total.samples == 0 {
+            total.min = -1;
+        }
+        (total, unreached, hist)
     }
 }
 

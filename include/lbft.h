@@ -311,6 +311,23 @@ typedef struct lbft_latency_summary {
  * (the bound on sum). */
 int lbft_latency_stats(lbft_sim* sim, const lbft_latency_spec* spec, lbft_latency_summary* out, uint64_t* hist);
 
+/* Block-latency statistics at a voting-rights threshold (lbft_block_latency_stats).  The blocks of an instance are the rows k
+ * of its longest log (the chain every log is a prefix of) whose proposed time p lies in [proposed_from, proposed_until); node n
+ * has committed row k iff k < its commit count, at the time t_n of lbft_commit_times, and holds the voting right w_n
+ * (lbft_config.voting_rights).  The threshold time of a block is the least t_n at which the voting rights of the nodes that
+ * committed it at or before t_n sum to at least `threshold`; it does not depend on the order of ties.  A block has one sample,
+ * T - p, or is unreached when the committed weight stays below the threshold to the end of the run.  Blocks that no node
+ * committed are on no log and are not counted.  Common thresholds, with total the sum of the voting rights: 1 (the first node
+ * to commit), (total + 2) / 3 (f + 1: a client can trust the block), 2 * total / 3 + 1 (a quorum), total (every node).
+ *
+ * Groups, exclusion of instances with an error bit, histogram bins, the window and the exactness of every value are those of
+ * lbft_latency_stats: out[num_groups] (samples counts the reached blocks; sum / min / max / hist cover their latencies),
+ * unreached[num_groups] the blocks that never reached the threshold, or NULL (then not copied), hist[group * num_bins + b] or
+ * NULL.  Refusals: those of lbft_latency_stats, with its messages, and LBFT_ERR_INVALID for a threshold of 0 or above the
+ * handle's total voting rights. */
+int lbft_block_latency_stats(lbft_sim* sim, const lbft_latency_spec* spec, uint64_t threshold, lbft_latency_summary* out,
+                             uint64_t* unreached, uint64_t* hist);
+
 #ifdef __cplusplus
 }
 #endif

@@ -2,8 +2,8 @@
 
 * ``csrc/liblbft_b200.so`` — the product: sm_90a (H100) CUDA kernels + the C ABI of ``include/lbft.h``.
 * ``oracle/liblbft_oracle.so``, ``tests/hostcore/libhostcore.so``, ``tests/hostcore/libhostcore_sweep.so``,
-  ``tests/hostcore/libhostcore_ct.so``, ``tests/hostcore/libhostcore_latency.so`` and ``tests/hostcore/libhostcore_fault.so`` —
-  test infrastructure only.
+  ``tests/hostcore/libhostcore_ct.so``, ``tests/hostcore/libhostcore_latency.so``, ``tests/hostcore/libhostcore_fault.so`` and
+  ``tests/hostcore/libhostcore_block_latency.so`` — test infrastructure only.
 All artefacts are built in-tree and git-ignored.
 """
 import os
@@ -21,6 +21,7 @@ SWEEP_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_sweep.so")
 CT_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_ct.so")
 LATENCY_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_latency.so")
 FAULT_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_fault.so")
+BLOCK_LATENCY_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_block_latency.so")
 
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
@@ -177,6 +178,20 @@ def build_fault_hostcore(force=False):
     return FAULT_HOSTCORE_PATH
 
 
+def build_block_latency_hostcore(force=False):
+    """The CT cores of plain handles, sweeps and fault sweeps with the product's block-latency statistics on the host
+    (tests/hostcore/block_latency_hostcore.cpp, which compiles fault_hostcore.cpp and ct_hostcore.cpp into itself): test
+    infrastructure."""
+    srcs = [os.path.join(HOSTCORE_DIR, f) for f in ("block_latency_hostcore.cpp", "fault_hostcore.cpp", "ct_hostcore.cpp")] + [
+        os.path.join(ROOT, "include", "lbft.h")] + [os.path.join(CSRC, f) for f in ("sim_core.cuh", "sim_params.h", "host_setup.hpp")] + [
+        os.path.join(ORACLE_DIR, f) for f in ("oracle_capi.cpp", "lbft_oracle.hpp")]
+    if not force and _newer(BLOCK_LATENCY_HOSTCORE_PATH, srcs):
+        return BLOCK_LATENCY_HOSTCORE_PATH
+    _run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-DLBFT_CHECK_C1",
+          "-o", BLOCK_LATENCY_HOSTCORE_PATH, "block_latency_hostcore.cpp"], HOSTCORE_DIR)
+    return BLOCK_LATENCY_HOSTCORE_PATH
+
+
 def build_all(force=False):
     return (build_product(force), build_oracle(force), build_hostcore(force), build_sweep_hostcore(force), build_ct_hostcore(force),
-            build_latency_hostcore(force), build_fault_hostcore(force))
+            build_latency_hostcore(force), build_fault_hostcore(force), build_block_latency_hostcore(force))

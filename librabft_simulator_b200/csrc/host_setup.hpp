@@ -592,4 +592,15 @@ inline const char* latency_spec_error(const HostSetup& hs, const lbft_latency_sp
   return nullptr;
 }
 
+// lbft_block_latency_stats: the total voting rights of a handle, and the check on a threshold (null when it is valid).
+inline uint64_t total_voting_rights(const HostSetup& hs) {
+  uint64_t total = 0;
+  for (uint32_t w : hs.weights) total += w;
+  return total;
+}
+inline const char* block_latency_threshold_error(const HostSetup& hs, uint64_t threshold) {
+  if (threshold < 1 || threshold > total_voting_rights(hs)) return "threshold must be in 1..total voting rights of the handle";
+  return nullptr;
+}
+
 }  // namespace lbft

@@ -95,7 +95,7 @@ struct lbft_sim {
   int32_t* d_times = nullptr;    // LBFT_FLAG_COMMIT_TIMES: the commit-time table [I][N + 1][round_cap] (sim_core.cuh Core CT)
   int64_t* d_times_out = nullptr;  // lbft_commit_times: [I][N][times_cap] committed, then [I][times_cap] proposed; on first use
   size_t times_cap = 0;
-  unsigned char* d_lat = nullptr;  // lbft_latency_stats: [groups] summaries, then [groups][num_bins] u64 bins; on first use
+  unsigned char* d_lat = nullptr;  // lbft_latency_stats / lbft_block_latency_stats: summaries, counts and bins; on first use
   size_t lat_bytes = 0;
   uint64_t device_bytes = 0;
   // pinned host staging: two seed buffers (lbft_set_seeds never writes the one an in-flight upload reads) and two
@@ -845,6 +845,132 @@ __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __g
   }
 }
 
+// lbft_block_latency_stats: per-group block-latency statistics at a voting-rights threshold W (sim_core.cuh
+// block_latency_samples_of).  An overload of the per-sample kernel above: the same reduction over other samples, so tools that
+// list the library's kernels by name see it as the latency reduction it is.  A group of G lanes per instance, G the smallest
+// power of two >= min(N, 32), so lane j holds nodes j and, when N > 32, j + 32.  Every lane of the group walks the chain (same
+// addresses: broadcast loads).  Per block, lane j loads its nodes' commit times (+inf where the node did not commit it) and
+// sums, over G width-G shuffles under the group's mask, the voting rights (P.c_weights, indexed by the source lane) of the
+// nodes with a time <= each of its own; the group then takes the least time whose sum reaches W (block_threshold_time, without
+// a per-node array), and lane 0 of the group accumulates the sample or the unreached block.  Histogram and summary paths are
+// those of the per-sample kernel: shared-memory bins when the block's instances share a group and bins <= kLatSharedBins,
+// global atomics otherwise; the summary fields are reduced per warp when its lanes share a group.  Integer atomics only.
+__global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __grid_constant__ Params P, uint32_t stride,
+                                                                       const int32_t* times, const uint32_t* set_of,
+                                                                       uint32_t G, uint32_t W, int64_t width, uint32_t bins,
+                                                                       int64_t from, int64_t until, lbft_latency_summary* sum,
+                                                                       unsigned long long* unreached_out,
+                                                                       unsigned long long* hist, uint32_t* bad) {
+  extern __shared__ uint32_t sh_bins[];
+  const uint32_t per_block = kLatBlock / G;
+  const uint32_t j = threadIdx.x & (G - 1);  // the lane within the group
+  const uint32_t inst = blockIdx.x * per_block + threadIdx.x / G;
+  const bool live = inst < P.num_instances;
+  const uint32_t g0 = set_of ? set_of[blockIdx.x * per_block] : 0u;
+  const uint32_t g = live && set_of ? set_of[inst] : g0;
+  const bool shared_hist = __syncthreads_and(g == g0) && bins <= kLatSharedBins;
+  if (shared_hist) {
+    for (uint32_t b = threadIdx.x; b < bins; b += blockDim.x) sh_bins[b] = 0;
+    __syncthreads();
+  }
+  unsigned long long clean = 0, excluded = 0, samples = 0, total = 0, unreached = 0;
+  long long lo = INT64_MAX, hi = -1;
+  if (live) {
+    if (P.out_status[inst] & ST_ERROR_BITS) {
+      excluded = j == 0;
+    } else {
+      clean = j == 0;
+      const Layout& L = P.L;
+      const uint32_t N = L.num_nodes, tile = inst / stride, lane = inst % stride;
+      const uint32_t* cc = P.out_commit_counts + (size_t)inst * N;
+      const int32_t* t_inst = times + (size_t)inst * (N + 1) * L.round_cap;
+      const uint32_t warp_lane = threadIdx.x & 31;
+      const uint32_t gmask = G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (warp_lane & ~(G - 1));
+      const uint32_t n0 = j, n1 = j + 32;  // (n1 < N only when N > 32, i.e. G == 32)
+      const uint32_t cc0 = n0 < N ? cc[n0] : 0u, cc1 = n1 < N ? cc[n1] : 0u;
+      unsigned long long* gh = hist + (size_t)g * bins;
+      auto time_of = [&](uint32_t k, uint32_t r) -> int64_t {
+        const int32_t t0 = cc0 > k ? t_inst[(size_t)n0 * L.round_cap + r] : INT32_MAX;
+        const int32_t t1 = cc1 > k ? t_inst[(size_t)n1 * L.round_cap + r] : INT32_MAX;
+        uint32_t s0 = 0, s1 = 0;  // the voting rights committed at or before t0, t1 (at most 64 * 2^24)
+        for (uint32_t src = 0; src < G; src++) {
+          const int32_t u0 = __shfl_sync(gmask, t0, src, G);
+          const uint32_t v0 = u0 == INT32_MAX ? 0u : P.c_weights[src];
+          s0 += u0 <= t0 ? v0 : 0u;
+          s1 += u0 <= t1 ? v0 : 0u;
+          if (N > 32) {
+            const int32_t u1 = __shfl_sync(gmask, t1, src, G);
+            const uint32_t v1 = u1 == INT32_MAX ? 0u : P.c_weights[src + 32];
+            s0 += u1 <= t0 ? v1 : 0u;
+            s1 += u1 <= t1 ? v1 : 0u;
+          }
+        }
+        int32_t best = INT32_MAX;
+        if (t0 != INT32_MAX && s0 >= W) best = t0;
+        if (t1 != INT32_MAX && s1 >= W && t1 < best) best = t1;
+        for (uint32_t o = G / 2; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(gmask, best, o, G));
+        return best == INT32_MAX ? INT64_MAX : (int64_t)best;
+      };
+      const bool ok = block_latency_samples_of(
+          L, P.state + (size_t)tile * L.total_words * stride + lane, stride, cc, P.out_lc_round + (size_t)inst * N, t_inst, from,
+          until, time_of,
+          [&](int64_t lat) {
+            if (j != 0) return;
+            samples++;
+            total += (unsigned long long)lat;
+            lo = lat < lo ? lat : lo;
+            hi = lat > hi ? lat : hi;
+            const uint32_t b = latency_bin(lat, width, bins);
+            if (shared_hist) atomicAdd(&sh_bins[b], 1u);
+            else atomicAdd(&gh[b], 1ull);
+          },
+          [&]() { unreached += j == 0; });
+      if (!ok && j == 0) atomicAdd(bad, 1u);
+    }
+  }
+  lbft_latency_summary* gs = sum + g;
+  const uint32_t full = 0xffffffffu;
+  if (__all_sync(full, g == __shfl_sync(full, g, 0))) {
+    for (int o = 16; o > 0; o >>= 1) {
+      clean += __shfl_down_sync(full, clean, o);
+      excluded += __shfl_down_sync(full, excluded, o);
+      samples += __shfl_down_sync(full, samples, o);
+      total += __shfl_down_sync(full, total, o);
+      unreached += __shfl_down_sync(full, unreached, o);
+      lo = min(lo, __shfl_down_sync(full, lo, o));
+      hi = max(hi, __shfl_down_sync(full, hi, o));
+    }
+    if ((threadIdx.x & 31) != 0) clean = excluded = samples = unreached = 0;  // (lane 0 holds the warp's totals)
+  }
+  if (clean) atomicAdd((unsigned long long*)&gs->instances, clean);
+  if (excluded) atomicAdd((unsigned long long*)&gs->excluded, excluded);
+  if (unreached) atomicAdd(&unreached_out[g], unreached);
+  if (samples) {
+    atomicAdd((unsigned long long*)&gs->samples, samples);
+    atomicAdd((unsigned long long*)&gs->sum, total);
+    atomicMin((long long*)&gs->min, lo);
+    atomicMax((long long*)&gs->max, hi);
+  }
+  if (shared_hist) {
+    __syncthreads();
+    unsigned long long* gh = hist + (size_t)g0 * bins;
+    for (uint32_t b = threadIdx.x; b < bins; b += blockDim.x)
+      if (sh_bins[b]) atomicAdd(&gh[b], (unsigned long long)sh_bins[b]);
+  }
+}
+
+// The buffer of lbft_latency_stats and lbft_block_latency_stats, grown to at least `bytes` on first use.
+static int grow_lat_buffer(lbft_sim* s, size_t bytes) {
+  if (bytes <= s->lat_bytes) return LBFT_OK;
+  cudaFree(s->d_lat);
+  s->d_lat = nullptr;
+  s->lat_bytes = 0;
+  cudaError_t e = cudaMalloc((void**)&s->d_lat, bytes);
+  if (e != cudaSuccess) return set_error(LBFT_ERR_NOMEM, std::string("latency-statistics buffer: ") + cudaGetErrorString(e));
+  s->lat_bytes = bytes;
+  return LBFT_OK;
+}
+
 extern "C" {
 
 int lbft_commit_times(lbft_sim* s, int64_t* committed, int64_t* proposed, size_t cap) {
@@ -891,15 +1017,7 @@ int lbft_latency_stats(lbft_sim* s, const lbft_latency_spec* spec, lbft_latency_
   CUDA_TRY(cudaSetDevice(s->device));
   const uint32_t groups = latency_groups(s->hs), bins = spec->num_bins;
   const size_t hist_len = (size_t)groups * bins;
-  const size_t bytes = groups * sizeof(lbft_latency_summary) + hist_len * sizeof(uint64_t);
-  if (bytes > s->lat_bytes) {
-    cudaFree(s->d_lat);
-    s->d_lat = nullptr;
-    s->lat_bytes = 0;
-    cudaError_t e = cudaMalloc((void**)&s->d_lat, bytes);
-    if (e != cudaSuccess) return set_error(LBFT_ERR_NOMEM, std::string("latency-statistics buffer: ") + cudaGetErrorString(e));
-    s->lat_bytes = bytes;
-  }
+  if (int r = grow_lat_buffer(s, groups * sizeof(lbft_latency_summary) + hist_len * sizeof(uint64_t))) return r;
   lbft_latency_summary* d_sum = reinterpret_cast<lbft_latency_summary*>(s->d_lat);
   unsigned long long* d_hist = reinterpret_cast<unsigned long long*>(s->d_lat + groups * sizeof(lbft_latency_summary));
   const size_t init_blocks = ((hist_len > groups ? hist_len : groups) + 255) / 256;
@@ -913,6 +1031,51 @@ int lbft_latency_stats(lbft_sim* s, const lbft_latency_spec* spec, lbft_latency_
   CUDA_TRY(cudaGetLastError());
   uint32_t bad = 0;
   CUDA_TRY(cudaMemcpyAsync(out, d_sum, groups * sizeof(lbft_latency_summary), cudaMemcpyDeviceToHost, s->stream));
+  if (hist) CUDA_TRY(cudaMemcpyAsync(hist, d_hist, hist_len * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(&bad, s->d_error, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  if (bad) {
+    char buf[160];
+    snprintf(buf, sizeof buf, "%u instance(s) have node logs that are not prefixes of one chain: read them with lbft_commit_log", bad);
+    return set_error(LBFT_ERR_STATE, buf);
+  }
+  for (uint32_t g = 0; g < groups; g++)
+    if (out[g].samples == 0) out[g].min = -1;
+  return LBFT_OK;
+}
+
+int lbft_block_latency_stats(lbft_sim* s, const lbft_latency_spec* spec, uint64_t threshold, lbft_latency_summary* out,
+                             uint64_t* unreached, uint64_t* hist) {
+  if (!s || !spec || !out) return set_error(LBFT_ERR_INVALID, "sim, spec and out must not be NULL");
+  if (!s->hs.sel.ct) return set_error(LBFT_ERR_STATE, "commit times were not recorded: set LBFT_FLAG_COMMIT_TIMES in lbft_config.flags");
+  if (!s->downloaded) return set_error(LBFT_ERR_STATE, "results are not available: call lbft_run first");
+  if (const char* e = latency_spec_error(s->hs, *spec)) return set_error(LBFT_ERR_INVALID, e);
+  if (const char* e = block_latency_threshold_error(s->hs, threshold)) return set_error(LBFT_ERR_INVALID, e);
+  if (int r = need_idle(s)) return r;
+  CUDA_TRY(cudaSetDevice(s->device));
+  const uint32_t groups = latency_groups(s->hs), bins = spec->num_bins;
+  const size_t hist_len = (size_t)groups * bins;
+  // [groups] summaries, then [groups] unreached counts and [groups][num_bins] bins (zeroed together)
+  if (int r = grow_lat_buffer(s, groups * sizeof(lbft_latency_summary) + (groups + hist_len) * sizeof(uint64_t))) return r;
+  lbft_latency_summary* d_sum = reinterpret_cast<lbft_latency_summary*>(s->d_lat);
+  unsigned long long* d_unreached = reinterpret_cast<unsigned long long*>(s->d_lat + groups * sizeof(lbft_latency_summary));
+  unsigned long long* d_hist = d_unreached + groups;
+  const size_t init_blocks = (groups + hist_len + 255) / 256;
+  lbft_latency_init_kernel<<<(unsigned)(init_blocks < 4096 ? init_blocks : 4096), 256, 0, s->stream>>>(d_sum, groups, d_unreached,
+                                                                                                       groups + hist_len);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
+  uint32_t G = 1;  // lanes per instance: the smallest power of two >= min(N, 32)
+  while (G < s->N && G < 32) G <<= 1;
+  const uint32_t per_block = kLatBlock / G;
+  const size_t smem = bins <= kLatSharedBins ? bins * sizeof(uint32_t) : 0;
+  lbft_latency_stats_kernel<<<(s->I + per_block - 1) / per_block, kLatBlock, smem, s->stream>>>(
+      s->P, s->stride, s->d_times, s->hs.sel.sweep ? s->d_set_of : nullptr, G, (uint32_t)threshold, spec->bin_width, bins,
+      spec->proposed_from, spec->proposed_until, d_sum, d_unreached, d_hist, s->d_error);
+  CUDA_TRY(cudaGetLastError());
+  uint32_t bad = 0;
+  CUDA_TRY(cudaMemcpyAsync(out, d_sum, groups * sizeof(lbft_latency_summary), cudaMemcpyDeviceToHost, s->stream));
+  if (unreached) CUDA_TRY(cudaMemcpyAsync(unreached, d_unreached, groups * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
   if (hist) CUDA_TRY(cudaMemcpyAsync(hist, d_hist, hist_len * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
   CUDA_TRY(cudaMemcpyAsync(&bad, s->d_error, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
   CUDA_TRY(cudaStreamSynchronize(s->stream));

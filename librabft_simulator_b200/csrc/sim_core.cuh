@@ -2004,6 +2004,46 @@ LBFT_HD bool latency_samples_of(const Layout& L, const uint32_t* tb, uint32_t st
   });
 }
 
+// lbft_block_latency_stats: the threshold time of row k (round r) of an instance's chain, or INT64_MAX when the block never
+// reaches the threshold.  Node n committed the block iff cc[n] > k, at times[n * round_cap + r]; w: the voting rights.  T is the
+// least commit time t_n at which the weight of the nodes that committed at or before t_n reaches W: independent of tie order, and
+// O(N^2) without a per-node array.  The serial form: lbft_api.cu's threshold overload of lbft_latency_stats_kernel spreads the
+// nodes over lanes.
+LBFT_HD int64_t block_threshold_time(const Layout& L, const uint32_t* cc, const int32_t* times, const uint32_t* w, uint32_t k,
+                                     uint32_t r, uint64_t W) {
+  const uint32_t N = L.num_nodes;
+  int64_t T = INT64_MAX;
+  for (uint32_t n = 0; n < N; n++) {
+    if (cc[n] <= k) continue;
+    const int64_t t = times[(size_t)n * L.round_cap + r];
+    if (t >= T) continue;
+    uint64_t s = 0;
+    for (uint32_t m = 0; m < N; m++)
+      if (cc[m] > k && times[(size_t)m * L.round_cap + r] <= t) s += w[m];
+    if (s >= W) T = t;
+  }
+  return T;
+}
+
+// lbft_block_latency_stats for one instance: for every row k of its chain (walk_commit_chain, every row: there is no cap) whose
+// proposed time p has from <= p < until, visit(T - p) when its threshold time time_of(k, r) is T < INT64_MAX, else unreached().
+// A row is on the chain only when some node committed it.  time_of: block_threshold_time with the instance's cc / times, or a
+// form that returns the same values.  The other arguments are those of commit_times_of.  Returns false when the logs of the
+// instance are not prefixes of one chain.
+template <class TimeOf, class Visit, class Unreached>
+LBFT_HD bool block_latency_samples_of(const Layout& L, const uint32_t* tb, uint32_t stride, const uint32_t* cc, const uint32_t* lc,
+                                      const int32_t* times, int64_t from, int64_t until, TimeOf time_of, Visit visit,
+                                      Unreached unreached) {
+  const uint32_t N = L.num_nodes;
+  return walk_commit_chain(L, tb, stride, cc, lc, [&](uint32_t k, uint32_t r, uint32_t) {
+    const int64_t p = times[(size_t)N * L.round_cap + r];
+    if (p < from || p >= until) return;
+    const int64_t T = time_of(k, r);
+    if (T == INT64_MAX) unreached();
+    else visit(T - p);
+  });
+}
+
 // The histogram bin of a latency: [b * w, (b + 1) * w) for b < bins - 1, the last bin also counting everything above.  (A
 // commit is never earlier than its proposal; the clamp at 0 only keeps the index inside the histogram.)
 LBFT_HD uint32_t latency_bin(int64_t lat, int64_t w, uint32_t bins) {

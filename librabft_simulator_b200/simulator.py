@@ -64,6 +64,30 @@ class LatencyStats:
         return out
 
 
+class BlockLatencyStats(LatencyStats):
+    """Block-latency statistics per group at a voting-rights threshold (``BatchResult.block_latency_stats``): the fields of
+    ``LatencyStats``, where a sample is one block's latency from its proposal to the time the nodes that committed it reach
+    ``threshold`` voting rights, plus ``unreached[groups]``, the blocks that never reached it, and the resolved integer
+    ``threshold``."""
+
+    def __init__(self, summary, unreached, hist, bin_width, threshold):
+        super().__init__(summary, hist, bin_width)
+        self.unreached = unreached
+        self.threshold = int(threshold)
+
+
+def resolve_threshold(threshold, total):
+    """A threshold of ``block_latency_stats`` as an integer weight, with ``total`` the sum of the voting rights: an int as it
+    is, or ``"first"`` (1), ``"validity"`` (f + 1: ``(total + 2) // 3``), ``"quorum"`` (``2 * total // 3 + 1``) or ``"all"``
+    (``total``)."""
+    if isinstance(threshold, str):
+        names = {"first": 1, "validity": (total + 2) // 3, "quorum": 2 * total // 3 + 1, "all": total}
+        if threshold not in names:
+            raise ValueError("threshold must be an int or one of %s, not %r" % (", ".join(map(repr, names)), threshold))
+        return names[threshold]
+    return int(threshold)
+
+
 @dataclass(frozen=True)
 class RandomDelay:
     """``RandomDelay`` (simulator.rs:39-43).  ``new`` is the reference's LogNormal; ``uniform`` is an extension."""
@@ -207,6 +231,16 @@ class BatchResult:
         in ``excluded``.  Returns a ``LatencyStats``."""
         self._check_current("latency statistics")
         return self._sim.latency_stats(num_bins, bin_width, proposed_from, proposed_until)
+
+    def block_latency_stats(self, threshold="quorum", num_bins=1024, bin_width=1, proposed_from=0, proposed_until=None):
+        """Block-latency statistics per group, reduced on the device (``lbft_block_latency_stats``; needs
+        ``commit_times=True``): one sample per block of each instance's chain (a row of its longest log) proposed in
+        ``[proposed_from, proposed_until)``, the time from its proposal until the nodes that committed it hold ``threshold``
+        voting rights.  ``threshold``: an int in 1..total voting rights, or ``"first"``, ``"validity"`` (f + 1), ``"quorum"``
+        or ``"all"`` (see ``resolve_threshold``).  Blocks that never reach it are counted in ``unreached``.  Groups, windows,
+        bins and excluded instances are those of ``latency_stats``.  Returns a ``BlockLatencyStats``."""
+        self._check_current("block latency statistics")
+        return self._sim.block_latency_stats(threshold, num_bins, bin_width, proposed_from, proposed_until)
 
     def contexts(self, instance=0):
         """The ``Vec<&Context>`` that ``loop_until`` returns for one instance."""
@@ -471,9 +505,7 @@ class BatchSimulator:
                                                int(cap)))
         return committed, proposed
 
-    def latency_stats(self, num_bins=1024, bin_width=1, proposed_from=0, proposed_until=None):
-        """``lbft_latency_stats``: per-group commit-latency statistics as a ``LatencyStats`` (see
-        ``BatchResult.latency_stats``)."""
+    def _latency_buffers(self, num_bins, bin_width, proposed_from, proposed_until):
         spec = _lib.LbftLatencySpec(struct_size=ctypes.sizeof(_lib.LbftLatencySpec), num_bins=int(num_bins), bin_width=int(bin_width),
                                     proposed_from=int(proposed_from),
                                     proposed_until=np.iinfo(np.int64).max if proposed_until is None else int(proposed_until))
@@ -481,9 +513,30 @@ class BatchSimulator:
         summary = np.zeros(groups, dtype=LATENCY_SUMMARY_DTYPE)
         # (a histogram the library refuses, num_bins out of range or num_groups * num_bins > 2^24, is not allocated here)
         hist = np.zeros((groups, spec.num_bins if 1 <= spec.num_bins and groups * spec.num_bins <= 1 << 24 else 0), dtype=np.uint64)
+        return spec, summary, hist
+
+    def latency_stats(self, num_bins=1024, bin_width=1, proposed_from=0, proposed_until=None):
+        """``lbft_latency_stats``: per-group commit-latency statistics as a ``LatencyStats`` (see
+        ``BatchResult.latency_stats``)."""
+        spec, summary, hist = self._latency_buffers(num_bins, bin_width, proposed_from, proposed_until)
         _lib.check(self._lib.lbft_latency_stats(self._handle, ctypes.byref(spec), ctypes.c_void_p(summary.ctypes.data),
                                                 ctypes.c_void_p(hist.ctypes.data) if hist.size else None))
         return LatencyStats(summary, hist, spec.bin_width)
+
+    def total_voting_rights(self):
+        """The sum of the voting rights of the committee (each node holds 1 unless ``voting_rights`` says otherwise)."""
+        return self.num_nodes if self.voting_rights is None else int(self.voting_rights.sum())
+
+    def block_latency_stats(self, threshold="quorum", num_bins=1024, bin_width=1, proposed_from=0, proposed_until=None):
+        """``lbft_block_latency_stats``: per-group block-latency statistics at a voting-rights threshold as a
+        ``BlockLatencyStats`` (see ``BatchResult.block_latency_stats``)."""
+        w = resolve_threshold(threshold, self.total_voting_rights())
+        spec, summary, hist = self._latency_buffers(num_bins, bin_width, proposed_from, proposed_until)
+        unreached = np.zeros(summary.shape[0], dtype=np.uint64)
+        _lib.check(self._lib.lbft_block_latency_stats(self._handle, ctypes.byref(spec), ctypes.c_uint64(min(max(w, 0), (1 << 64) - 1)),
+                                                      ctypes.c_void_p(summary.ctypes.data), ctypes.c_void_p(unreached.ctypes.data),
+                                                      ctypes.c_void_p(hist.ctypes.data) if hist.size else None))
+        return BlockLatencyStats(summary, unreached, hist, spec.bin_width, w)
 
     def round_switches(self, instance):
         """``DataWriter::nodes_round_switch`` of one instance as ``[(node, round, time)]``, node-major
