@@ -90,12 +90,13 @@ struct lbft_sim {
   // summaries a multi-GPU caller all-gathers travel in a single collective (lbft_device_buffer(5))
   unsigned char* d_summary = nullptr;
   size_t summary_bytes = 0;
-  lbft_commit* d_logs = nullptr;  // lbft_commit_logs: [I][logs_cap], allocated on first use
-  size_t logs_cap = 0;
+  // the read-out buffers, allocated on first use and grown by grow_buffer: each with its size in bytes
+  lbft_commit* d_logs = nullptr;  // lbft_commit_logs: [I][cap]
+  size_t logs_bytes = 0;
   int32_t* d_times = nullptr;    // LBFT_FLAG_COMMIT_TIMES: the commit-time table [I][N + 1][round_cap] (sim_core.cuh Core CT)
-  int64_t* d_times_out = nullptr;  // lbft_commit_times: [I][N][times_cap] committed, then [I][times_cap] proposed; on first use
-  size_t times_cap = 0;
-  unsigned char* d_lat = nullptr;  // lbft_latency_stats / lbft_block_latency_stats: summaries, counts and bins; on first use
+  int64_t* d_times_out = nullptr;  // lbft_commit_times: [I][N][cap] committed, then [I][cap] proposed
+  size_t times_bytes = 0;
+  unsigned char* d_lat = nullptr;  // lbft_latency_stats / lbft_block_latency_stats: summaries, unreached counts and bins
   size_t lat_bytes = 0;
   uint64_t device_bytes = 0;
   // pinned host staging: two seed buffers (lbft_set_seeds never writes the one an in-flight upload reads) and two
@@ -215,57 +216,50 @@ static int need_idle(lbft_sim* s) {
   return LBFT_OK;
 }
 
+static int create_on_device(lbft_sim* s, const lbft_config* config, lbft_sim** out_sim);
+
+// The body of lbft_create / lbft_create_sweep / lbft_create_sweep_faults: build(hs) fills the host setup of a new handle, or
+// returns false with hs.error set; then the device half.
+template <class Build>
+static int create_handle(const lbft_config* config, lbft_sim** out_sim, Build build) {
+  if (!config || !out_sim) return set_error(LBFT_ERR_INVALID, "config and out_sim must not be NULL");
+  *out_sim = nullptr;
+  lbft_sim* s = new (std::nothrow) lbft_sim();
+  if (!s) return set_error(LBFT_ERR_NOMEM, "out of host memory");
+  if (!build(s->hs)) {
+    std::string e = s->hs.error;
+    delete s;
+    return set_error(LBFT_ERR_INVALID, e);
+  }
+  return create_on_device(s, config, out_sim);
+}
+
 extern "C" {
 
 uint32_t lbft_abi_version(void) { return LBFT_ABI_VERSION; }
 const char* lbft_last_error(void) { return g_last_error.c_str(); }
 
-static int create_on_device(lbft_sim* s, const lbft_config* config, lbft_sim** out_sim);
-
 int lbft_create(const lbft_config* config, lbft_sim** out_sim) {
-  if (!config || !out_sim) return set_error(LBFT_ERR_INVALID, "config and out_sim must not be NULL");
-  *out_sim = nullptr;
-  lbft_sim* s = new (std::nothrow) lbft_sim();
-  if (!s) return set_error(LBFT_ERR_NOMEM, "out of host memory");
-  if (!s->hs.build(*config)) {
-    std::string e = s->hs.error;
-    delete s;
-    return set_error(LBFT_ERR_INVALID, e);
-  }
-  if (s->hs.params.L.epochs > 1 && (s->hs.params.record_rs || s->hs.params.resumable)) {
-    delete s;
-    return set_error(LBFT_ERR_INVALID, "recording / resumable handles need commands_per_epoch >= round_cap: the kernels with the epoch "
-                                       "machinery (node.rs:329-348) are built for plain runs only");
-  }
-  return create_on_device(s, config, out_sim);
+  return create_handle(config, out_sim, [&](HostSetup& hs) {
+    if (!hs.build(*config)) return false;
+    if (hs.params.L.epochs > 1 && (hs.params.record_rs || hs.params.resumable)) {
+      hs.error = "recording / resumable handles need commands_per_epoch >= round_cap: the kernels with the epoch machinery "
+                 "(node.rs:329-348) are built for plain runs only";
+      return false;
+    }
+    return true;
+  });
 }
 
 int lbft_create_sweep(const lbft_config* config, const lbft_param_set* sets, uint32_t num_sets, const uint32_t* set_of_instance,
                       lbft_sim** out_sim) {
-  if (!config || !out_sim) return set_error(LBFT_ERR_INVALID, "config and out_sim must not be NULL");
-  *out_sim = nullptr;
-  lbft_sim* s = new (std::nothrow) lbft_sim();
-  if (!s) return set_error(LBFT_ERR_NOMEM, "out of host memory");
-  if (!s->hs.build_sweep(*config, sets, num_sets, set_of_instance)) {
-    std::string e = s->hs.error;
-    delete s;
-    return set_error(LBFT_ERR_INVALID, e);
-  }
-  return create_on_device(s, config, out_sim);
+  return create_handle(config, out_sim, [&](HostSetup& hs) { return hs.build_sweep(*config, sets, num_sets, set_of_instance); });
 }
 
 int lbft_create_sweep_faults(const lbft_config* config, const lbft_param_set* sets, const lbft_fault_set* faults, uint32_t num_sets,
                              const uint32_t* set_of_instance, lbft_sim** out_sim) {
-  if (!config || !out_sim) return set_error(LBFT_ERR_INVALID, "config and out_sim must not be NULL");
-  *out_sim = nullptr;
-  lbft_sim* s = new (std::nothrow) lbft_sim();
-  if (!s) return set_error(LBFT_ERR_NOMEM, "out of host memory");
-  if (!s->hs.build_sweep_faults(*config, sets, faults, num_sets, set_of_instance)) {
-    std::string e = s->hs.error;
-    delete s;
-    return set_error(LBFT_ERR_INVALID, e);
-  }
-  return create_on_device(s, config, out_sim);
+  return create_handle(config, out_sim,
+                       [&](HostSetup& hs) { return hs.build_sweep_faults(*config, sets, faults, num_sets, set_of_instance); });
 }
 
 }  // extern "C"
@@ -668,16 +662,39 @@ int lbft_commit_log(lbft_sim* s, uint32_t instance, uint32_t node, lbft_commit* 
 
 }  // extern "C"
 
+// A read-out buffer grown to at least `bytes` on first use (its contents are not kept); `label` names it in the error.
+template <class T>
+static int grow_buffer(T*& buf, size_t& held, size_t bytes, const char* label) {
+  if (bytes <= held) return LBFT_OK;
+  cudaFree(buf);
+  buf = nullptr;
+  held = 0;
+  cudaError_t e = cudaMalloc((void**)&buf, bytes);
+  if (e != cudaSuccess) return set_error(LBFT_ERR_NOMEM, std::string(label) + ": " + cudaGetErrorString(e));
+  held = bytes;
+  return LBFT_OK;
+}
+
+// The end of a bulk read-out, once its copies are enqueued: waits for them and fails the call if the kernel counted, in
+// d_error, instances whose node logs are not prefixes of one chain.
+static int finish_chain_check(lbft_sim* s) {
+  uint32_t bad = 0;
+  CUDA_TRY(cudaMemcpyAsync(&bad, s->d_error, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  if (!bad) return LBFT_OK;
+  char buf[160];
+  snprintf(buf, sizeof buf, "%u instance(s) have node logs that are not prefixes of one chain: read them with lbft_commit_log", bad);
+  return set_error(LBFT_ERR_STATE, buf);
+}
+
 // ---------------------------------------------------------------------------------------------
 // Bulk read-out of the commit logs: one device pass + one device->host copy for the whole batch
 // (committed_history() of every context, simulated_context.rs:98-100; lbft_commit_log does one strided copy per
 // (instance, node) and is meant for spot checks).
 // Every commit extends the previous one by exactly one block (simulated_context.rs:172-174), so a node's log is the
 // ancestor chain of its last committed block; the kernel lays out the LONGEST log of each instance in commit order
-// and verifies that every other node's last committed block lies on it at depth == its commit count (SURVEY App.
-// C.3).  Instances where that does not hold are counted in *bad.
-// The same walk, written once for the host and the device, is sim_core.cuh walk_commit_chain (lbft_commit_times); this kernel
-// keeps its own copy so that its code stays what it was before that function existed.  The two must walk alike.
+// (sim_core.cuh walk_commit_chain, which also verifies that every other node's last committed block lies on it at
+// depth == its commit count, SURVEY App. C.3).  Instances where that does not hold are counted in *bad.
 // ---------------------------------------------------------------------------------------------
 __global__ void lbft_commit_logs_kernel(const __grid_constant__ Params P, uint32_t stride, lbft_commit* out, uint32_t cap, uint32_t* bad) {
   const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
@@ -685,31 +702,17 @@ __global__ void lbft_commit_logs_kernel(const __grid_constant__ Params P, uint32
   const Layout& L = P.L;
   const uint32_t N = L.num_nodes, tile = inst / stride, lane = inst % stride;
   const uint32_t* tb = P.state + (size_t)tile * L.total_words * stride + lane;
-  const uint32_t* cc = P.out_commit_counts + (size_t)inst * N;
-  const uint32_t* lc = P.out_lc_round + (size_t)inst * N;
-  uint32_t best = 0;
-  for (uint32_t n = 1; n < N; n++)
-    if (cc[n] > cc[best]) best = n;
-  uint32_t k = cc[best], r = lc[best], matched = 0;
   lbft_commit* row = out + (size_t)inst * cap;
-  while (r != 0 && k > 0) {
-    for (uint32_t n = 0; n < N; n++)
-      if (cc[n] == k) matched += lc[n] == r ? 1u : 0x10000u;
-    --k;
-    const uint32_t c0 = tb[(size_t)(L.chain_base + 2 * r) * stride];
-    if (k < cap) {
-      lbft_commit e;
-      e.proposer = P.leader[r % L.rspan];
-      e.index = c0 >> 16;
-      e.time = (int64_t)(int32_t)tb[(size_t)(L.chain_base + 2 * r + 1) * stride];
-      row[k] = e;
-    }
-    const uint32_t p = c0 & 0xffffu, ep = r / L.rspan;
-    r = p ? ep * L.rspan + p : (L.epochs > 1 ? tb[(size_t)(L.einit_base + ep) * stride] : 0u);
-  }
-  uint32_t empty = 0;
-  for (uint32_t n = 0; n < N; n++) empty += cc[n] == 0 ? (lc[n] == 0 ? 1u : 0x10000u) : 0u;
-  if (r != 0 || k != 0 || matched + empty != N) atomicAdd(bad, 1u);
+  if (!walk_commit_chain(L, tb, stride, P.out_commit_counts + (size_t)inst * N, P.out_lc_round + (size_t)inst * N,
+                         [&](uint32_t k, uint32_t r, uint32_t c0) {
+                           if (k >= cap) return;
+                           lbft_commit e;
+                           e.proposer = P.leader[r % L.rspan];
+                           e.index = c0 >> 16;
+                           e.time = (int64_t)(int32_t)tb[(size_t)(L.chain_base + 2 * r + 1) * stride];
+                           row[k] = e;
+                         }))
+    atomicAdd(bad, 1u);
 }
 
 int lbft_commit_logs(lbft_sim* s, lbft_commit* out, size_t cap, uint32_t* lens) {
@@ -718,30 +721,17 @@ int lbft_commit_logs(lbft_sim* s, lbft_commit* out, size_t cap, uint32_t* lens) 
   if (cap > 0xffffu) return set_error(LBFT_ERR_INVALID, "cap must be <= 65535 rows per instance");
   if (int r = need_idle(s)) return r;
   CUDA_TRY(cudaSetDevice(s->device));
-  if (cap > s->logs_cap) {
-    cudaFree(s->d_logs);
-    s->d_logs = nullptr;
-    s->logs_cap = 0;
-    cudaError_t e = cudaMalloc((void**)&s->d_logs, (size_t)s->I * cap * sizeof(lbft_commit));
-    if (e != cudaSuccess) return set_error(LBFT_ERR_NOMEM, std::string("commit-log buffer: ") + cudaGetErrorString(e));
-    s->logs_cap = cap;
-  }
+  const size_t bytes = (size_t)s->I * cap * sizeof(lbft_commit);
+  if (int r = grow_buffer(s->d_logs, s->logs_bytes, bytes, "commit-log buffer")) return r;
   // rows beyond a log's length are zero
-  CUDA_TRY(cudaMemsetAsync(s->d_logs, 0, (size_t)s->I * cap * sizeof(lbft_commit), s->stream));
+  CUDA_TRY(cudaMemsetAsync(s->d_logs, 0, bytes, s->stream));
   CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
   lbft_commit_logs_kernel<<<(s->I + 127) / 128, 128, 0, s->stream>>>(s->P, s->stride, s->d_logs, (uint32_t)cap, s->d_error);
   CUDA_TRY(cudaGetLastError());
-  uint32_t bad = 0;
-  CUDA_TRY(cudaMemcpyAsync(out, s->d_logs, (size_t)s->I * cap * sizeof(lbft_commit), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(&bad, s->d_error, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaStreamSynchronize(s->stream));
-  if (lens) memcpy(lens, s->res[s->done].commit_counts, (size_t)s->I * s->N * sizeof(uint32_t));
-  if (bad) {
-    char buf[160];
-    snprintf(buf, sizeof buf, "%u instance(s) have node logs that are not prefixes of one chain: read them with lbft_commit_log", bad);
-    return set_error(LBFT_ERR_STATE, buf);
-  }
-  return LBFT_OK;
+  CUDA_TRY(cudaMemcpyAsync(out, s->d_logs, bytes, cudaMemcpyDeviceToHost, s->stream));
+  const int r = finish_chain_check(s);  // (the lengths are returned when the chain check fails too)
+  if (lens && r != LBFT_ERR_CUDA) memcpy(lens, s->res[s->done].commit_counts, (size_t)s->I * s->N * sizeof(uint32_t));
+  return r;
 }
 
 // Bulk read-out of the commit-time table (LBFT_FLAG_COMMIT_TIMES), aligned with lbft_commit_logs: one thread per instance
@@ -767,82 +757,113 @@ __global__ void lbft_latency_init_kernel(lbft_latency_summary* sum, uint32_t gro
   }
 }
 
-// Per-group commit-latency statistics: one thread per instance walks its chain (sim_core.cuh latency_samples_of) unless its
-// status has an error bit.  Integer atomics only, so every value is exact and independent of launch shape and atomic order.
-// The kernel picks its path from what it sees:
+// The per-group reduction of both overloads of lbft_latency_stats_kernel, one object per thread: the instance it counts, the
+// samples it adds, then the block's share of the totals (finish).  Integer atomics only, so every value is exact and
+// independent of launch shape and atomic order.  The path is picked from what the block sees:
 //  * all instances of the block in one group (a plain handle, or a sweep laid out set by set as SweepSimulator.grid does) and
 //    num_bins <= kLatSharedBins: the histogram is built in shared memory (u32: a block holds at most 128 instances x 64 nodes x
 //    32 768 rows = 2^28 samples) and added to the group's with one atomic per non-zero bin;
 //  * otherwise every sample adds to its group's histogram in global memory.
 // The summary fields are summed over each warp whose lanes share a group (shuffles, then one atomic per field), else per thread.
+// kUnreached: the count of blocks that never reach the threshold, which only the threshold overload has (the per-sample one
+// compiles no shuffle or atomic for it).
 constexpr uint32_t kLatSharedBins = 8192;
 constexpr uint32_t kLatBlock = 128;
+extern __shared__ uint32_t lat_sh_bins[];
+template <bool kUnreached>
+struct LatencyReduction {
+  int64_t width;
+  uint32_t bins, g;          // g: the group of this thread's instance
+  bool shared_hist;
+  unsigned long long* gh;    // the group's histogram in global memory
+  unsigned long long clean = 0, excluded = 0, samples = 0, total = 0, unreached = 0;
+  long long lo = INT64_MAX, hi = -1;
+
+  // Every thread of the block constructs one.  first: the block's first instance; inst: this thread's, live if in the batch.
+  __device__ __forceinline__ LatencyReduction(const uint32_t* set_of, uint32_t first, uint32_t inst, bool live, int64_t width,
+                                              uint32_t bins, unsigned long long* hist)
+      : width(width), bins(bins) {
+    const uint32_t g0 = set_of ? set_of[first] : 0u;
+    g = live && set_of ? set_of[inst] : g0;
+    gh = hist + (size_t)g * bins;  // (with shared_hist, the same for every thread: g == g0)
+    shared_hist = __syncthreads_and(g == g0) && bins <= kLatSharedBins;
+    if (shared_hist) {
+      for (uint32_t b = threadIdx.x; b < bins; b += blockDim.x) lat_sh_bins[b] = 0;
+      __syncthreads();
+    }
+  }
+  // Counts a live instance as clean, or as excluded when its status has an error bit; lead: whether this thread counts it.
+  // Returns whether its chain is walked.
+  __device__ __forceinline__ bool admit(uint32_t status, bool lead) {
+    if (status & ST_ERROR_BITS) {
+      excluded = lead;
+      return false;
+    }
+    clean = lead;
+    return true;
+  }
+  __device__ __forceinline__ void add(int64_t lat) {
+    samples++;
+    total += (unsigned long long)lat;
+    lo = lat < lo ? lat : lo;
+    hi = lat > hi ? lat : hi;
+    const uint32_t b = latency_bin(lat, width, bins);
+    if (shared_hist) atomicAdd(&lat_sh_bins[b], 1u);
+    else atomicAdd(&gh[b], 1ull);
+  }
+  // Every thread of the block calls this.  unreached_out: [groups], with kUnreached only.
+  __device__ __forceinline__ void finish(lbft_latency_summary* sum, unsigned long long* unreached_out) {
+    lbft_latency_summary* gs = sum + g;
+    const uint32_t full = 0xffffffffu;
+    if (__all_sync(full, g == __shfl_sync(full, g, 0))) {
+      for (int o = 16; o > 0; o >>= 1) {
+        clean += __shfl_down_sync(full, clean, o);
+        excluded += __shfl_down_sync(full, excluded, o);
+        samples += __shfl_down_sync(full, samples, o);
+        total += __shfl_down_sync(full, total, o);
+        if constexpr (kUnreached) unreached += __shfl_down_sync(full, unreached, o);
+        lo = min(lo, __shfl_down_sync(full, lo, o));
+        hi = max(hi, __shfl_down_sync(full, hi, o));
+      }
+      if ((threadIdx.x & 31) != 0) clean = excluded = samples = unreached = 0;  // (lane 0 holds the warp's totals)
+    }
+    if (clean) atomicAdd((unsigned long long*)&gs->instances, clean);
+    if (excluded) atomicAdd((unsigned long long*)&gs->excluded, excluded);
+    if constexpr (kUnreached)
+      if (unreached) atomicAdd(&unreached_out[g], unreached);
+    if (samples) {
+      atomicAdd((unsigned long long*)&gs->samples, samples);
+      atomicAdd((unsigned long long*)&gs->sum, total);
+      atomicMin((long long*)&gs->min, lo);
+      atomicMax((long long*)&gs->max, hi);
+    }
+    if (shared_hist) {
+      __syncthreads();
+      for (uint32_t b = threadIdx.x; b < bins; b += blockDim.x)
+        if (lat_sh_bins[b]) atomicAdd(&gh[b], (unsigned long long)lat_sh_bins[b]);
+    }
+  }
+};
+
+// Per-group commit-latency statistics: one thread per instance walks its chain (sim_core.cuh latency_samples_of) unless its
+// status has an error bit, and adds every sample.
 __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __grid_constant__ Params P, uint32_t stride,
                                                                        const int32_t* times, const uint32_t* set_of, int64_t width,
                                                                        uint32_t bins, int64_t from, int64_t until,
                                                                        lbft_latency_summary* sum, unsigned long long* hist,
                                                                        uint32_t* bad) {
-  extern __shared__ uint32_t sh_bins[];
   const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
   const bool live = inst < P.num_instances;
-  const uint32_t g0 = set_of ? set_of[blockIdx.x * blockDim.x] : 0u;
-  const uint32_t g = live && set_of ? set_of[inst] : g0;
-  const bool shared_hist = __syncthreads_and(g == g0) && bins <= kLatSharedBins;
-  if (shared_hist) {
-    for (uint32_t b = threadIdx.x; b < bins; b += blockDim.x) sh_bins[b] = 0;
-    __syncthreads();
+  LatencyReduction<false> red(set_of, blockIdx.x * blockDim.x, inst, live, width, bins, hist);
+  if (live && red.admit(P.out_status[inst], true)) {
+    const Layout& L = P.L;
+    const uint32_t N = L.num_nodes, tile = inst / stride, lane = inst % stride;
+    if (!latency_samples_of(L, P.state + (size_t)tile * L.total_words * stride + lane, stride, P.out_commit_counts + (size_t)inst * N,
+                            P.out_lc_round + (size_t)inst * N, times + (size_t)inst * (N + 1) * L.round_cap, from, until,
+                            [&](int64_t lat) { red.add(lat); }))
+      atomicAdd(bad, 1u);
   }
-  unsigned long long clean = 0, excluded = 0, samples = 0, total = 0;
-  long long lo = INT64_MAX, hi = -1;
-  if (live) {
-    if (P.out_status[inst] & ST_ERROR_BITS) {
-      excluded = 1;
-    } else {
-      clean = 1;
-      const Layout& L = P.L;
-      const uint32_t N = L.num_nodes, tile = inst / stride, lane = inst % stride;
-      unsigned long long* gh = hist + (size_t)g * bins;
-      const bool ok = latency_samples_of(L, P.state + (size_t)tile * L.total_words * stride + lane, stride,
-                                         P.out_commit_counts + (size_t)inst * N, P.out_lc_round + (size_t)inst * N,
-                                         times + (size_t)inst * (N + 1) * L.round_cap, from, until, [&](int64_t lat) {
-                                           samples++;
-                                           total += (unsigned long long)lat;
-                                           lo = lat < lo ? lat : lo;
-                                           hi = lat > hi ? lat : hi;
-                                           const uint32_t b = latency_bin(lat, width, bins);
-                                           if (shared_hist) atomicAdd(&sh_bins[b], 1u);
-                                           else atomicAdd(&gh[b], 1ull);
-                                         });
-      if (!ok) atomicAdd(bad, 1u);
-    }
-  }
-  lbft_latency_summary* gs = sum + g;
-  const uint32_t full = 0xffffffffu;
-  if (__all_sync(full, g == __shfl_sync(full, g, 0))) {
-    for (int o = 16; o > 0; o >>= 1) {
-      clean += __shfl_down_sync(full, clean, o);
-      excluded += __shfl_down_sync(full, excluded, o);
-      samples += __shfl_down_sync(full, samples, o);
-      total += __shfl_down_sync(full, total, o);
-      lo = min(lo, __shfl_down_sync(full, lo, o));
-      hi = max(hi, __shfl_down_sync(full, hi, o));
-    }
-    if ((threadIdx.x & 31) != 0) clean = excluded = samples = 0;  // (lane 0 holds the warp's totals)
-  }
-  if (clean) atomicAdd((unsigned long long*)&gs->instances, clean);
-  if (excluded) atomicAdd((unsigned long long*)&gs->excluded, excluded);
-  if (samples) {
-    atomicAdd((unsigned long long*)&gs->samples, samples);
-    atomicAdd((unsigned long long*)&gs->sum, total);
-    atomicMin((long long*)&gs->min, lo);
-    atomicMax((long long*)&gs->max, hi);
-  }
-  if (shared_hist) {
-    __syncthreads();
-    unsigned long long* gh = hist + (size_t)g0 * bins;
-    for (uint32_t b = threadIdx.x; b < bins; b += blockDim.x)
-      if (sh_bins[b]) atomicAdd(&gh[b], (unsigned long long)sh_bins[b]);
-  }
+  red.finish(sum, nullptr);
 }
 
 // lbft_block_latency_stats: per-group block-latency statistics at a voting-rights threshold W (sim_core.cuh
@@ -852,211 +873,81 @@ __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __g
 // addresses: broadcast loads).  Per block, lane j loads its nodes' commit times (+inf where the node did not commit it) and
 // sums, over G width-G shuffles under the group's mask, the voting rights (P.c_weights, indexed by the source lane) of the
 // nodes with a time <= each of its own; the group then takes the least time whose sum reaches W (block_threshold_time, without
-// a per-node array), and lane 0 of the group accumulates the sample or the unreached block.  Histogram and summary paths are
-// those of the per-sample kernel: shared-memory bins when the block's instances share a group and bins <= kLatSharedBins,
-// global atomics otherwise; the summary fields are reduced per warp when its lanes share a group.  Integer atomics only.
+// a per-node array), and lane 0 of the group accumulates the sample or the unreached block into the reduction of the
+// per-sample kernel (LatencyReduction).
 __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __grid_constant__ Params P, uint32_t stride,
                                                                        const int32_t* times, const uint32_t* set_of,
                                                                        uint32_t G, uint32_t W, int64_t width, uint32_t bins,
                                                                        int64_t from, int64_t until, lbft_latency_summary* sum,
                                                                        unsigned long long* unreached_out,
                                                                        unsigned long long* hist, uint32_t* bad) {
-  extern __shared__ uint32_t sh_bins[];
   const uint32_t per_block = kLatBlock / G;
   const uint32_t j = threadIdx.x & (G - 1);  // the lane within the group
   const uint32_t inst = blockIdx.x * per_block + threadIdx.x / G;
   const bool live = inst < P.num_instances;
-  const uint32_t g0 = set_of ? set_of[blockIdx.x * per_block] : 0u;
-  const uint32_t g = live && set_of ? set_of[inst] : g0;
-  const bool shared_hist = __syncthreads_and(g == g0) && bins <= kLatSharedBins;
-  if (shared_hist) {
-    for (uint32_t b = threadIdx.x; b < bins; b += blockDim.x) sh_bins[b] = 0;
-    __syncthreads();
-  }
-  unsigned long long clean = 0, excluded = 0, samples = 0, total = 0, unreached = 0;
-  long long lo = INT64_MAX, hi = -1;
-  if (live) {
-    if (P.out_status[inst] & ST_ERROR_BITS) {
-      excluded = j == 0;
-    } else {
-      clean = j == 0;
-      const Layout& L = P.L;
-      const uint32_t N = L.num_nodes, tile = inst / stride, lane = inst % stride;
-      const uint32_t* cc = P.out_commit_counts + (size_t)inst * N;
-      const int32_t* t_inst = times + (size_t)inst * (N + 1) * L.round_cap;
-      const uint32_t warp_lane = threadIdx.x & 31;
-      const uint32_t gmask = G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (warp_lane & ~(G - 1));
-      const uint32_t n0 = j, n1 = j + 32;  // (n1 < N only when N > 32, i.e. G == 32)
-      const uint32_t cc0 = n0 < N ? cc[n0] : 0u, cc1 = n1 < N ? cc[n1] : 0u;
-      unsigned long long* gh = hist + (size_t)g * bins;
-      auto time_of = [&](uint32_t k, uint32_t r) -> int64_t {
-        const int32_t t0 = cc0 > k ? t_inst[(size_t)n0 * L.round_cap + r] : INT32_MAX;
-        const int32_t t1 = cc1 > k ? t_inst[(size_t)n1 * L.round_cap + r] : INT32_MAX;
-        uint32_t s0 = 0, s1 = 0;  // the voting rights committed at or before t0, t1 (at most 64 * 2^24)
-        for (uint32_t src = 0; src < G; src++) {
-          const int32_t u0 = __shfl_sync(gmask, t0, src, G);
-          const uint32_t v0 = u0 == INT32_MAX ? 0u : P.c_weights[src];
-          s0 += u0 <= t0 ? v0 : 0u;
-          s1 += u0 <= t1 ? v0 : 0u;
-          if (N > 32) {
-            const int32_t u1 = __shfl_sync(gmask, t1, src, G);
-            const uint32_t v1 = u1 == INT32_MAX ? 0u : P.c_weights[src + 32];
-            s0 += u1 <= t0 ? v1 : 0u;
-            s1 += u1 <= t1 ? v1 : 0u;
-          }
+  LatencyReduction<true> red(set_of, blockIdx.x * per_block, inst, live, width, bins, hist);
+  if (live && red.admit(P.out_status[inst], j == 0)) {
+    const Layout& L = P.L;
+    const uint32_t N = L.num_nodes, tile = inst / stride, lane = inst % stride;
+    const uint32_t* cc = P.out_commit_counts + (size_t)inst * N;
+    const int32_t* t_inst = times + (size_t)inst * (N + 1) * L.round_cap;
+    const uint32_t warp_lane = threadIdx.x & 31;
+    const uint32_t gmask = G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (warp_lane & ~(G - 1));
+    const uint32_t n0 = j, n1 = j + 32;  // (n1 < N only when N > 32, i.e. G == 32)
+    const uint32_t cc0 = n0 < N ? cc[n0] : 0u, cc1 = n1 < N ? cc[n1] : 0u;
+    auto time_of = [&](uint32_t k, uint32_t r) -> int64_t {
+      const int32_t t0 = cc0 > k ? t_inst[(size_t)n0 * L.round_cap + r] : INT32_MAX;
+      const int32_t t1 = cc1 > k ? t_inst[(size_t)n1 * L.round_cap + r] : INT32_MAX;
+      uint32_t s0 = 0, s1 = 0;  // the voting rights committed at or before t0, t1 (at most 64 * 2^24)
+      for (uint32_t src = 0; src < G; src++) {
+        const int32_t u0 = __shfl_sync(gmask, t0, src, G);
+        const uint32_t v0 = u0 == INT32_MAX ? 0u : P.c_weights[src];
+        s0 += u0 <= t0 ? v0 : 0u;
+        s1 += u0 <= t1 ? v0 : 0u;
+        if (N > 32) {
+          const int32_t u1 = __shfl_sync(gmask, t1, src, G);
+          const uint32_t v1 = u1 == INT32_MAX ? 0u : P.c_weights[src + 32];
+          s0 += u1 <= t0 ? v1 : 0u;
+          s1 += u1 <= t1 ? v1 : 0u;
         }
-        int32_t best = INT32_MAX;
-        if (t0 != INT32_MAX && s0 >= W) best = t0;
-        if (t1 != INT32_MAX && s1 >= W && t1 < best) best = t1;
-        for (uint32_t o = G / 2; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(gmask, best, o, G));
-        return best == INT32_MAX ? INT64_MAX : (int64_t)best;
-      };
-      const bool ok = block_latency_samples_of(
-          L, P.state + (size_t)tile * L.total_words * stride + lane, stride, cc, P.out_lc_round + (size_t)inst * N, t_inst, from,
-          until, time_of,
-          [&](int64_t lat) {
-            if (j != 0) return;
-            samples++;
-            total += (unsigned long long)lat;
-            lo = lat < lo ? lat : lo;
-            hi = lat > hi ? lat : hi;
-            const uint32_t b = latency_bin(lat, width, bins);
-            if (shared_hist) atomicAdd(&sh_bins[b], 1u);
-            else atomicAdd(&gh[b], 1ull);
-          },
-          [&]() { unreached += j == 0; });
-      if (!ok && j == 0) atomicAdd(bad, 1u);
-    }
+      }
+      int32_t best = INT32_MAX;
+      if (t0 != INT32_MAX && s0 >= W) best = t0;
+      if (t1 != INT32_MAX && s1 >= W && t1 < best) best = t1;
+      for (uint32_t o = G / 2; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(gmask, best, o, G));
+      return best == INT32_MAX ? INT64_MAX : (int64_t)best;
+    };
+    const bool ok = block_latency_samples_of(
+        L, P.state + (size_t)tile * L.total_words * stride + lane, stride, cc, P.out_lc_round + (size_t)inst * N, t_inst, from, until,
+        time_of,
+        [&](int64_t lat) {
+          if (j == 0) red.add(lat);
+        },
+        [&]() { red.unreached += j == 0; });
+    if (!ok && j == 0) atomicAdd(bad, 1u);
   }
-  lbft_latency_summary* gs = sum + g;
-  const uint32_t full = 0xffffffffu;
-  if (__all_sync(full, g == __shfl_sync(full, g, 0))) {
-    for (int o = 16; o > 0; o >>= 1) {
-      clean += __shfl_down_sync(full, clean, o);
-      excluded += __shfl_down_sync(full, excluded, o);
-      samples += __shfl_down_sync(full, samples, o);
-      total += __shfl_down_sync(full, total, o);
-      unreached += __shfl_down_sync(full, unreached, o);
-      lo = min(lo, __shfl_down_sync(full, lo, o));
-      hi = max(hi, __shfl_down_sync(full, hi, o));
-    }
-    if ((threadIdx.x & 31) != 0) clean = excluded = samples = unreached = 0;  // (lane 0 holds the warp's totals)
-  }
-  if (clean) atomicAdd((unsigned long long*)&gs->instances, clean);
-  if (excluded) atomicAdd((unsigned long long*)&gs->excluded, excluded);
-  if (unreached) atomicAdd(&unreached_out[g], unreached);
-  if (samples) {
-    atomicAdd((unsigned long long*)&gs->samples, samples);
-    atomicAdd((unsigned long long*)&gs->sum, total);
-    atomicMin((long long*)&gs->min, lo);
-    atomicMax((long long*)&gs->max, hi);
-  }
-  if (shared_hist) {
-    __syncthreads();
-    unsigned long long* gh = hist + (size_t)g0 * bins;
-    for (uint32_t b = threadIdx.x; b < bins; b += blockDim.x)
-      if (sh_bins[b]) atomicAdd(&gh[b], (unsigned long long)sh_bins[b]);
-  }
+  red.finish(sum, unreached_out);
 }
 
-// The buffer of lbft_latency_stats and lbft_block_latency_stats, grown to at least `bytes` on first use.
-static int grow_lat_buffer(lbft_sim* s, size_t bytes) {
-  if (bytes <= s->lat_bytes) return LBFT_OK;
-  cudaFree(s->d_lat);
-  s->d_lat = nullptr;
-  s->lat_bytes = 0;
-  cudaError_t e = cudaMalloc((void**)&s->d_lat, bytes);
-  if (e != cudaSuccess) return set_error(LBFT_ERR_NOMEM, std::string("latency-statistics buffer: ") + cudaGetErrorString(e));
-  s->lat_bytes = bytes;
+// The state checks of the read-outs of the commit-time table, after their NULL checks: the flag, then a finished run.
+static int need_commit_times(lbft_sim* s) {
+  if (!s->hs.sel.ct) return set_error(LBFT_ERR_STATE, "commit times were not recorded: set LBFT_FLAG_COMMIT_TIMES in lbft_config.flags");
+  if (!s->downloaded) return set_error(LBFT_ERR_STATE, "results are not available: call lbft_run first");
   return LBFT_OK;
 }
 
-extern "C" {
-
-int lbft_commit_times(lbft_sim* s, int64_t* committed, int64_t* proposed, size_t cap) {
-  if (!s || !committed) return set_error(LBFT_ERR_INVALID, "sim and committed must not be NULL");
-  if (!s->hs.sel.ct) return set_error(LBFT_ERR_STATE, "commit times were not recorded: set LBFT_FLAG_COMMIT_TIMES in lbft_config.flags");
-  if (!s->downloaded) return set_error(LBFT_ERR_STATE, "results are not available: call lbft_run first");
-  if (cap == 0 || cap > 0xffffu) return set_error(LBFT_ERR_INVALID, "cap must be in 1..65535 rows per instance");
-  if (int r = need_idle(s)) return r;
-  CUDA_TRY(cudaSetDevice(s->device));
-  const size_t I = s->I, N = s->N;
-  if (cap > s->times_cap) {
-    cudaFree(s->d_times_out);
-    s->d_times_out = nullptr;
-    s->times_cap = 0;
-    cudaError_t e = cudaMalloc((void**)&s->d_times_out, I * (N + 1) * cap * sizeof(int64_t));
-    if (e != cudaSuccess) return set_error(LBFT_ERR_NOMEM, std::string("commit-time buffer: ") + cudaGetErrorString(e));
-    s->times_cap = cap;
-  }
-  int64_t* d_committed = s->d_times_out;
-  int64_t* d_proposed = s->d_times_out + I * N * cap;
-  CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
-  lbft_commit_times_kernel<<<(s->I + 127) / 128, 128, 0, s->stream>>>(s->P, s->stride, s->d_times, (uint32_t)cap, d_committed,
-                                                                        d_proposed, s->d_error);
-  CUDA_TRY(cudaGetLastError());
-  uint32_t bad = 0;
-  CUDA_TRY(cudaMemcpyAsync(committed, d_committed, I * N * cap * sizeof(int64_t), cudaMemcpyDeviceToHost, s->stream));
-  if (proposed) CUDA_TRY(cudaMemcpyAsync(proposed, d_proposed, I * cap * sizeof(int64_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(&bad, s->d_error, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaStreamSynchronize(s->stream));
-  if (bad) {
-    char buf[160];
-    snprintf(buf, sizeof buf, "%u instance(s) have node logs that are not prefixes of one chain: read them with lbft_commit_log", bad);
-    return set_error(LBFT_ERR_STATE, buf);
-  }
-  return LBFT_OK;
-}
-
-int lbft_latency_stats(lbft_sim* s, const lbft_latency_spec* spec, lbft_latency_summary* out, uint64_t* hist) {
-  if (!s || !spec || !out) return set_error(LBFT_ERR_INVALID, "sim, spec and out must not be NULL");
-  if (!s->hs.sel.ct) return set_error(LBFT_ERR_STATE, "commit times were not recorded: set LBFT_FLAG_COMMIT_TIMES in lbft_config.flags");
-  if (!s->downloaded) return set_error(LBFT_ERR_STATE, "results are not available: call lbft_run first");
-  if (const char* e = latency_spec_error(s->hs, *spec)) return set_error(LBFT_ERR_INVALID, e);
+// lbft_latency_stats (threshold 0: the per-sample overload of lbft_latency_stats_kernel) and lbft_block_latency_stats (the
+// threshold overload), once their arguments are checked.  The buffer holds [groups] summaries, [groups] unreached counts and
+// the [groups][num_bins] bins, which lbft_latency_init_kernel sets in one pass; unreached is NULL for a per-sample call.
+static int latency_stats(lbft_sim* s, const lbft_latency_spec* spec, uint64_t threshold, lbft_latency_summary* out,
+                         uint64_t* unreached, uint64_t* hist) {
   if (int r = need_idle(s)) return r;
   CUDA_TRY(cudaSetDevice(s->device));
   const uint32_t groups = latency_groups(s->hs), bins = spec->num_bins;
   const size_t hist_len = (size_t)groups * bins;
-  if (int r = grow_lat_buffer(s, groups * sizeof(lbft_latency_summary) + hist_len * sizeof(uint64_t))) return r;
-  lbft_latency_summary* d_sum = reinterpret_cast<lbft_latency_summary*>(s->d_lat);
-  unsigned long long* d_hist = reinterpret_cast<unsigned long long*>(s->d_lat + groups * sizeof(lbft_latency_summary));
-  const size_t init_blocks = ((hist_len > groups ? hist_len : groups) + 255) / 256;
-  lbft_latency_init_kernel<<<(unsigned)(init_blocks < 4096 ? init_blocks : 4096), 256, 0, s->stream>>>(d_sum, groups, d_hist, hist_len);
-  CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
-  const size_t smem = bins <= kLatSharedBins ? bins * sizeof(uint32_t) : 0;
-  lbft_latency_stats_kernel<<<(s->I + kLatBlock - 1) / kLatBlock, kLatBlock, smem, s->stream>>>(
-      s->P, s->stride, s->d_times, s->hs.sel.sweep ? s->d_set_of : nullptr, spec->bin_width, bins, spec->proposed_from,
-      spec->proposed_until, d_sum, d_hist, s->d_error);
-  CUDA_TRY(cudaGetLastError());
-  uint32_t bad = 0;
-  CUDA_TRY(cudaMemcpyAsync(out, d_sum, groups * sizeof(lbft_latency_summary), cudaMemcpyDeviceToHost, s->stream));
-  if (hist) CUDA_TRY(cudaMemcpyAsync(hist, d_hist, hist_len * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(&bad, s->d_error, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaStreamSynchronize(s->stream));
-  if (bad) {
-    char buf[160];
-    snprintf(buf, sizeof buf, "%u instance(s) have node logs that are not prefixes of one chain: read them with lbft_commit_log", bad);
-    return set_error(LBFT_ERR_STATE, buf);
-  }
-  for (uint32_t g = 0; g < groups; g++)
-    if (out[g].samples == 0) out[g].min = -1;
-  return LBFT_OK;
-}
-
-int lbft_block_latency_stats(lbft_sim* s, const lbft_latency_spec* spec, uint64_t threshold, lbft_latency_summary* out,
-                             uint64_t* unreached, uint64_t* hist) {
-  if (!s || !spec || !out) return set_error(LBFT_ERR_INVALID, "sim, spec and out must not be NULL");
-  if (!s->hs.sel.ct) return set_error(LBFT_ERR_STATE, "commit times were not recorded: set LBFT_FLAG_COMMIT_TIMES in lbft_config.flags");
-  if (!s->downloaded) return set_error(LBFT_ERR_STATE, "results are not available: call lbft_run first");
-  if (const char* e = latency_spec_error(s->hs, *spec)) return set_error(LBFT_ERR_INVALID, e);
-  if (const char* e = block_latency_threshold_error(s->hs, threshold)) return set_error(LBFT_ERR_INVALID, e);
-  if (int r = need_idle(s)) return r;
-  CUDA_TRY(cudaSetDevice(s->device));
-  const uint32_t groups = latency_groups(s->hs), bins = spec->num_bins;
-  const size_t hist_len = (size_t)groups * bins;
-  // [groups] summaries, then [groups] unreached counts and [groups][num_bins] bins (zeroed together)
-  if (int r = grow_lat_buffer(s, groups * sizeof(lbft_latency_summary) + (groups + hist_len) * sizeof(uint64_t))) return r;
+  if (int r = grow_buffer(s->d_lat, s->lat_bytes, groups * sizeof(lbft_latency_summary) + (groups + hist_len) * sizeof(uint64_t),
+                          "latency-statistics buffer"))
+    return r;
   lbft_latency_summary* d_sum = reinterpret_cast<lbft_latency_summary*>(s->d_lat);
   unsigned long long* d_unreached = reinterpret_cast<unsigned long long*>(s->d_lat + groups * sizeof(lbft_latency_summary));
   unsigned long long* d_hist = d_unreached + groups;
@@ -1065,28 +956,65 @@ int lbft_block_latency_stats(lbft_sim* s, const lbft_latency_spec* spec, uint64_
                                                                                                        groups + hist_len);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
-  uint32_t G = 1;  // lanes per instance: the smallest power of two >= min(N, 32)
-  while (G < s->N && G < 32) G <<= 1;
-  const uint32_t per_block = kLatBlock / G;
+  const uint32_t* set_of = s->hs.sel.sweep ? s->d_set_of : nullptr;
   const size_t smem = bins <= kLatSharedBins ? bins * sizeof(uint32_t) : 0;
-  lbft_latency_stats_kernel<<<(s->I + per_block - 1) / per_block, kLatBlock, smem, s->stream>>>(
-      s->P, s->stride, s->d_times, s->hs.sel.sweep ? s->d_set_of : nullptr, G, (uint32_t)threshold, spec->bin_width, bins,
-      spec->proposed_from, spec->proposed_until, d_sum, d_unreached, d_hist, s->d_error);
+  if (threshold == 0) {
+    lbft_latency_stats_kernel<<<(s->I + kLatBlock - 1) / kLatBlock, kLatBlock, smem, s->stream>>>(
+        s->P, s->stride, s->d_times, set_of, spec->bin_width, bins, spec->proposed_from, spec->proposed_until, d_sum, d_hist,
+        s->d_error);
+  } else {
+    uint32_t G = 1;  // lanes per instance: the smallest power of two >= min(N, 32)
+    while (G < s->N && G < 32) G <<= 1;
+    const uint32_t per_block = kLatBlock / G;
+    lbft_latency_stats_kernel<<<(s->I + per_block - 1) / per_block, kLatBlock, smem, s->stream>>>(
+        s->P, s->stride, s->d_times, set_of, G, (uint32_t)threshold, spec->bin_width, bins, spec->proposed_from,
+        spec->proposed_until, d_sum, d_unreached, d_hist, s->d_error);
+  }
   CUDA_TRY(cudaGetLastError());
-  uint32_t bad = 0;
   CUDA_TRY(cudaMemcpyAsync(out, d_sum, groups * sizeof(lbft_latency_summary), cudaMemcpyDeviceToHost, s->stream));
   if (unreached) CUDA_TRY(cudaMemcpyAsync(unreached, d_unreached, groups * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
   if (hist) CUDA_TRY(cudaMemcpyAsync(hist, d_hist, hist_len * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(&bad, s->d_error, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaStreamSynchronize(s->stream));
-  if (bad) {
-    char buf[160];
-    snprintf(buf, sizeof buf, "%u instance(s) have node logs that are not prefixes of one chain: read them with lbft_commit_log", bad);
-    return set_error(LBFT_ERR_STATE, buf);
-  }
+  if (int r = finish_chain_check(s)) return r;
   for (uint32_t g = 0; g < groups; g++)
     if (out[g].samples == 0) out[g].min = -1;
   return LBFT_OK;
+}
+
+extern "C" {
+
+int lbft_commit_times(lbft_sim* s, int64_t* committed, int64_t* proposed, size_t cap) {
+  if (!s || !committed) return set_error(LBFT_ERR_INVALID, "sim and committed must not be NULL");
+  if (int r = need_commit_times(s)) return r;
+  if (cap == 0 || cap > 0xffffu) return set_error(LBFT_ERR_INVALID, "cap must be in 1..65535 rows per instance");
+  if (int r = need_idle(s)) return r;
+  CUDA_TRY(cudaSetDevice(s->device));
+  const size_t I = s->I, N = s->N;
+  if (int r = grow_buffer(s->d_times_out, s->times_bytes, I * (N + 1) * cap * sizeof(int64_t), "commit-time buffer")) return r;
+  int64_t* d_committed = s->d_times_out;
+  int64_t* d_proposed = s->d_times_out + I * N * cap;
+  CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
+  lbft_commit_times_kernel<<<(s->I + 127) / 128, 128, 0, s->stream>>>(s->P, s->stride, s->d_times, (uint32_t)cap, d_committed,
+                                                                        d_proposed, s->d_error);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemcpyAsync(committed, d_committed, I * N * cap * sizeof(int64_t), cudaMemcpyDeviceToHost, s->stream));
+  if (proposed) CUDA_TRY(cudaMemcpyAsync(proposed, d_proposed, I * cap * sizeof(int64_t), cudaMemcpyDeviceToHost, s->stream));
+  return finish_chain_check(s);
+}
+
+int lbft_latency_stats(lbft_sim* s, const lbft_latency_spec* spec, lbft_latency_summary* out, uint64_t* hist) {
+  if (!s || !spec || !out) return set_error(LBFT_ERR_INVALID, "sim, spec and out must not be NULL");
+  if (int r = need_commit_times(s)) return r;
+  if (const char* e = latency_spec_error(s->hs, *spec)) return set_error(LBFT_ERR_INVALID, e);
+  return latency_stats(s, spec, 0, out, nullptr, hist);
+}
+
+int lbft_block_latency_stats(lbft_sim* s, const lbft_latency_spec* spec, uint64_t threshold, lbft_latency_summary* out,
+                             uint64_t* unreached, uint64_t* hist) {
+  if (!s || !spec || !out) return set_error(LBFT_ERR_INVALID, "sim, spec and out must not be NULL");
+  if (int r = need_commit_times(s)) return r;
+  if (const char* e = latency_spec_error(s->hs, *spec)) return set_error(LBFT_ERR_INVALID, e);
+  if (const char* e = block_latency_threshold_error(s->hs, threshold)) return set_error(LBFT_ERR_INVALID, e);
+  return latency_stats(s, spec, threshold, out, unreached, hist);
 }
 
 int lbft_round_switches(lbft_sim* s, uint32_t instance, lbft_round_switch* out, size_t cap, size_t* n) {

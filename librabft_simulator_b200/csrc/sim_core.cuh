@@ -1948,8 +1948,7 @@ struct Core {
 // visit(k, r, c0) for row k = depth - 1, ..., 0 of that log, round r (a global round id) and r's chain word c0 (prev | cmd << 16).
 // tb: the instance's state word 0, its words `stride` apart; cc / lc: the instance's commit counts and last committed rounds.
 // Returns false unless every node's last committed block lies on that chain at depth == its commit count (SURVEY App. C.3):
-// the logs of the instance are then not prefixes of one chain.  (lbft_api.cu lbft_commit_logs_kernel keeps its own copy of this
-// walk; the two must stay alike.)
+// the logs of the instance are then not prefixes of one chain.
 template <class Visit>
 LBFT_HD bool walk_commit_chain(const Layout& L, const uint32_t* tb, uint32_t stride, const uint32_t* cc, const uint32_t* lc, Visit visit) {
   const uint32_t N = L.num_nodes;

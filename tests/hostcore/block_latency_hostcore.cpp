@@ -24,7 +24,7 @@ int block_latency_hostcore_stats(const lbft_config* c, const lbft_param_set* set
   if (const char* e = latency_spec_error(hs, *spec)) { g_ct_err = e; return LBFT_ERR_INVALID; }
   if (const char* e = block_latency_threshold_error(hs, threshold)) { g_ct_err = e; return LBFT_ERR_INVALID; }
   if (cap == 0 || cap > 0xffffu) { g_ct_err = "cap must be in 1..65535 rows per instance"; return LBFT_ERR_INVALID; }
-  const uint32_t I = c->num_instances, N = c->num_nodes, groups = latency_groups(hs), bins = spec->num_bins;
+  const uint32_t I = c->num_instances, N = c->num_nodes, groups = latency_groups(hs);
   // the run, as ct_hostcore.cpp's run_impl and fault_hostcore.cpp's fault_hostcore_run_ct make it
   std::vector<uint32_t> cc((size_t)I * N), lc((size_t)I * N), counters((size_t)I * 12), state;
   std::vector<uint64_t> ls((size_t)I * N);
@@ -36,34 +36,23 @@ int block_latency_hostcore_stats(const lbft_config* c, const lbft_param_set* set
   else if (hs.sel.sweep) run_dispatch<true>(P, N, state, times.data(), nullptr, so, hs.sets.data());
   else run_dispatch<false>(P, N, state, times.data(), nullptr, so, nullptr);
   // the commit times, and the statistics
-  std::vector<uint64_t> h((size_t)groups * bins, 0), un(groups, 0);
-  for (uint32_t g = 0; g < groups; g++) out[g] = lbft_latency_summary{0, 0, 0, 0, INT64_MAX, -1};
+  LatencyAccumulator acc(out, groups, *spec);
+  std::vector<uint64_t> un(groups, 0);
   for (uint32_t i = 0; i < I; i++) {
     const uint32_t* tb = state.data() + (size_t)(i / 32) * L.total_words * 32 + i % 32;
     const uint32_t *icc = cc.data() + (size_t)i * N, *ilc = lc.data() + (size_t)i * N;
     const int32_t* t = times.data() + (size_t)i * (N + 1) * L.round_cap;
     const bool ok = commit_times_of(L, tb, 32, icc, ilc, t, (uint32_t)cap, committed + (size_t)i * N * cap, proposed + (size_t)i * cap);
     const uint32_t g = so ? so[i] : 0u;
-    lbft_latency_summary& s = out[g];
-    if (status[i] & ST_ERROR_BITS) { s.excluded++; continue; }
+    if (!acc.admit(g, status[i])) continue;
     if (!ok) { g_ct_err = "node logs that are not prefixes of one chain"; return LBFT_ERR_STATE; }
-    s.instances++;
     block_latency_samples_of(
         L, tb, 32, icc, ilc, t, spec->proposed_from, spec->proposed_until,
         [&](uint32_t k, uint32_t r) { return block_threshold_time(L, icc, t, P.c_weights, k, r, threshold); },
-        [&](int64_t lat) {
-          s.samples++;
-          s.sum += (uint64_t)lat;
-          s.min = lat < s.min ? lat : s.min;
-          s.max = lat > s.max ? lat : s.max;
-          h[(size_t)g * bins + latency_bin(lat, spec->bin_width, bins)]++;
-        },
-        [&]() { un[g]++; });
+        [&](int64_t lat) { acc.add(g, lat); }, [&]() { un[g]++; });
   }
-  for (uint32_t g = 0; g < groups; g++)
-    if (out[g].samples == 0) out[g].min = -1;
+  acc.finish(hist);
   if (unreached) std::copy(un.begin(), un.end(), unreached);
-  if (hist) std::copy(h.begin(), h.end(), hist);
   return LBFT_OK;
 }
 

@@ -108,6 +108,41 @@ int run_impl(lbft::HostSetup& hs, const lbft_config* c, const uint64_t* first_se
     }
   return LBFT_OK;
 }
+
+// The per-group accumulation of lbft_latency_stats_kernel, for the latency harnesses: summaries out[groups] and the bins of
+// `spec`.  admit() counts an instance as clean or excluded and says whether its chain is walked, add() folds in one sample,
+// finish() copies the bins to hist (may be NULL) and turns min into -1 for an empty group.
+struct LatencyAccumulator {
+  lbft_latency_summary* out;
+  uint32_t groups;
+  lbft_latency_spec spec;
+  std::vector<uint64_t> h;
+  LatencyAccumulator(lbft_latency_summary* out, uint32_t groups, const lbft_latency_spec& spec)
+      : out(out), groups(groups), spec(spec), h((size_t)groups * spec.num_bins, 0) {
+    for (uint32_t g = 0; g < groups; g++) out[g] = lbft_latency_summary{0, 0, 0, 0, INT64_MAX, -1};
+  }
+  bool admit(uint32_t g, uint32_t status) {
+    if (status & lbft::ST_ERROR_BITS) {
+      out[g].excluded++;
+      return false;
+    }
+    out[g].instances++;
+    return true;
+  }
+  void add(uint32_t g, int64_t lat) {
+    lbft_latency_summary& s = out[g];
+    s.samples++;
+    s.sum += (uint64_t)lat;
+    s.min = lat < s.min ? lat : s.min;
+    s.max = lat > s.max ? lat : s.max;
+    h[(size_t)g * spec.num_bins + lbft::latency_bin(lat, spec.bin_width, spec.num_bins)]++;
+  }
+  void finish(uint64_t* hist) {
+    for (uint32_t g = 0; g < groups; g++)
+      if (out[g].samples == 0) out[g].min = -1;
+    if (hist) std::copy(h.begin(), h.end(), hist);
+  }
+};
 }  // namespace
 
 extern "C" {

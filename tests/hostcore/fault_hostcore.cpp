@@ -135,28 +135,16 @@ int fault_hostcore_run_ct(const lbft_config* c, const lbft_param_set* sets, cons
     }
   }
   if (!spec) return LBFT_OK;
-  const uint32_t bins = spec->num_bins;
-  std::vector<uint64_t> h((size_t)num_sets * bins, 0);
-  for (uint32_t g = 0; g < num_sets; g++) out[g] = lbft_latency_summary{0, 0, 0, 0, INT64_MAX, -1};
+  LatencyAccumulator acc(out, num_sets, *spec);
   for (uint32_t i = 0; i < I; i++) {
     const uint32_t g = set_of[i];
-    lbft_latency_summary& s = out[g];
-    if (status[i] & ST_ERROR_BITS) { s.excluded++; continue; }
-    s.instances++;
+    if (!acc.admit(g, status[i])) continue;
     const bool ok = latency_samples_of(L, state.data() + (size_t)(i / 32) * L.total_words * 32 + i % 32, 32, commit_counts + (size_t)i * N,
                                        lc_round + (size_t)i * N, times.data() + (size_t)i * (N + 1) * L.round_cap, spec->proposed_from,
-                                       spec->proposed_until, [&](int64_t lat) {
-                                         s.samples++;
-                                         s.sum += (uint64_t)lat;
-                                         s.min = lat < s.min ? lat : s.min;
-                                         s.max = lat > s.max ? lat : s.max;
-                                         h[(size_t)g * bins + latency_bin(lat, spec->bin_width, bins)]++;
-                                       });
+                                       spec->proposed_until, [&](int64_t lat) { acc.add(g, lat); });
     if (!ok) { g_ct_err = "node logs that are not prefixes of one chain"; return LBFT_ERR_STATE; }
   }
-  for (uint32_t g = 0; g < num_sets; g++)
-    if (out[g].samples == 0) out[g].min = -1;
-  if (hist) std::copy(h.begin(), h.end(), hist);
+  acc.finish(hist);
   return LBFT_OK;
 }
 }  // extern "C"

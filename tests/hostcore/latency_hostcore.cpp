@@ -16,7 +16,7 @@ int latency_hostcore_stats(const lbft_config* c, const lbft_param_set* sets, uin
   if (!(sets ? hs.build_sweep(*c, sets, num_sets, set_of) : hs.build(*c))) { g_ct_err = hs.error; return LBFT_ERR_INVALID; }
   if (!hs.sel.ct) { g_ct_err = "commit times were not recorded: set LBFT_FLAG_COMMIT_TIMES in lbft_config.flags"; return LBFT_ERR_STATE; }
   if (const char* e = latency_spec_error(hs, *spec)) { g_ct_err = e; return LBFT_ERR_INVALID; }
-  const uint32_t I = c->num_instances, N = c->num_nodes, groups = latency_groups(hs), bins = spec->num_bins;
+  const uint32_t I = c->num_instances, N = c->num_nodes, groups = latency_groups(hs);
   // the run, as ct_hostcore.cpp's run_impl makes it
   Params P = hs.params;
   P.zig_x = hs.zig_x.data();
@@ -43,27 +43,16 @@ int latency_hostcore_stats(const lbft_config* c, const lbft_param_set* sets, uin
   if (hs.sel.sweep) run_dispatch<true>(P, N, state, times.data(), nullptr, so, ss);
   else run_dispatch<false>(P, N, state, times.data(), nullptr, so, ss);
   // the statistics
-  std::vector<uint64_t> h((size_t)groups * bins, 0);
-  for (uint32_t g = 0; g < groups; g++) out[g] = lbft_latency_summary{0, 0, 0, 0, INT64_MAX, -1};
+  LatencyAccumulator acc(out, groups, *spec);
   for (uint32_t i = 0; i < I; i++) {
     const uint32_t g = so ? so[i] : 0u;
-    lbft_latency_summary& s = out[g];
-    if (status[i] & ST_ERROR_BITS) { s.excluded++; continue; }
-    s.instances++;
+    if (!acc.admit(g, status[i])) continue;
     const bool ok = latency_samples_of(L, state.data() + (size_t)(i / 32) * L.total_words * 32 + i % 32, 32, cc.data() + (size_t)i * N,
                                        lc.data() + (size_t)i * N, times.data() + (size_t)i * (N + 1) * L.round_cap, spec->proposed_from,
-                                       spec->proposed_until, [&](int64_t lat) {
-                                         s.samples++;
-                                         s.sum += (uint64_t)lat;
-                                         s.min = lat < s.min ? lat : s.min;
-                                         s.max = lat > s.max ? lat : s.max;
-                                         h[(size_t)g * bins + latency_bin(lat, spec->bin_width, bins)]++;
-                                       });
+                                       spec->proposed_until, [&](int64_t lat) { acc.add(g, lat); });
     if (!ok) { g_ct_err = "node logs that are not prefixes of one chain"; return LBFT_ERR_STATE; }
   }
-  for (uint32_t g = 0; g < groups; g++)
-    if (out[g].samples == 0) out[g].min = -1;
-  if (hist) std::copy(h.begin(), h.end(), hist);
+  acc.finish(hist);
   return LBFT_OK;
 }
 
