@@ -3,7 +3,8 @@
 * ``csrc/liblbft_b200.so`` — the product: sm_90a (H100) CUDA kernels + the C ABI of ``include/lbft.h``.
 * ``oracle/liblbft_oracle.so``, ``tests/hostcore/libhostcore.so``, ``tests/hostcore/libhostcore_sweep.so``,
   ``tests/hostcore/libhostcore_ct.so``, ``tests/hostcore/libhostcore_latency.so``, ``tests/hostcore/libhostcore_fault.so`` and
-  ``tests/hostcore/libhostcore_block_latency.so`` — test infrastructure only.
+  ``tests/hostcore/libhostcore_block_latency.so`` — test infrastructure only; so is ``tests/gpuprobe/libblock_threshold_probe.so``,
+  a CUDA probe of one device function.
 All artefacts are built in-tree and git-ignored.
 """
 import os
@@ -22,6 +23,8 @@ CT_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_ct.so")
 LATENCY_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_latency.so")
 FAULT_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_fault.so")
 BLOCK_LATENCY_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_block_latency.so")
+GPUPROBE_DIR = os.path.join(ROOT, "tests", "gpuprobe")
+BLOCK_THRESHOLD_PROBE_PATH = os.path.join(GPUPROBE_DIR, "libblock_threshold_probe.so")
 
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
@@ -192,6 +195,18 @@ def build_block_latency_hostcore(force=False):
     return BLOCK_LATENCY_HOSTCORE_PATH
 
 
+def build_block_threshold_probe(force=False):
+    """The lane form of the block threshold time (sim_core.cuh block_threshold_time_lanes) over synthetic tables on the device
+    (tests/gpuprobe/block_threshold_probe.cu), with the product's nvcc flags: test infrastructure, never linked into the
+    product library."""
+    srcs = [os.path.join(GPUPROBE_DIR, "block_threshold_probe.cu")] + [os.path.join(CSRC, f) for f in ("sim_core.cuh", "sim_params.h")]
+    if not force and _newer(BLOCK_THRESHOLD_PROBE_PATH, srcs):
+        return BLOCK_THRESHOLD_PROBE_PATH
+    _run([nvcc_path()] + NVCC_FLAGS + ["-shared", "-o", BLOCK_THRESHOLD_PROBE_PATH, "block_threshold_probe.cu"], GPUPROBE_DIR)
+    return BLOCK_THRESHOLD_PROBE_PATH
+
+
 def build_all(force=False):
     return (build_product(force), build_oracle(force), build_hostcore(force), build_sweep_hostcore(force), build_ct_hostcore(force),
-            build_latency_hostcore(force), build_fault_hostcore(force), build_block_latency_hostcore(force))
+            build_latency_hostcore(force), build_fault_hostcore(force), build_block_latency_hostcore(force),
+            build_block_threshold_probe(force))

@@ -872,9 +872,9 @@ __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __g
 // power of two >= min(N, 32), so lane j holds nodes j and, when N > 32, j + 32.  Every lane of the group walks the chain (same
 // addresses: broadcast loads).  Per block, lane j loads its nodes' commit times (+inf where the node did not commit it) and
 // sums, over G width-G shuffles under the group's mask, the voting rights (P.c_weights, indexed by the source lane) of the
-// nodes with a time <= each of its own; the group then takes the least time whose sum reaches W (block_threshold_time, without
-// a per-node array), and lane 0 of the group accumulates the sample or the unreached block into the reduction of the
-// per-sample kernel (LatencyReduction).
+// nodes with a time <= each of its own; the group then takes the least time whose sum reaches W (sim_core.cuh
+// block_threshold_time_lanes: block_threshold_time without a per-node array), and lane 0 of the group accumulates the sample or
+// the unreached block into the reduction of the per-sample kernel (LatencyReduction).
 __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __grid_constant__ Params P, uint32_t stride,
                                                                        const int32_t* times, const uint32_t* set_of,
                                                                        uint32_t G, uint32_t W, int64_t width, uint32_t bins,
@@ -896,26 +896,7 @@ __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __g
     const uint32_t n0 = j, n1 = j + 32;  // (n1 < N only when N > 32, i.e. G == 32)
     const uint32_t cc0 = n0 < N ? cc[n0] : 0u, cc1 = n1 < N ? cc[n1] : 0u;
     auto time_of = [&](uint32_t k, uint32_t r) -> int64_t {
-      const int32_t t0 = cc0 > k ? t_inst[(size_t)n0 * L.round_cap + r] : INT32_MAX;
-      const int32_t t1 = cc1 > k ? t_inst[(size_t)n1 * L.round_cap + r] : INT32_MAX;
-      uint32_t s0 = 0, s1 = 0;  // the voting rights committed at or before t0, t1 (at most 64 * 2^24)
-      for (uint32_t src = 0; src < G; src++) {
-        const int32_t u0 = __shfl_sync(gmask, t0, src, G);
-        const uint32_t v0 = u0 == INT32_MAX ? 0u : P.c_weights[src];
-        s0 += u0 <= t0 ? v0 : 0u;
-        s1 += u0 <= t1 ? v0 : 0u;
-        if (N > 32) {
-          const int32_t u1 = __shfl_sync(gmask, t1, src, G);
-          const uint32_t v1 = u1 == INT32_MAX ? 0u : P.c_weights[src + 32];
-          s0 += u1 <= t0 ? v1 : 0u;
-          s1 += u1 <= t1 ? v1 : 0u;
-        }
-      }
-      int32_t best = INT32_MAX;
-      if (t0 != INT32_MAX && s0 >= W) best = t0;
-      if (t1 != INT32_MAX && s1 >= W && t1 < best) best = t1;
-      for (uint32_t o = G / 2; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(gmask, best, o, G));
-      return best == INT32_MAX ? INT64_MAX : (int64_t)best;
+      return block_threshold_time_lanes(L, G, gmask, j, cc0, cc1, t_inst, P.c_weights, k, r, W);
     };
     const bool ok = block_latency_samples_of(
         L, P.state + (size_t)tile * L.total_words * stride + lane, stride, cc, P.out_lc_round + (size_t)inst * N, t_inst, from, until,

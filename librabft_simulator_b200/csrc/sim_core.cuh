@@ -2024,6 +2024,40 @@ LBFT_HD int64_t block_threshold_time(const Layout& L, const uint32_t* cc, const 
   return T;
 }
 
+#if defined(__CUDACC__)
+// The lane form of block_threshold_time, which the threshold overload of lbft_latency_stats_kernel runs: every lane of a group
+// of G lanes (G a power of two, the smallest >= min(N, 32); gmask: the group's lanes in the warp) calls it and gets T.  Lane j
+// holds node j and, when N > 32 (so G == 32), node j + 32; cc0 / cc1 are their commit counts (0 for a node it does not hold).
+// times, w, k, r and W are those of block_threshold_time.  Each lane loads its nodes' times (INT32_MAX where the node did not
+// commit row k), sums over G width-G shuffles the voting rights (indexed by the source lane) of the nodes with a time <= each
+// of its own, and the group takes the least time whose sum reaches W with an xor-shuffle minimum.
+__device__ __forceinline__ int64_t block_threshold_time_lanes(const Layout& L, uint32_t G, uint32_t gmask, uint32_t j, uint32_t cc0,
+                                                              uint32_t cc1, const int32_t* times, const uint32_t* w, uint32_t k,
+                                                              uint32_t r, uint32_t W) {
+  const uint32_t N = L.num_nodes, n0 = j, n1 = j + 32;  // (n1 < N only when N > 32, i.e. G == 32)
+  const int32_t t0 = cc0 > k ? times[(size_t)n0 * L.round_cap + r] : INT32_MAX;
+  const int32_t t1 = cc1 > k ? times[(size_t)n1 * L.round_cap + r] : INT32_MAX;
+  uint32_t s0 = 0, s1 = 0;  // the voting rights committed at or before t0, t1 (at most 64 * 2^24)
+  for (uint32_t src = 0; src < G; src++) {
+    const int32_t u0 = __shfl_sync(gmask, t0, src, G);
+    const uint32_t v0 = u0 == INT32_MAX ? 0u : w[src];
+    s0 += u0 <= t0 ? v0 : 0u;
+    s1 += u0 <= t1 ? v0 : 0u;
+    if (N > 32) {
+      const int32_t u1 = __shfl_sync(gmask, t1, src, G);
+      const uint32_t v1 = u1 == INT32_MAX ? 0u : w[src + 32];
+      s0 += u1 <= t0 ? v1 : 0u;
+      s1 += u1 <= t1 ? v1 : 0u;
+    }
+  }
+  int32_t best = INT32_MAX;
+  if (t0 != INT32_MAX && s0 >= W) best = t0;
+  if (t1 != INT32_MAX && s1 >= W && t1 < best) best = t1;
+  for (uint32_t o = G / 2; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(gmask, best, o, G));
+  return best == INT32_MAX ? INT64_MAX : (int64_t)best;
+}
+#endif
+
 // lbft_block_latency_stats for one instance: for every row k of its chain (walk_commit_chain, every row: there is no cap) whose
 // proposed time p has from <= p < until, visit(T - p) when its threshold time time_of(k, r) is T < INT64_MAX, else unreached().
 // A row is on the chain only when some node committed it.  time_of: block_threshold_time with the instance's cc / times, or a

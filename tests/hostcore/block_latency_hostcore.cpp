@@ -2,8 +2,9 @@
 // ct_hostcore.cpp (plain handles and sweeps) and fault_hostcore.cpp (fault sweeps), compiled into this unit as they are, run over
 // the product's host setup; then the product's spec and threshold checks (latency_spec_error, block_latency_threshold_error) and
 // per-instance walk (block_latency_samples_of with the serial block_threshold_time, latency_bin) into a host accumulator, with
-// the grouping and exclusion rules of the kernel (the threshold overload of lbft_latency_stats_kernel).  Never part of, linked
-// into, or reachable from the product library.
+// the grouping and exclusion rules of the kernel (the threshold overload of lbft_latency_stats_kernel); and block_threshold_time
+// alone over synthetic tables, the reference of the device probe of its lane form.  Never part of, linked into, or reachable
+// from the product library.
 #include "fault_hostcore.cpp"
 
 extern "C" {
@@ -53,6 +54,22 @@ int block_latency_hostcore_stats(const lbft_config* c, const lbft_param_set* set
   }
   acc.finish(hist);
   if (unreached) std::copy(un.begin(), un.end(), unreached);
+  return LBFT_OK;
+}
+
+// The serial block_threshold_time over synthetic tables laid out as tests/gpuprobe/block_threshold_probe.cu takes them: cc
+// [I][N], times [I][N + 1][round_cap], w [N], W [I]; for every row r, k = r.  T: [I][round_cap], INT64_MAX when unreached.
+int block_threshold_hostcore_times(uint32_t N, uint32_t I, uint32_t round_cap, const uint32_t* cc, const int32_t* times,
+                                   const uint32_t* w, const uint64_t* W, int64_t* T) {
+  using namespace lbft;
+  if (N < 1 || N > 64 || round_cap < 1) { g_ct_err = "N must be in 1..64 and round_cap >= 1"; return LBFT_ERR_INVALID; }
+  Layout L{};
+  L.num_nodes = N;
+  L.round_cap = round_cap;
+  for (uint32_t i = 0; i < I; i++)
+    for (uint32_t r = 0; r < round_cap; r++)
+      T[(size_t)i * round_cap + r] =
+          block_threshold_time(L, cc + (size_t)i * N, times + (size_t)i * (N + 1) * round_cap, w, r, r, W[i]);
   return LBFT_OK;
 }
 

@@ -2,12 +2,14 @@
 runs the entry's kernel, no instance ends with an error bit, and the oracle agrees bit for bit on commit counts, state keys,
 counters, the epoch-change bit and the commit logs of the instances it checks.  Where the oracle checks a sample of a large
 batch, the whole batch is compared with the same seeds through another instantiation (results depend on the seed alone).
-Recording, resumable, true-data-sync and commit-times kernels are also checked on what only they produce."""
+Recording, resumable, true-data-sync and commit-times kernels are also checked on what only they produce; on the commit-times
+twins that includes both latency read-outs, so every lane-group width of the block-latency reduction (N = 1 .. 64) runs here."""
 import numpy as np
 import pytest
 
 from librabft_simulator_b200 import SweepSimulator, _lib
 from tests import fault_support, sweep_support
+from tests.block_latency_support import assert_same_block_stats, numpy_block_stats, thresholds
 from tests.ct_support import CtHarness
 from tests.kernel_matrix import CT, MATRIX, REC, RES, TDS, flag_off
 from tests.latency_support import numpy_stats
@@ -171,8 +173,9 @@ def check_stops_and_snapshot(oracle, e, sim, idx):
 
 
 def check_commit_times(ct, e, monkeypatch, res, idx):
-    """Commit times against the oracle observed event by event; the latency statistics against numpy over the handle's own
-    commit times (a window and an overflowing last bin); every other output as the flag-off kernel's on the same seeds."""
+    """Commit times against the oracle observed event by event; the per-sample and block latency statistics against numpy over
+    the handle's own commit times (a window and an overflowing last bin); every other output as the flag-off kernel's on the
+    same seeds."""
     off_entry = flag_off(e)
     off, off_res = run(off_entry, monkeypatch, off_entry.force)
     try:
@@ -197,3 +200,29 @@ def check_commit_times(ct, e, monkeypatch, res, idx):
         np.testing.assert_array_equal(getattr(got, f), getattr(want, f), err_msg=f)
     assert got.samples.sum() > 0, "no commit latency in the window"
     assert got.hist[:, -1].sum() > 0, "no latency overflowed the last bin"
+    check_block_latency(e, res, committed, proposed, group_of, ngroups, spec)
+
+
+def check_block_latency(e, res, committed, proposed, group_of, ngroups, spec):
+    """Block latency at the named thresholds, one in between and total - 1, field by field against numpy over the same commit
+    times, with the invariants across thresholds; on a single-group entry also with 8 193 bins (the global histogram)."""
+    weights = np.asarray(e.kw.get("voting_rights", [1] * e.N), np.int64)
+    total = int(weights.sum())
+    ws = sorted(set(thresholds(total)) | ({total - 1} if total > 1 else set()))
+    stats = {}
+    for w in ws:
+        got = res.block_latency_stats(w, **spec)
+        want = numpy_block_stats(committed, proposed, res.status, group_of, ngroups, weights, w, **spec)
+        assert_same_block_stats(got, want, "W=%d" % w)
+        stats[w] = got
+    blocks = stats[ws[0]].samples + stats[ws[0]].unreached
+    for a, b in zip(ws, ws[1:]):
+        np.testing.assert_array_equal(stats[b].samples + stats[b].unreached, blocks, err_msg="blocks at W=%d" % b)
+        assert (stats[b].samples <= stats[a].samples).all(), (a, b)
+    assert ws[0] == 1 and (stats[1].unreached == 0).all()
+    assert blocks.sum() > 0, "no block in the window"
+    if ngroups == 1:
+        wide = dict(spec, num_bins=8193)
+        for w in (1, ws[len(ws) // 2], total):
+            want = numpy_block_stats(committed, proposed, res.status, group_of, ngroups, weights, w, **wide)
+            assert_same_block_stats(res.block_latency_stats(w, **wide), want, "8 193 bins, W=%d" % w)
