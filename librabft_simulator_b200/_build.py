@@ -2,8 +2,8 @@
 
 * ``csrc/liblbft_b200.so`` — the product: sm_90a (H100) CUDA kernels + the C ABI of ``include/lbft.h``.
 * ``oracle/liblbft_oracle.so``, ``tests/hostcore/libhostcore.so``, ``tests/hostcore/libhostcore_sweep.so``,
-  ``tests/hostcore/libhostcore_ct.so``, ``tests/hostcore/libhostcore_latency.so``, ``tests/hostcore/libhostcore_fault.so`` and
-  ``tests/hostcore/libhostcore_block_latency.so`` — test infrastructure only; so is ``tests/gpuprobe/libblock_threshold_probe.so``,
+  ``tests/hostcore/libhostcore_ct.so``, ``tests/hostcore/libhostcore_latency.so``, ``tests/hostcore/libhostcore_fault.so``,
+  ``tests/hostcore/libhostcore_block_latency.so`` and ``tests/hostcore/libhostcore_lane_block.so`` — test infrastructure only; so is ``tests/gpuprobe/libblock_threshold_probe.so``,
   a CUDA probe of one device function.
 All artefacts are built in-tree and git-ignored.
 """
@@ -23,6 +23,7 @@ CT_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_ct.so")
 LATENCY_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_latency.so")
 FAULT_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_fault.so")
 BLOCK_LATENCY_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_block_latency.so")
+LANE_BLOCK_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_lane_block.so")
 GPUPROBE_DIR = os.path.join(ROOT, "tests", "gpuprobe")
 BLOCK_THRESHOLD_PROBE_PATH = os.path.join(GPUPROBE_DIR, "libblock_threshold_probe.so")
 
@@ -195,6 +196,18 @@ def build_block_latency_hostcore(force=False):
     return BLOCK_LATENCY_HOSTCORE_PATH
 
 
+def build_lane_block_hostcore(force=False):
+    """The bench kernel's core with its compact node words and slots in lane blocks (tests/hostcore/lane_block_hostcore.cpp):
+    test infrastructure."""
+    srcs = [os.path.join(HOSTCORE_DIR, "lane_block_hostcore.cpp")] + [
+        os.path.join(CSRC, f) for f in ("sim_core.cuh", "sim_params.h", "host_setup.hpp")]
+    if not force and _newer(LANE_BLOCK_HOSTCORE_PATH, srcs):
+        return LANE_BLOCK_HOSTCORE_PATH
+    _run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-DLBFT_CHECK_C1",
+          "-o", LANE_BLOCK_HOSTCORE_PATH, "lane_block_hostcore.cpp"], HOSTCORE_DIR)
+    return LANE_BLOCK_HOSTCORE_PATH
+
+
 def build_block_threshold_probe(force=False):
     """The lane form of the block threshold time (sim_core.cuh block_threshold_time_lanes) over synthetic tables on the device
     (tests/gpuprobe/block_threshold_probe.cu), with the product's nvcc flags: test infrastructure, never linked into the
@@ -209,4 +222,4 @@ def build_block_threshold_probe(force=False):
 def build_all(force=False):
     return (build_product(force), build_oracle(force), build_hostcore(force), build_sweep_hostcore(force), build_ct_hostcore(force),
             build_latency_hostcore(force), build_fault_hostcore(force), build_block_latency_hostcore(force),
-            build_block_threshold_probe(force))
+            build_lane_block_hostcore(force), build_block_threshold_probe(force))

@@ -61,7 +61,9 @@ __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, d
   const uint32_t inst = tile * TILE + lane;
   if (lane >= TILE || inst >= P.num_instances) return;
   const uint32_t total_words = FX ? fixed_layout(FX).total_words : P.L.total_words;
-  TileMem<TILE> mem{P.state + (size_t)tile * total_words * TILE, lane};
+  // the compact encoding (FX_DEFAULT4, Core::PACK) keeps its node words and slots in lane blocks (TileMem LB)
+  using Mem = TileMem<TILE, FX == FX_DEFAULT4>;
+  Mem mem{P.state + (size_t)tile * total_words * TILE, lane};
   uint32_t* sk = nullptr;
   uint16_t* sd = nullptr;
   if (QMODE == 2) {
@@ -73,7 +75,7 @@ __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, d
   // sparse tiles over the calendar queue: the kind-occupancy words of the tile's instances in shared memory, a column per
   // lane (sim_core.cuh KS; the host only selects sparse tiles when 14 warps' worth fits, host_setup.hpp)
   constexpr bool KS = QMODE == 3 && TILE < 32;
-  Core<TileMem<TILE>, NMAX, QMODE, FX, REC, RES, 1, EP, TDS, KS, SW, CT> core(P, mem, s_zx, s_zf, thr_fits ? s_thr : P.delay_thr, sk, sd);
+  Core<Mem, NMAX, QMODE, FX, REC, RES, 1, EP, TDS, KS, SW, CT> core(P, mem, s_zx, s_zf, thr_fits ? s_thr : P.delay_thr, sk, sd);
   if (KS) core.km = s_queue + (size_t)(threadIdx.x >> 5) * calendar_kmask_words(FX ? fixed_layout(FX) : P.L) * TILE + lane;
   if constexpr (CT) core.ct = times + (size_t)inst * (core.L.num_nodes + 1) * core.L.round_cap;
   if constexpr (SW) {

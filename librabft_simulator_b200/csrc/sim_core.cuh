@@ -160,15 +160,27 @@ struct SipWords {
 // (word w -> tile[w*STRIDE + lane]); the scan queue's 64-bit entries are interleaved at 8-byte granularity
 // (entry j of the region starting at word wbase -> tile[wbase*STRIDE + j*2*STRIDE + lane*2 .. +1]), so a warp
 // reading entry j issues one 256-byte coalesced access.
-template <int STRIDE_>
+// LB ("lane blocks", the bench kernel's compact encoding, Core::PACK): a compact block of K words (a node's compact words, a
+// notification slot) keeps the K rows x STRIDE lanes it owns, but each lane's K words are contiguous in them, so that a thread
+// moves its block with 128-bit accesses where its lanes touch different blocks.  Every other word is interleaved as above.
+template <int STRIDE_, bool LB_ = false>
 struct TileMem {
   static constexpr int STRIDE = STRIDE_;
+  static constexpr bool LB = LB_;
+  static constexpr int BLOCK_PITCH = LB ? 1 : STRIDE;  // words between consecutive words of a block (block())
   uint32_t* tile;  // first word of the tile
   uint32_t lane;
   LBFT_HD uint32_t* at(uint32_t w) const { return tile + (size_t)w * STRIDE + lane; }  // then p[k * STRIDE]
   LBFT_HD uint32_t ld(uint32_t w) const { return tile[(size_t)w * STRIDE + lane]; }
   LBFT_HD void st(uint32_t w, uint32_t v) const { tile[(size_t)w * STRIDE + lane] = v; }
   LBFT_HD uint64_t* at64(uint32_t wbase) const { return reinterpret_cast<uint64_t*>(tile + (size_t)wbase * STRIDE + lane * 2); }  // then q[j * STRIDE]
+  // Where word k of `lane`'s block lives in the region of K-word blocks that starts at word `base`: the tile offset
+  // (base + k) * STRIDE + lane interleaved, base * STRIDE + lane * K + k in lane blocks.  The one definition of the mapping
+  // (the host tests map lane-block states back to the interleaved form through it).
+  LBFT_HD static constexpr size_t block_word(uint32_t base, uint32_t K, uint32_t k, uint32_t lane) {
+    return LB ? (size_t)base * STRIDE + lane * K + k : ((size_t)base + k) * STRIDE + lane;
+  }
+  LBFT_HD uint32_t* block(uint32_t base, uint32_t K) const { return tile + block_word(base, K, 0, lane); }  // then p[k * BLOCK_PITCH]
 };
 
 // List of authors used for the shuffled fan-out (simulator.rs:326-343, 356-370).
@@ -630,6 +642,8 @@ struct Core {
   // dropped at a stop must be the one the reference drops).
   static constexpr bool ELIDE = !(REC || RES);
   static constexpr int S = Mem::STRIDE;
+  static_assert(!Mem::LB || PACK, "lane blocks: the compact node words and slots only");
+  static constexpr int PS = Mem::BLOCK_PITCH;  // PACK: words between consecutive words of a compact node block or slot
   const Params& P;
   const Layout L;
   Mem m;
@@ -795,6 +809,8 @@ struct Core {
   //   word 13    flags (bits 0-3 and the leader in 8-15, as F_FLAGS) | TC authors << 4 | votes << 16 | timeouts << 20 |
   //              NEXT_CMD << 24
   //   words 14 / 15  highest_certified_block_round of the current timeouts / of the TC, a byte per author
+  // The 16 words are a block of pk_at(): with lane blocks (TileMem LB, the device kernels) a node's 16 rows x 32 lanes hold
+  // each lane's 16 words contiguously, and load_node / store_node move them in 16-byte units.
   // Bounds (single epoch, four authors, rspan = round_cap = 128): update_current_round never sets a round >= rspan (it
   // raises ST_ROUND_OVERFLOW and the loop stops), so every round id, and the hcbr values (<= HQC), is < 128; PMR and LVR
   // (an active round, HQC or HTC + 1) are <= 128; a node proposes at most once per round and commits each round at most
@@ -838,18 +854,54 @@ struct Core {
       default: return {13, 24, 0xffu};  // F_NEXT_CMD
     }
   }
+  // The compact words of the node whose block starts at word b (nbase): word k at [k * PS].
+  LBFT_HD uint32_t* pk_at(uint32_t b) const { return m.block(b, kPackedWords); }
+  // K words of a compact block (pk_at, a slot's pay_at) to or from registers: 128-bit accesses in lane blocks (each block is
+  // 16-byte aligned: the tile and every region of blocks start on a 128-byte boundary), otherwise one word per row.  A
+  // store of 14 words ends in a 64-bit access.
+  template <int K>
+  LBFT_HD static void ld_block(const uint32_t* p, uint32_t (&w)[K]) {
+    static_assert(K % 4 == 0, "whole 16-byte units");
+#if defined(__CUDA_ARCH__)
+    if constexpr (Mem::LB) {
+#pragma unroll
+      for (int i = 0; i < K / 4; i++) {
+        const uint4 v = reinterpret_cast<const uint4*>(p)[i];
+        w[4 * i] = v.x, w[4 * i + 1] = v.y, w[4 * i + 2] = v.z, w[4 * i + 3] = v.w;
+      }
+      return;
+    }
+#endif
+#pragma unroll
+    for (int i = 0; i < K; i++) w[i] = p[i * PS];
+  }
+  template <int K>
+  LBFT_HD static void st_block(uint32_t* p, const uint32_t (&w)[K]) {
+    static_assert(K % 4 == 0 || K % 4 == 2, "whole 8-byte units");
+#if defined(__CUDA_ARCH__)
+    if constexpr (Mem::LB) {
+#pragma unroll
+      for (int i = 0; i < K / 4; i++) reinterpret_cast<uint4*>(p)[i] = make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], w[4 * i + 3]);
+      if constexpr (K % 4 != 0) reinterpret_cast<uint2*>(p)[K / 2 - 1] = make_uint2(w[K - 2], w[K - 1]);
+      return;
+    }
+#endif
+#pragma unroll
+    for (int i = 0; i < K; i++) p[i * PS] = w[i];
+  }
   // Scalar f of the node whose block starts at word b (nbase), outside the event loop (init, finalize).
   LBFT_HD uint32_t node_ld(uint32_t b, uint32_t f) const {
     if constexpr (PACK) {
       const PackedField pf = packed_field(f);
-      return (m.ld(b + pf.word) >> pf.shift) & pf.mask;
+      return (pk_at(b)[pf.word * PS] >> pf.shift) & pf.mask;
     }
     return m.ld(b + f);
   }
   LBFT_HD void node_st(uint32_t b, uint32_t f, uint32_t v) const {
     if constexpr (PACK) {
       const PackedField pf = packed_field(f);
-      m.st(b + pf.word, (m.ld(b + pf.word) & ~(pf.mask << pf.shift)) | ((v & pf.mask) << pf.shift));
+      uint32_t* p = pk_at(b) + pf.word * PS;
+      *p = (*p & ~(pf.mask << pf.shift)) | ((v & pf.mask) << pf.shift);
     } else {
       m.st(b + f, v);
     }
@@ -908,15 +960,16 @@ struct Core {
     uint32_t dirty;                 // bit0 chb, bit1 chq, bit2 cpd modified
     uint32_t gb;                    // epoch_id * rspan: global id of this node's round 0 (0 in single-epoch layouts)
     uint32_t* nb;                   // this node's block in the tile
+    uint32_t* pk;                   // PACK: its compact words (pk_at)
   };
   LBFT_HD static uint32_t epoch_of(const NodeRegs& d) { return (d.f[F_FLAGS] >> FL_EPOCH_SHIFT) & FL_EPOCH_BITS; }
   LBFT_HD void load_node(uint32_t n, NodeRegs& d) {
     uint32_t* nb = m.at(nbase(n));
     d.nb = nb;
     if constexpr (PACK) {
-      uint32_t w[kPackedScalarWords];
-#pragma unroll
-      for (int i = 0; i < (int)kPackedScalarWords; i++) w[i] = nb[i * S];
+      d.pk = pk_at(nbase(n));
+      uint32_t w[kPackedWords];  // (the hcbr words come along in the last 16-byte unit; they are read in place)
+      ld_block(d.pk, w);
       auto get = [&](uint32_t f) { const PackedField pf = packed_field(f); return (w[pf.word] >> pf.shift) & pf.mask; };
 #pragma unroll
       for (int i = 0; i < (int)F_NSCALAR; i++) d.f[i] = get(i);
@@ -955,8 +1008,7 @@ struct Core {
       put(F_NSCALAR, d.vmask);
       put(F_NSCALAR + 1, d.tmask);
       put(F_NSCALAR + 2, d.tcmask);
-#pragma unroll
-      for (int i = 0; i < (int)kPackedScalarWords; i++) nb[i * S] = w[i];  // (the hcbr words are written in place)
+      st_block(d.pk, w);  // (the hcbr words are written in place)
     } else {
 #pragma unroll
       for (int i = 0; i < (int)F_NSCALAR; i++) nb[i * S] = d.f[i];
@@ -987,12 +1039,12 @@ struct Core {
   }
   // highest_certified_block_round of the node's current timeouts (author a) and of its highest TC: in memory, not in NodeRegs
   LBFT_HD void put_timeout_hcbr(const NodeRegs& d, uint32_t a, uint32_t hcbr) const {
-    if constexpr (PACK) reinterpret_cast<uint8_t*>(d.nb + kPackedTimeoutHcbr * S)[a] = (uint8_t)hcbr;  // little-endian bytes
+    if constexpr (PACK) reinterpret_cast<uint8_t*>(d.pk + kPackedTimeoutHcbr * PS)[a] = (uint8_t)hcbr;  // little-endian bytes
     else st_u16(d.nb + L.n_thcbr * S, a, hcbr);
   }
   LBFT_HD void copy_timeout_hcbr_to_tc(const NodeRegs& d) const {
     if constexpr (PACK) {
-      d.nb[kPackedTcHcbr * S] = d.nb[kPackedTimeoutHcbr * S];
+      d.pk[kPackedTcHcbr * PS] = d.pk[kPackedTimeoutHcbr * PS];
     } else {
       group_sync<G>(gm);  // the st_u16 of put_timeout_hcbr is read by another lane below
       for (uint32_t i = wl; i < L.hcbr_words; i += G) d.nb[(L.n_tchcbr + i) * S] = d.nb[(L.n_thcbr + i) * S];
@@ -1037,10 +1089,14 @@ struct Core {
   // hcbr, a byte per author.
   static constexpr uint32_t kPayRef = PACK ? 1 : 2;  // the word with the reference count in its low 16 bits
   LBFT_HD uint32_t pay_word(uint32_t s) const { return L.pay_base + s * (PACK ? 4u : L.pay_words); }
-  LBFT_HD uint32_t* pay_at(uint32_t s) const { return m.at(pay_word(s)); }
-  LBFT_HD uint32_t pay_refs(uint32_t s) const { return m.ld(pay_word(s) + kPayRef); }
+  // slot s: word k at [k * S], or (PACK, a compact block) at [k * PS]
+  LBFT_HD uint32_t* pay_at(uint32_t s) const { return PACK ? m.block(pay_word(s), 4) : m.at(pay_word(s)); }
+  LBFT_HD uint32_t* pay_ref_at(uint32_t s) const { return PACK ? pay_at(s) + kPayRef * PS : m.at(pay_word(s) + kPayRef); }
+  LBFT_HD uint32_t pay_refs(uint32_t s) const { return *pay_ref_at(s); }
   // the hcbr vector of the TC (which = 0) or of the current timeouts (1) in slot pb, and author a's entry in it
-  LBFT_HD const uint32_t* pay_hcbr(const uint32_t* pb, int which) const { return pb + (PACK ? 2u + which : (which ? L.p_curhcbr : L.p_tchcbr)) * S; }
+  LBFT_HD const uint32_t* pay_hcbr(const uint32_t* pb, int which) const {
+    return PACK ? pb + (2u + which) * PS : pb + (which ? L.p_curhcbr : L.p_tchcbr) * S;
+  }
   LBFT_HD static uint32_t hcbr_of(const uint32_t* hp, uint32_t a) {
     if constexpr (PACK) return (hp[0] >> (8 * a)) & 0xffu;
     else return ld_u16(hp, a);
@@ -1067,13 +1123,13 @@ struct Core {
   }
   LBFT_HD void pay_release(uint32_t s) {
     if (L.payload_cap <= 32) { pay_free |= 1u << s; return; }
-    m.st(pay_word(s) + kPayRef, pay_free);  // link into the free list through the reference count
+    *pay_ref_at(s) = pay_free;  // link into the free list through the reference count
     pay_free = s;
   }
   LBFT_HD void pay_unref(uint32_t slot, uint32_t w2) {
     uint32_t refs = (w2 & 0xffffu) - 1;
     if (refs == 0) pay_release(slot);
-    else m.st(pay_word(slot) + kPayRef, (w2 & 0xffff0000u) | refs);
+    else *pay_ref_at(slot) = (w2 & 0xffff0000u) | refs;
   }
 
   // ------------------------------------------------------------------------------------------
@@ -1376,8 +1432,8 @@ struct Core {
   LBFT_HD void prefetch_hcbr(const NodeRegs& d, HcbrRegs& h) const {
     const bool has_tc = d.f[F_FLAGS] & FL_HAS_TC;
     if constexpr (PACK) {
-      h.tc[0] = has_tc ? d.nb[kPackedTcHcbr * S] : 0u;
-      h.cur[0] = d.tmask ? d.nb[kPackedTimeoutHcbr * S] : 0u;
+      h.tc[0] = has_tc ? d.pk[kPackedTcHcbr * PS] : 0u;
+      h.cur[0] = d.tmask ? d.pk[kPackedTimeoutHcbr * PS] : 0u;
       return;
     }
     if (L.hcbr_words > 2) return;
@@ -1399,11 +1455,11 @@ struct Core {
       ep = epoch_of(d);
       if (((d.f[F_FLAGS] >> FL_PM_EPOCH_SHIFT) & FL_EPOCH_BITS) != ep) prop = 0;
     }
-    if constexpr (PACK) {
-      pb[0] = d.f[F_HCC] | (d.f[F_HQC] << 8) | (d.f[F_CUR] << 16) | ((has_tc ? d.f[F_TC_ROUND] : 0u) << 24);
-      pb[kPayRef * S] = refs | ((vote | (prop << 1)) << 16) | ((has_tc ? d.tcmask : 0u) << 24) | (d.tmask << 28);
-      if (has_tc) pb[2 * S] = h.tc[0];
-      if (d.tmask) pb[3 * S] = h.cur[0];
+    if constexpr (PACK) {  // the whole slot in one store (an hcbr word outside its mask is 0, prefetch_hcbr)
+      const uint32_t w[4] = {d.f[F_HCC] | (d.f[F_HQC] << 8) | (d.f[F_CUR] << 16) | ((has_tc ? d.f[F_TC_ROUND] : 0u) << 24),
+                             refs | ((vote | (prop << 1)) << 16) | ((has_tc ? d.tcmask : 0u) << 24) | (d.tmask << 28), h.tc[0],
+                             h.cur[0]};
+      st_block(pb, w);
       return;
     }
     pb[0] = d.f[F_HCC] | (d.f[F_HQC] << 16);
@@ -1432,8 +1488,10 @@ struct Core {
     uint32_t hcc, hqc, cur_s, tc_round, w2;
     mask_t tcm, curm;
     if constexpr (PACK) {
-      const uint32_t w0 = pb[0];
-      w2 = pb[kPayRef * S];
+      uint32_t w[4];  // (the hcbr words are read in place by insert_timeout_groups)
+      ld_block(pb, w);
+      const uint32_t w0 = w[0];
+      w2 = w[kPayRef];
       hcc = w0 & 0xffu, hqc = (w0 >> 8) & 0xffu, cur_s = (w0 >> 16) & 0xffu, tc_round = w0 >> 24;
       tcm = (w2 >> 24) & 0xfu, curm = w2 >> 28;
     } else {
@@ -1637,7 +1695,8 @@ struct Core {
     q.clear(m, L, wl, km);
     if constexpr (PACK) {  // the compact words and the bitsets: the other words of the generic block are never touched
       for (uint32_t n = 0; n < N; n++) {
-        for (uint32_t w = 0; w < kPackedWords; w++) m.st(nbase(n) + w, 0);
+        const uint32_t zero[kPackedWords] = {};
+        st_block(pk_at(nbase(n)), zero);
         for (uint32_t w = L.n_hasblk; w < L.node_words; w++) m.st(nbase(n) + w, 0);
       }
     } else {
@@ -1743,8 +1802,8 @@ struct Core {
       const bool is_request = kind == EV_REQUEST;  // answered by `receiver` itself (simulator.rs:446): no state change
       if (TDS && is_request) load_node(sender, d);  // ... unless the node it was sent to answers (read only, never stored)
       if (!is_request) {
-        // A timer pop cancelled by ignore_scheduled_updates_until (simulator.rs:403-410), ~40 % of the events of the bench
-        // workload, changes nothing: with the compact encoding it reads the one word it tests before the node block is loaded
+        // A timer pop cancelled by ignore_scheduled_updates_until (simulator.rs:403-410), ~9 % of the pops of the bench
+        // workload (the duplicates push_timer elides never reach the queue), changes nothing: with the compact encoding it reads the one word it tests before the node block is loaded
         // (measured ~1 % faster there).  The test on the loaded block below then never fires in that kernel; compiling it out
         // measured as slow as having no early test, so it stays for every kernel.
         if (PACK && kind == EV_TIMER && clock <= (int32_t)node_ld(nbase(receiver), F_IGNORE)) {
