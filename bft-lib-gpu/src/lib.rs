@@ -160,6 +160,9 @@ pub mod ffi {
                                  out_sim: *mut *mut LbftSim) -> c_int;
         pub fn lbft_create_sweep_faults(config: *const LbftConfig, sets: *const lbft_param_set, faults: *const lbft_fault_set, num_sets: u32,
                                         set_of_instance: *const u32, out_sim: *mut *mut LbftSim) -> c_int;
+        pub fn lbft_create_sweep_rights(config: *const LbftConfig, sets: *const lbft_param_set, faults: *const lbft_fault_set,
+                                        voting_rights: *const u64, num_sets: u32, set_of_instance: *const u32,
+                                        out_sim: *mut *mut LbftSim) -> c_int;
         pub fn lbft_destroy(sim: *mut LbftSim);
         pub fn lbft_set_seeds(sim: *mut LbftSim, seeds: *const u64) -> c_int;
         pub fn lbft_run(sim: *mut LbftSim) -> c_int;
@@ -177,6 +180,8 @@ pub mod ffi {
         pub fn lbft_latency_stats(sim: *mut LbftSim, spec: *const lbft_latency_spec, out: *mut lbft_latency_summary, hist: *mut u64) -> c_int;
         pub fn lbft_block_latency_stats(sim: *mut LbftSim, spec: *const lbft_latency_spec, threshold: u64,
                                         out: *mut lbft_latency_summary, unreached: *mut u64, hist: *mut u64) -> c_int;
+        pub fn lbft_block_latency_stats_groups(sim: *mut LbftSim, spec: *const lbft_latency_spec, thresholds: *const u64,
+                                               out: *mut lbft_latency_summary, unreached: *mut u64, hist: *mut u64) -> c_int;
         pub fn lbft_round_switches(sim: *mut LbftSim, instance: u32, out: *mut LbftRoundSwitch, cap: usize, n: *mut usize) -> c_int;
         pub fn lbft_snapshot_size(sim: *mut LbftSim, bytes: *mut usize) -> c_int;
         pub fn lbft_snapshot_save(sim: *mut LbftSim, buf: *mut u8, cap: usize) -> c_int;

@@ -191,6 +191,21 @@ typedef struct lbft_fault_set {
 int lbft_create_sweep_faults(const lbft_config* config, const lbft_param_set* sets, const lbft_fault_set* faults,
                              uint32_t num_sets, const uint32_t* set_of_instance, lbft_sim** out_sim);
 
+/* A rights sweep: lbft_create_sweep / lbft_create_sweep_faults with the voting rights per parameter set as well.
+ * voting_rights[s * num_nodes + n] is node n's voting right in set s.  faults may be NULL: then the configuration's shared
+ * silent nodes / partition plan apply to every set, as in lbft_create_sweep; otherwise the rules of lbft_create_sweep_faults.
+ * Every output of instance i (with the exceptions of lbft_create_sweep_faults) is what lbft_create + lbft_run give it with
+ * sets[s], faults[s] (or the shared faults) and row s of voting_rights substituted into `config`, s = set_of_instance[i]; the
+ * proposers of lbft_commit_log(s) and the state keys come from the set's own leaders.  The layout and kernel are what
+ * lbft_create_sweep / lbft_create_sweep_faults pick for the same call: voting rights enter no kernel choice.  One leader table
+ * of round_cap + 1 bytes is kept per distinct row (lbft_memory_info counts them).  Refused (LBFT_ERR_INVALID, before any device
+ * work): whatever the corresponding sweep entry point refuses, NULL voting_rights, config->voting_rights != NULL (a rights sweep
+ * takes its rights per set only), and a row with an entry above 2^24 or a total of 0 (the error names the set).  Every other
+ * entry point as for a sweep; lbft_block_latency_stats / lbft_block_latency_stats_groups weigh each group with its set's rights. */
+int lbft_create_sweep_rights(const lbft_config* config, const lbft_param_set* sets, const lbft_fault_set* faults,
+                             const uint64_t* voting_rights, uint32_t num_sets, const uint32_t* set_of_instance,
+                             lbft_sim** out_sim);
+
 /* Simulator::new for every instance followed by loop_until(max_clock) (simulator.rs:200-250,
  * 380-475): copies the seeds host->device, runs the event-loop kernel to completion, copies the
  * per-node summaries (commit counts, last-committed-state keys, counters, status) device->host.
@@ -324,9 +339,17 @@ int lbft_latency_stats(lbft_sim* sim, const lbft_latency_spec* spec, lbft_latenc
  * lbft_latency_stats: out[num_groups] (samples counts the reached blocks; sum / min / max / hist cover their latencies),
  * unreached[num_groups] the blocks that never reached the threshold, or NULL (then not copied), hist[group * num_bins + b] or
  * NULL.  Refusals: those of lbft_latency_stats, with its messages, and LBFT_ERR_INVALID for a threshold of 0 or above the
- * handle's total voting rights. */
+ * handle's total voting rights.  On a rights sweep (lbft_create_sweep_rights) each group is weighed with its set's voting
+ * rights, and a threshold above any group's total is refused (the error names the group). */
 int lbft_block_latency_stats(lbft_sim* sim, const lbft_latency_spec* spec, uint64_t threshold, lbft_latency_summary* out,
                              uint64_t* unreached, uint64_t* hist);
+
+/* lbft_block_latency_stats with one threshold per group: thresholds[num_groups], each in 1..that group's total voting rights.
+ * Works on every handle with LBFT_FLAG_COMMIT_TIMES (a plain handle has one group).  Everything else, refusals and their
+ * messages included, is that of lbft_block_latency_stats; with the same threshold W for every group it returns what
+ * lbft_block_latency_stats(W) returns. */
+int lbft_block_latency_stats_groups(lbft_sim* sim, const lbft_latency_spec* spec, const uint64_t* thresholds,
+                                    lbft_latency_summary* out, uint64_t* unreached, uint64_t* hist);
 
 #ifdef __cplusplus
 }

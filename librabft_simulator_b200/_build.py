@@ -2,7 +2,7 @@
 
 * ``csrc/liblbft_b200.so`` — the product: sm_90a (H100) CUDA kernels + the C ABI of ``include/lbft.h``.
 * ``oracle/liblbft_oracle.so``, ``tests/hostcore/libhostcore.so``, ``tests/hostcore/libhostcore_sweep.so``,
-  ``tests/hostcore/libhostcore_ct.so``, ``tests/hostcore/libhostcore_latency.so``, ``tests/hostcore/libhostcore_fault.so``,
+  ``tests/hostcore/libhostcore_ct.so``, ``tests/hostcore/libhostcore_latency.so``, ``tests/hostcore/libhostcore_fault.so``, ``tests/hostcore/libhostcore_rights.so``,
   ``tests/hostcore/libhostcore_block_latency.so`` and ``tests/hostcore/libhostcore_lane_block.so`` — test infrastructure only; so is ``tests/gpuprobe/libblock_threshold_probe.so``,
   a CUDA probe of one device function.
 All artefacts are built in-tree and git-ignored.
@@ -22,6 +22,7 @@ SWEEP_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_sweep.so")
 CT_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_ct.so")
 LATENCY_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_latency.so")
 FAULT_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_fault.so")
+RIGHTS_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_rights.so")
 BLOCK_LATENCY_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_block_latency.so")
 LANE_BLOCK_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_lane_block.so")
 GPUPROBE_DIR = os.path.join(ROOT, "tests", "gpuprobe")
@@ -219,7 +220,20 @@ def build_block_threshold_probe(force=False):
     return BLOCK_THRESHOLD_PROBE_PATH
 
 
+def build_rights_hostcore(force=False):
+    """The SW and SW + CT cores of rights sweeps over the product's host setup and set table (tests/hostcore/rights_hostcore.cpp,
+    which compiles fault_hostcore.cpp and ct_hostcore.cpp into itself): test infrastructure."""
+    srcs = [os.path.join(HOSTCORE_DIR, f) for f in ("rights_hostcore.cpp", "fault_hostcore.cpp", "ct_hostcore.cpp")] + [
+        os.path.join(ROOT, "include", "lbft.h")] + [os.path.join(CSRC, f) for f in ("sim_core.cuh", "sim_params.h", "host_setup.hpp")] + [
+        os.path.join(ORACLE_DIR, f) for f in ("oracle_capi.cpp", "lbft_oracle.hpp")]
+    if not force and _newer(RIGHTS_HOSTCORE_PATH, srcs):
+        return RIGHTS_HOSTCORE_PATH
+    _run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-DLBFT_CHECK_C1",
+          "-o", RIGHTS_HOSTCORE_PATH, "rights_hostcore.cpp"], HOSTCORE_DIR)
+    return RIGHTS_HOSTCORE_PATH
+
+
 def build_all(force=False):
     return (build_product(force), build_oracle(force), build_hostcore(force), build_sweep_hostcore(force), build_ct_hostcore(force),
             build_latency_hostcore(force), build_fault_hostcore(force), build_block_latency_hostcore(force),
-            build_lane_block_hostcore(force), build_block_threshold_probe(force))
+            build_lane_block_hostcore(force), build_block_threshold_probe(force), build_rights_hostcore(force))

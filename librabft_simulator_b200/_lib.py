@@ -76,7 +76,7 @@ ST_INVARIANT, ST_EPOCH_CHANGE, ST_DELAY_NEAR_INT, ST_TIME_OVERFLOW = 16, 32, 64,
 ST_ERROR_MASK = ST_ROUND_OVERFLOW | ST_QUEUE_OVERFLOW | ST_PAYLOAD_OVERFLOW | ST_INVARIANT | ST_TIME_OVERFLOW
 
 EXPORTS = [
-    "lbft_create", "lbft_create_sweep", "lbft_create_sweep_faults", "lbft_run", "lbft_run_async", "lbft_wait", "lbft_commit_logs", "lbft_commit_times", "lbft_latency_stats", "lbft_block_latency_stats", "lbft_upload", "lbft_run_device", "lbft_download", "lbft_commit_counts",
+    "lbft_create", "lbft_create_sweep", "lbft_create_sweep_faults", "lbft_create_sweep_rights", "lbft_run", "lbft_run_async", "lbft_wait", "lbft_commit_logs", "lbft_commit_times", "lbft_latency_stats", "lbft_block_latency_stats_groups", "lbft_block_latency_stats", "lbft_upload", "lbft_run_device", "lbft_download", "lbft_commit_counts",
     "lbft_last_states", "lbft_commit_log", "lbft_round_switches", "lbft_active_rounds", "lbft_counters", "lbft_status", "lbft_timing_info",
     "lbft_memory_info", "lbft_kernel_info", "lbft_run_until", "lbft_snapshot_size", "lbft_snapshot_save", "lbft_snapshot_load", "lbft_set_seeds", "lbft_device_buffer", "lbft_destroy", "lbft_last_error", "lbft_abi_version",
 ]
@@ -105,6 +105,8 @@ def load():
     lib.lbft_create_sweep.argtypes = [ctypes.POINTER(LbftConfig), ctypes.POINTER(LbftParamSet), c_u32, P, ctypes.POINTER(P)]
     lib.lbft_create_sweep_faults.argtypes = [ctypes.POINTER(LbftConfig), ctypes.POINTER(LbftParamSet), ctypes.POINTER(LbftFaultSet), c_u32, P,
                                              ctypes.POINTER(P)]
+    lib.lbft_create_sweep_rights.argtypes = [ctypes.POINTER(LbftConfig), ctypes.POINTER(LbftParamSet), ctypes.POINTER(LbftFaultSet), P, c_u32,
+                                             P, ctypes.POINTER(P)]
     for name in ("lbft_run", "lbft_run_async", "lbft_wait", "lbft_upload", "lbft_run_device", "lbft_download"):
         getattr(lib, name).argtypes = [P]
     for name in ("lbft_commit_counts", "lbft_last_states", "lbft_active_rounds", "lbft_counters", "lbft_status"):
@@ -114,6 +116,7 @@ def load():
     lib.lbft_commit_times.argtypes = [P, P, P, ctypes.c_size_t]
     lib.lbft_latency_stats.argtypes = [P, ctypes.POINTER(LbftLatencySpec), P, P]
     lib.lbft_block_latency_stats.argtypes = [P, ctypes.POINTER(LbftLatencySpec), c_u64, P, P, P]
+    lib.lbft_block_latency_stats_groups.argtypes = [P, ctypes.POINTER(LbftLatencySpec), P, P, P, P]
     lib.lbft_round_switches.argtypes = [P, c_u32, ctypes.POINTER(LbftRoundSwitch), ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)]
     lib.lbft_timing_info.argtypes = [P, ctypes.POINTER(LbftTiming)]
     lib.lbft_run_until.argtypes = [P, c_i64]

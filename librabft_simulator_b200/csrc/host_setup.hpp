@@ -10,10 +10,12 @@
 // independently of oracle/ (the oracle is the checker, not a dependency).
 #pragma once
 #include <cmath>
+#include <cstddef>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <string>
 #include <vector>
 
@@ -365,7 +367,8 @@ struct HostSetup {
   std::vector<double> delay_thr;  // see build_delay_table()
   std::vector<SweepSet> sets;     // sweep handles: one record per parameter set (build_sweep); empty otherwise
   std::vector<uint32_t> set_of;   // sweep handles: [num_instances] the set of each instance
-  std::vector<SweepFaults> faults;  // fault sweeps: one record per parameter set (build_sweep_faults); empty otherwise
+  std::vector<SweepFaults> faults;  // fault and rights sweeps: one record per parameter set (build_sweep_faults / _rights); empty otherwise
+  std::vector<SweepRights> rights;  // rights sweeps: one record per parameter set (build_sweep_rights); empty otherwise
   std::string error;
   KernelSel sel{};
 
@@ -390,8 +393,14 @@ struct HostSetup {
   // configuration carries none, and the layout and kernel are what a sweep picks with the largest window count of any set in
   // the configuration; `faults` gets each set's record, and Params::silent_mask the union of the sets' silent nodes (the
   // kernels' launch-uniform test for whether any node can be silent: sim_core.cuh Core::any_silent).
+  //
+  // A rights sweep (lbft_create_sweep_rights, `vr` not null: [num_sets][num_nodes]): each set's voting rights are substituted
+  // as well and the configuration carries none.  Layout and kernel do not depend on the rights.  `rights` gets each set's
+  // record, with one leader table per distinct row of `vr` appended to `leader` (set 0's first, where a plain handle has its
+  // own); `faults` gets each set's fault record, the configuration's shared faults when `fs` is null; and weights, Params'
+  // quorum and c_weights are set 0's.
   bool build_sweep(const lbft_config& c, const lbft_param_set* ps, uint32_t num_sets, const uint32_t* set_of_instance,
-                   const lbft_fault_set* fs = nullptr) {
+                   const lbft_fault_set* fs = nullptr, const uint64_t* vr = nullptr) {
     if (c.struct_size != sizeof(lbft_config)) return fail("lbft_config.struct_size does not match this library (ABI mismatch)");
     if (!ps || !set_of_instance) return fail("sets and set_of_instance must not be NULL");
     if (num_sets == 0 || num_sets > c.num_instances || num_sets > 65536u) return fail("num_sets must be in 1..min(num_instances, 65536)");
@@ -401,10 +410,13 @@ struct HostSetup {
     if (fs && (c.silent || c.partition_windows || c.partition_max_len))
       return fail("a fault sweep takes its silent nodes and partitions per set only: lbft_config.silent must be NULL and "
                   "partition_windows / partition_max_len 0");
+    if (vr && c.voting_rights)
+      return fail("a rights sweep takes its voting rights per set only: lbft_config.voting_rights must be NULL");
     uint32_t fastest = 0, windows = 0;
     for (uint32_t s = 0; s < num_sets; s++) {
       uint8_t silent[64];
-      const lbft_config cs = fs ? with_faults(with_set(c, ps[s]), fs[s], silent) : with_set(c, ps[s]);
+      lbft_config cs = fs ? with_faults(with_set(c, ps[s]), fs[s], silent) : with_set(c, ps[s]);
+      if (vr) cs.voting_rights = vr + (size_t)s * c.num_nodes;
       const char* e = config_error(cs);
       if (!e && fs && c.num_nodes < 64 && (fs[s].silent_mask >> c.num_nodes)) e = "silent_mask has a bit at or above num_nodes";
       if (e || ps[s].reserved)
@@ -414,6 +426,7 @@ struct HostSetup {
     }
     lbft_config cf = with_set(c, ps[fastest]);
     if (fs) cf.partition_windows = windows;
+    if (vr) cf.voting_rights = vr;  // (set 0's: build_shared's weights, quorum and first leader table; no decision reads them)
     const uint32_t rcap = round_cap_of(cf);
     if (c.commands_per_epoch < rcap)
       return fail("sweep handles need commands_per_epoch >= round_cap (single-epoch runs: epochs are plain handles only)");
@@ -429,7 +442,10 @@ struct HostSetup {
         faults[s] = SweepFaults{fs[s].silent_mask, fs[s].partition_windows, fs[s].partition_max_len};
         params.silent_mask |= fs[s].silent_mask;  // the union: the kernels' launch-uniform "any silent node" test
       }
+    } else if (vr) {
+      faults.assign(num_sets, SweepFaults{params.silent_mask, params.L.part_windows, params.part_max_len});
     }
+    if (vr) add_rights(vr, num_sets);
     sel = select_kernel(cf, tile, params, true);
     return true;
   }
@@ -439,6 +455,32 @@ struct HostSetup {
                           const uint32_t* set_of_instance) {
     if (!fs) return fail("faults must not be NULL");
     return build_sweep(c, ps, num_sets, set_of_instance, fs);
+  }
+
+  // A rights sweep (lbft_create_sweep_rights): build_sweep with each set's voting rights, and its faults when `fs` is not null.
+  bool build_sweep_rights(const lbft_config& c, const lbft_param_set* ps, const lbft_fault_set* fs, const uint64_t* vr,
+                          uint32_t num_sets, const uint32_t* set_of_instance) {
+    if (!vr) return fail("voting_rights must not be NULL");
+    return build_sweep(c, ps, num_sets, set_of_instance, fs, vr);
+  }
+
+  // Which records follow each set in the sweep's device table (sim_core.cuh sweep_set_at): bit 0 faults, bit 1 rights.
+  uint32_t records() const { return (faults.empty() ? 0u : 1u) | (rights.empty() ? 0u : 2u); }
+
+  // A sweep's device table of parameter sets, the bytes the runtime uploads: `sets`, each followed by its fault record and then
+  // its rights record where records() has them (SweepSet, SweepSetFaults or SweepSetRights entries).
+  std::vector<uint64_t> set_table() const {
+    const uint32_t rec = records();
+    const size_t pitch = (rec & 2) ? sizeof(SweepSetRights) : ((rec & 1) ? sizeof(SweepSetFaults) : sizeof(SweepSet));
+    static_assert(sizeof(SweepSet) % 8 == 0 && sizeof(SweepSetFaults) % 8 == 0 && sizeof(SweepSetRights) % 8 == 0, "whole words");
+    std::vector<uint64_t> t(sets.size() * pitch / 8);
+    for (size_t k = 0; k < sets.size(); k++) {
+      char* e = reinterpret_cast<char*>(t.data()) + k * pitch;
+      memcpy(e, &sets[k], sizeof(SweepSet));
+      if (rec & 1) memcpy(e + offsetof(SweepSetFaults, faults), &faults[k], sizeof(SweepFaults));
+      if (rec & 2) memcpy(e + offsetof(SweepSetRights, rights), &rights[k], sizeof(SweepRights));
+    }
+    return t;
   }
 
  private:
@@ -456,7 +498,7 @@ struct HostSetup {
       if (c.voting_rights) weights[i] = (uint32_t)c.voting_rights[i];
       total += weights[i];
     }
-    p.quorum = (uint32_t)(2 * total / 3 + 1);
+    p.quorum = quorum_of(total);
     for (uint32_t i = 0; i < 64; i++) p.c_weights[i] = i < N ? weights[i] : 0;
     if (c.silent)
       for (uint32_t i = 0; i < N; i++)
@@ -468,10 +510,40 @@ struct HostSetup {
     p.resumable = (c.flags & LBFT_FLAG_RESUMABLE) ? 1u : 0u;
     p.stop_clock = p.max_clock;
     p.L = L;
-    // leader(round) for every representable round (+1: the pacemaker looks at active_round <= round_cap)
-    leader.resize(L.rspan + 1);
-    for (uint32_t r = 0; r <= L.rspan; r++) leader[r] = (uint8_t)pick_author(weights, total, siphash13_u64(r));
+    leader.clear();
+    add_leader_table(weights, total);
     build_ziggurat();
+  }
+
+  static uint32_t quorum_of(uint64_t total) { return (uint32_t)(2 * total / 3 + 1); }
+
+  // leader(round) under voting rights `w` for every representable round (+1: the pacemaker looks at active_round <= round_cap),
+  // appended to `leader`; returns where it starts.
+  uint32_t add_leader_table(const std::vector<uint32_t>& w, uint64_t total) {
+    const uint32_t off = (uint32_t)leader.size(), rspan = params.L.rspan;
+    leader.resize((size_t)off + rspan + 1);
+    for (uint32_t r = 0; r <= rspan; r++) leader[(size_t)off + r] = (uint8_t)pick_author(w, total, siphash13_u64(r));
+    return off;
+  }
+
+  // A rights sweep's records (`vr`: [num_sets][num_nodes], checked by config_error): per set its weights and quorum, and one
+  // leader table per distinct row.  Set 0's table is the one build_shared made.
+  void add_rights(const uint64_t* vr, uint32_t num_sets) {
+    const uint32_t N = params.L.num_nodes;
+    std::map<std::vector<uint32_t>, uint32_t> table_of;
+    table_of.emplace(weights, 0u);
+    rights.assign(num_sets, SweepRights{});
+    std::vector<uint32_t> row(N);
+    for (uint32_t s = 0; s < num_sets; s++) {
+      uint64_t total = 0;
+      for (uint32_t n = 0; n < N; n++) total += row[n] = (uint32_t)vr[(size_t)s * N + n];
+      auto it = table_of.find(row);
+      if (it == table_of.end()) it = table_of.emplace(row, add_leader_table(row, total)).first;
+      SweepRights& r = rights[s];
+      r.quorum = quorum_of(total);
+      r.leader_off = it->second;
+      for (uint32_t n = 0; n < N; n++) r.weights[n] = row[n];
+    }
   }
 
   // The part of a configuration a sweep varies per parameter set (lbft_param_set): its delay model and tci into `s`, its delay
@@ -592,14 +664,37 @@ inline const char* latency_spec_error(const HostSetup& hs, const lbft_latency_sp
   return nullptr;
 }
 
-// lbft_block_latency_stats: the total voting rights of a handle, and the check on a threshold (null when it is valid).
-inline uint64_t total_voting_rights(const HostSetup& hs) {
+// lbft_block_latency_stats: the total voting rights of group g of a handle (on a rights sweep its parameter set's, on every
+// other handle the one committee's), and the checks on one threshold for every group (lbft_block_latency_stats) and on a
+// threshold per group (lbft_block_latency_stats_groups, thresholds[latency_groups(hs)]): null when valid.  A message that
+// names a group lives until the next check on this thread.
+inline uint64_t total_voting_rights(const HostSetup& hs, uint32_t g = 0) {
   uint64_t total = 0;
+  if (!hs.rights.empty()) {
+    for (uint32_t w : hs.rights[g].weights) total += w;  // (0 past num_nodes)
+    return total;
+  }
   for (uint32_t w : hs.weights) total += w;
   return total;
 }
+inline const char* group_threshold_message(const char* what, uint32_t g, uint64_t total) {
+  static thread_local std::string msg;
+  msg = std::string(what) + " must be in 1..total voting rights of group " + std::to_string(g) + " (" + std::to_string(total) + ")";
+  return msg.c_str();
+}
 inline const char* block_latency_threshold_error(const HostSetup& hs, uint64_t threshold) {
-  if (threshold < 1 || threshold > total_voting_rights(hs)) return "threshold must be in 1..total voting rights of the handle";
+  if (hs.rights.empty()) {
+    if (threshold < 1 || threshold > total_voting_rights(hs)) return "threshold must be in 1..total voting rights of the handle";
+    return nullptr;
+  }
+  for (uint32_t g = 0; g < latency_groups(hs); g++)
+    if (threshold < 1 || threshold > total_voting_rights(hs, g)) return group_threshold_message("threshold", g, total_voting_rights(hs, g));
+  return nullptr;
+}
+inline const char* block_latency_thresholds_error(const HostSetup& hs, const uint64_t* thresholds) {
+  for (uint32_t g = 0; g < latency_groups(hs); g++)
+    if (thresholds[g] < 1 || thresholds[g] > total_voting_rights(hs, g))
+      return group_threshold_message(("thresholds[" + std::to_string(g) + "]").c_str(), g, total_voting_rights(hs, g));
   return nullptr;
 }
 

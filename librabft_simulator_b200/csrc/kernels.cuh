@@ -3,7 +3,8 @@
 //   lbft_event_loop_kernel<NMAX, QMODE, FIXED, REC, RES>   one THREAD per instance, 32 instances per warp tile (large batches)
 //   lbft_wide_kernel<NMAX, QMODE>                          one WARP per instance (small batches, large committees)
 //   lbft_sweep_event_loop_kernel / lbft_sweep_wide_kernel  the same bodies for sweep handles (lbft_create_sweep: per-instance
-//                                                          delay model and NodeConfig; lbft_create_sweep_faults: and faults)
+//                                                          delay model and NodeConfig; lbft_create_sweep_faults: and faults;
+//                                                          lbft_create_sweep_rights: and voting rights)
 //   lbft_ct_*_kernel                                       the same bodies with the commit-time stores (LBFT_FLAG_COMMIT_TIMES),
 //                                                          a twin of every one-shot single-epoch plain and sweep kernel
 //
@@ -38,15 +39,18 @@ struct LaunchShape {
 // each other's code paths, so a warp of 8 instances finishes far sooner than a warp of 32, and four times as many warps hide
 // each other's latency.  Plain kernels over the calendar queue and the shared-memory queue (whose columns keep their
 // 32-entry pitch); the state layout interleaves TILE instances.
+// The records behind each set of a sweep's table (sim_core.cuh sweep_set_at): bit 0 faults, bit 1 rights.
+__host__ __device__ __forceinline__ uint32_t sweep_records(const SweepParams& S) { return (S.faults ? 1u : 0u) | (S.rights ? 2u : 0u); }
 // The body of both thread kernels (lbft_event_loop_kernel, lbft_sweep_event_loop_kernel), given the kernel's shared memory.
-// SW (sweep handles): the instance's parameter set supplies the delay model and NodeConfig, and on a fault sweep (`faults`:
-// `sets` heads a SweepSetFaults table) the silent nodes and partition plan; its thresholds are read through L1 from the
-// concatenated table, as the instances of one warp may belong to different sets.
+// SW (sweep handles): the instance's parameter set supplies the delay model and NodeConfig, on a fault sweep (`records` bit 0:
+// `sets` heads a SweepSetFaults table) the silent nodes and partition plan, and on a rights sweep (bit 1: a SweepSetRights table)
+// the voting rights, quorum and leaders; its thresholds are read through L1 from the concatenated table, as the instances of one
+// warp may belong to different sets.
 // CT: the commit-time stores (sim_core.cuh Core CT) into `times`, [num_instances][N + 1][round_cap].
 template <int NMAX, int QMODE, int FX, bool REC, bool RES, bool EP, bool TDS, int TILE, bool SW, bool CT = false>
 __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, double* s_zf, double* s_thr, uint32_t* s_queue,
                                                 const uint32_t* set_of, const SweepSet* sets, int32_t* times = nullptr,
-                                                bool faults = false) {
+                                                uint32_t records = 0) {
   static_assert(TILE == 32 || ((QMODE == 3 || QMODE == 2) && !REC && !RES && !EP && !TDS), "sparse tiles: plain kernels over the calendar / shared-memory queue");
   for (int i = threadIdx.x; i < 257; i += blockDim.x) {
     s_zx[i] = P.zig_x[i];
@@ -79,8 +83,9 @@ __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, d
   if (KS) core.km = s_queue + (size_t)(threadIdx.x >> 5) * calendar_kmask_words(FX ? fixed_layout(FX) : P.L) * TILE + lane;
   if constexpr (CT) core.ct = times + (size_t)inst * (core.L.num_nodes + 1) * core.L.round_cap;
   if constexpr (SW) {
-    core.bind_set(faults ? &reinterpret_cast<const SweepSetFaults*>(sets)[set_of[inst]].set : sets + set_of[inst]);
-    core.bind_faults(faults);
+    core.bind_set(sweep_set_at(sets, set_of[inst], records));
+    core.bind_faults(records & 1);
+    core.bind_rights(records & 2);
   }
   if (RES && (P.run_flags & 1u)) core.restore_regs();  // a later lbft_run_until: continue where the last launch stopped
   else core.init(P.seeds[inst]);
@@ -109,7 +114,7 @@ __global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMOD
   __shared__ double s_zf[257];
   extern __shared__ uint32_t s_queue[];
   event_loop_body<NMAX, QMODE, FX_NONE, false, false, false, false, TILE, true>(S.P, s_zx, s_zf, nullptr, s_queue, S.set_of, S.sets, nullptr,
-                                                                               S.faults != 0);
+                                                                               sweep_records(S));
 }
 
 // ---- a group of G lanes per instance ("wide") ---------------------------------------------------------------------
@@ -138,7 +143,7 @@ LBFT_LAYOUT_FN uint32_t wide_smem_words_per_group(const Layout& L, int qmode, bo
 // The body of both wide kernels (lbft_wide_kernel, lbft_sweep_wide_kernel).  SW: as event_loop_body.
 template <int NMAX, int QMODE, bool SMEM, int G, bool EP, int FX, bool SW, bool CT = false>
 __device__ __forceinline__ void wide_body(const Params& P, uint32_t* s_wide, const uint32_t* set_of, const SweepSet* sets,
-                                          int32_t* times = nullptr, bool faults = false) {
+                                          int32_t* times = nullptr, uint32_t records = 0) {
   constexpr uint32_t kPerBlock = wide_warps(G) * 32 / G;
   const uint32_t grp = threadIdx.x / G, wl = threadIdx.x % G;
   const uint32_t inst = blockIdx.x * kPerBlock + grp;
@@ -157,8 +162,9 @@ __device__ __forceinline__ void wide_body(const Params& P, uint32_t* s_wide, con
   core.gm = G == 32 ? 0xffffffffu : (((1u << (G & 31)) - 1u) << ((threadIdx.x & 31u) & ~(uint32_t)(G - 1)));
   core.ws = ws;
   if constexpr (SW) {
-    core.bind_set(faults ? &reinterpret_cast<const SweepSetFaults*>(sets)[set_of[inst]].set : sets + set_of[inst]);
-    core.bind_faults(faults);
+    core.bind_set(sweep_set_at(sets, set_of[inst], records));
+    core.bind_faults(records & 1);
+    core.bind_rights(records & 2);
   }
   core.init(P.seeds[inst]);
   core.run();
@@ -181,7 +187,7 @@ __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbf
 template <int NMAX, int QMODE, bool SMEM, int G>
 __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbft_sweep_wide_kernel(const __grid_constant__ SweepParams S) {
   extern __shared__ __align__(8) uint32_t s_wide[];
-  wide_body<NMAX, QMODE, SMEM, G, false, FX_NONE, true>(S.P, s_wide, S.set_of, S.sets, nullptr, S.faults != 0);
+  wide_body<NMAX, QMODE, SMEM, G, false, FX_NONE, true>(S.P, s_wide, S.set_of, S.sets, nullptr, sweep_records(S));
 }
 
 // The parameter block of a commit-times kernel (LBFT_FLAG_COMMIT_TIMES): the plain (Params) or sweep (SweepParams) block and
@@ -208,7 +214,7 @@ __global__ void __launch_bounds__(LaunchShape<QMODE>::kThreads, LaunchShape<QMOD
   __shared__ double s_zf[257];
   extern __shared__ uint32_t s_queue[];
   event_loop_body<NMAX, QMODE, FX_NONE, false, false, false, false, TILE, true, true>(C.base.P, s_zx, s_zf, nullptr, s_queue, C.base.set_of,
-                                                                                     C.base.sets, C.times, C.base.faults != 0);
+                                                                                     C.base.sets, C.times, sweep_records(C.base));
 }
 template <int NMAX, int QMODE, bool SMEM, int G, int FX>
 __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbft_ct_wide_kernel(const __grid_constant__ CtParams<Params> C) {
@@ -218,7 +224,7 @@ __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbf
 template <int NMAX, int QMODE, bool SMEM, int G>
 __global__ void __launch_bounds__(wide_warps(G) * 32, wide_blocks_per_sm(G)) lbft_ct_sweep_wide_kernel(const __grid_constant__ CtParams<SweepParams> C) {
   extern __shared__ __align__(8) uint32_t s_wide[];
-  wide_body<NMAX, QMODE, SMEM, G, false, FX_NONE, true, true>(C.base.P, s_wide, C.base.set_of, C.base.sets, C.times, C.base.faults != 0);
+  wide_body<NMAX, QMODE, SMEM, G, false, FX_NONE, true, true>(C.base.P, s_wide, C.base.set_of, C.base.sets, C.times, sweep_records(C.base));
 }
 
 // One per translation unit: launches the instantiation the selection names, or returns cudaErrorInvalidValue if the unit

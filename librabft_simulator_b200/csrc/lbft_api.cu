@@ -75,9 +75,8 @@ struct lbft_sim {
   int32_t* d_period = nullptr;
   uint32_t* d_weights = nullptr;
   double* d_delay_thr = nullptr;
-  SweepSet* d_sets = nullptr;    // sweep handles only
+  uint64_t* d_sets = nullptr;    // sweep handles only: HostSetup::set_table (each set with the records HostSetup::records names)
   uint32_t* d_set_of = nullptr;  // sweep handles only
-  SweepSetFaults* d_set_faults = nullptr;  // fault sweeps only: each set with its fault record (instead of d_sets)
   uint32_t* d_state = nullptr;
   uint32_t* d_commit_counts = nullptr;
   uint32_t* d_lc_round = nullptr;
@@ -129,7 +128,7 @@ static void free_all(lbft_sim* s) {
   cudaFree(s->d_seeds); cudaFree(s->d_zx); cudaFree(s->d_zf); cudaFree(s->d_leader); cudaFree(s->d_duration);
   cudaFree(s->d_period); cudaFree(s->d_weights); cudaFree(s->d_delay_thr); cudaFree(s->d_state); cudaFree(s->d_summary);
   cudaFree(s->d_lc_round); cudaFree(s->d_counters); cudaFree(s->d_status);
-  cudaFree(s->d_error); cudaFree(s->d_logs); cudaFree(s->d_sets); cudaFree(s->d_set_of); cudaFree(s->d_set_faults);
+  cudaFree(s->d_error); cudaFree(s->d_logs); cudaFree(s->d_sets); cudaFree(s->d_set_of);
   cudaFree(s->d_times); cudaFree(s->d_times_out); cudaFree(s->d_lat);
   for (int b = 0; b < 2; b++) {
     cudaFreeHost(s->h_seeds[b]);
@@ -218,15 +217,22 @@ static int need_idle(lbft_sim* s) {
 
 static int create_on_device(lbft_sim* s, const lbft_config* config, lbft_sim** out_sim);
 
-// The body of lbft_create / lbft_create_sweep / lbft_create_sweep_faults: build(hs) fills the host setup of a new handle, or
-// returns false with hs.error set; then the device half.
+// The body of the lbft_create* entry points: build(hs) fills the host setup of a new handle, or returns false with hs.error set;
+// then the device half.  (The host tables can be large: a rights sweep keeps a leader table per distinct row of rights.)
 template <class Build>
 static int create_handle(const lbft_config* config, lbft_sim** out_sim, Build build) {
   if (!config || !out_sim) return set_error(LBFT_ERR_INVALID, "config and out_sim must not be NULL");
   *out_sim = nullptr;
   lbft_sim* s = new (std::nothrow) lbft_sim();
   if (!s) return set_error(LBFT_ERR_NOMEM, "out of host memory");
-  if (!build(s->hs)) {
+  bool built = false;
+  try {
+    built = build(s->hs);
+  } catch (const std::bad_alloc&) {
+    delete s;
+    return set_error(LBFT_ERR_NOMEM, "out of host memory for the handle's host tables");
+  }
+  if (!built) {
     std::string e = s->hs.error;
     delete s;
     return set_error(LBFT_ERR_INVALID, e);
@@ -262,10 +268,15 @@ int lbft_create_sweep_faults(const lbft_config* config, const lbft_param_set* se
                        [&](HostSetup& hs) { return hs.build_sweep_faults(*config, sets, faults, num_sets, set_of_instance); });
 }
 
+int lbft_create_sweep_rights(const lbft_config* config, const lbft_param_set* sets, const lbft_fault_set* faults,
+                             const uint64_t* voting_rights, uint32_t num_sets, const uint32_t* set_of_instance, lbft_sim** out_sim) {
+  return create_handle(config, out_sim,
+                       [&](HostSetup& hs) { return hs.build_sweep_rights(*config, sets, faults, voting_rights, num_sets, set_of_instance); });
+}
+
 }  // extern "C"
 
-// The device half of lbft_create / lbft_create_sweep / lbft_create_sweep_faults, once the host setup `s->hs` is built: takes
-// ownership of `s`.
+// The device half of the lbft_create* entry points, once the host setup `s->hs` is built: takes ownership of `s`.
 static int create_on_device(lbft_sim* s, const lbft_config* config, lbft_sim** out_sim) {
   s->I = config->num_instances;
   s->N = config->num_nodes;
@@ -336,17 +347,10 @@ static int create_on_device(lbft_sim* s, const lbft_config* config, lbft_sim** o
   CREATE_TRY(cudaMemcpy(s->d_weights, s->hs.weights.data(), N * sizeof(uint32_t), cudaMemcpyHostToDevice));
   if (s->d_delay_thr)
     CREATE_TRY(cudaMemcpy(s->d_delay_thr, s->hs.delay_thr.data(), s->hs.delay_thr.size() * sizeof(double), cudaMemcpyHostToDevice));
-  if (!s->hs.sets.empty() && s->hs.faults.empty()) {
-    CREATE_TRY(dev_alloc(s, &s->d_sets, s->hs.sets.size()));
-    CREATE_TRY(cudaMemcpy(s->d_sets, s->hs.sets.data(), s->hs.sets.size() * sizeof(SweepSet), cudaMemcpyHostToDevice));
-  }
-  if (!s->hs.faults.empty()) {
-    std::vector<SweepSetFaults> table(s->hs.sets.size());
-    for (size_t k = 0; k < table.size(); k++) table[k] = SweepSetFaults{s->hs.sets[k], s->hs.faults[k]};
-    CREATE_TRY(dev_alloc(s, &s->d_set_faults, table.size()));
-    CREATE_TRY(cudaMemcpy(s->d_set_faults, table.data(), table.size() * sizeof(SweepSetFaults), cudaMemcpyHostToDevice));
-  }
   if (!s->hs.sets.empty()) {
+    const std::vector<uint64_t> table = s->hs.set_table();
+    CREATE_TRY(dev_alloc(s, &s->d_sets, table.size()));
+    CREATE_TRY(cudaMemcpy(s->d_sets, table.data(), table.size() * sizeof(uint64_t), cudaMemcpyHostToDevice));
     CREATE_TRY(dev_alloc(s, &s->d_set_of, I));
     CREATE_TRY(cudaMemcpy(s->d_set_of, s->hs.set_of.data(), I * sizeof(uint32_t), cudaMemcpyHostToDevice));
   }
@@ -477,14 +481,19 @@ int lbft_run_until(lbft_sim* s, int64_t stop_clock) {
 
 }  // extern "C"
 
+// A rights sweep's device table (lbft_create_sweep_rights), or null: the read-outs take each instance's leaders and weights from it.
+static const SweepSetRights* rights_table(const lbft_sim* s) {
+  return s->hs.rights.empty() ? nullptr : reinterpret_cast<const SweepSetRights*>(s->d_sets);
+}
+
 static int enqueue_kernel(lbft_sim* s) {
   s->P.stop_clock = (int32_t)(s->P.resumable ? s->next_stop : (int64_t)s->P.max_clock);
   s->P.run_flags = (s->P.resumable && s->started) ? 1u : 0u;
   CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
   CUDA_TRY(cudaEventRecord(s->ev[2], s->stream));
   const KernelSel& k = s->hs.sel;
-  const SweepParams sp{s->P, s->d_set_of, s->d_set_faults ? reinterpret_cast<const SweepSet*>(s->d_set_faults) : s->d_sets,
-                       s->d_set_faults ? 1u : 0u, 0u};
+  const uint32_t records = s->hs.records();
+  const SweepParams sp{s->P, s->d_set_of, reinterpret_cast<const SweepSet*>(s->d_sets), records & 1u, (records >> 1) & 1u};
   const CtParams<Params> cp{s->P, s->d_times};
   const CtParams<SweepParams> csp{sp, s->d_times};
   cudaError_t e = k.ct ? (k.sweep ? (k.wide ? launch_ct_sweep_wide(k, csp, s->stream) : launch_ct_sweep_thread(k, csp, s->stream))
@@ -644,11 +653,12 @@ int lbft_commit_log(lbft_sim* s, uint32_t instance, uint32_t node, lbft_commit* 
     CUDA_TRY(cudaMemcpy2D(einit.data(), sizeof(uint32_t), s->d_state + ((size_t)tile * L.total_words + L.einit_base) * S + lane,
                           S * sizeof(uint32_t), sizeof(uint32_t), L.epochs, cudaMemcpyDeviceToHost));
   std::vector<lbft_commit> log(count);
+  const uint32_t leaders = rights_table(s) ? s->hs.rights[s->hs.set_of[instance]].leader_off : 0u;  // the instance's leader table
   uint32_t i = count;
   for (uint32_t r = lc; r != 0 && i > 0;) {
     if (r >= L.round_cap) return set_error(LBFT_ERR_STATE, "corrupt chain table");
     --i;
-    log[i].proposer = s->hs.leader[r % L.rspan];
+    log[i].proposer = s->hs.leader[leaders + r % L.rspan];
     log[i].index = chain[2 * r] >> 16;
     log[i].time = (int64_t)(int32_t)chain[2 * r + 1];
     const uint32_t p = chain[2 * r] & 0xffffu, e = r / L.rspan;
@@ -695,19 +705,22 @@ static int finish_chain_check(lbft_sim* s) {
 // ancestor chain of its last committed block; the kernel lays out the LONGEST log of each instance in commit order
 // (sim_core.cuh walk_commit_chain, which also verifies that every other node's last committed block lies on it at
 // depth == its commit count, SURVEY App. C.3).  Instances where that does not hold are counted in *bad.
+// The proposer of round r is leader(r) of the instance's leader table: on a rights sweep (`rights` not null) its set's.
 // ---------------------------------------------------------------------------------------------
-__global__ void lbft_commit_logs_kernel(const __grid_constant__ Params P, uint32_t stride, lbft_commit* out, uint32_t cap, uint32_t* bad) {
+__global__ void lbft_commit_logs_kernel(const __grid_constant__ Params P, uint32_t stride, const uint32_t* set_of, const SweepSetRights* rights,
+                                        lbft_commit* out, uint32_t cap, uint32_t* bad) {
   const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= P.num_instances) return;
   const Layout& L = P.L;
   const uint32_t N = L.num_nodes, tile = inst / stride, lane = inst % stride;
   const uint32_t* tb = P.state + (size_t)tile * L.total_words * stride + lane;
+  const uint8_t* leader = P.leader + (rights ? rights[set_of[inst]].rights.leader_off : 0u);
   lbft_commit* row = out + (size_t)inst * cap;
   if (!walk_commit_chain(L, tb, stride, P.out_commit_counts + (size_t)inst * N, P.out_lc_round + (size_t)inst * N,
                          [&](uint32_t k, uint32_t r, uint32_t c0) {
                            if (k >= cap) return;
                            lbft_commit e;
-                           e.proposer = P.leader[r % L.rspan];
+                           e.proposer = leader[r % L.rspan];
                            e.index = c0 >> 16;
                            e.time = (int64_t)(int32_t)tb[(size_t)(L.chain_base + 2 * r + 1) * stride];
                            row[k] = e;
@@ -726,7 +739,8 @@ int lbft_commit_logs(lbft_sim* s, lbft_commit* out, size_t cap, uint32_t* lens) 
   // rows beyond a log's length are zero
   CUDA_TRY(cudaMemsetAsync(s->d_logs, 0, bytes, s->stream));
   CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
-  lbft_commit_logs_kernel<<<(s->I + 127) / 128, 128, 0, s->stream>>>(s->P, s->stride, s->d_logs, (uint32_t)cap, s->d_error);
+  lbft_commit_logs_kernel<<<(s->I + 127) / 128, 128, 0, s->stream>>>(s->P, s->stride, s->d_set_of, rights_table(s), s->d_logs,
+                                                                       (uint32_t)cap, s->d_error);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaMemcpyAsync(out, s->d_logs, bytes, cudaMemcpyDeviceToHost, s->stream));
   const int r = finish_chain_check(s);  // (the lengths are returned when the chain check fails too)
@@ -866,18 +880,19 @@ __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __g
   red.finish(sum, nullptr);
 }
 
-// lbft_block_latency_stats: per-group block-latency statistics at a voting-rights threshold W (sim_core.cuh
-// block_latency_samples_of).  An overload of the per-sample kernel above: the same reduction over other samples, so tools that
+// lbft_block_latency_stats / lbft_block_latency_stats_groups: per-group block-latency statistics at a voting-rights threshold
+// W[g] per group g (sim_core.cuh block_latency_samples_of).  An overload of the per-sample kernel above: the same reduction over other samples, so tools that
 // list the library's kernels by name see it as the latency reduction it is.  A group of G lanes per instance, G the smallest
 // power of two >= min(N, 32), so lane j holds nodes j and, when N > 32, j + 32.  Every lane of the group walks the chain (same
 // addresses: broadcast loads).  Per block, lane j loads its nodes' commit times (+inf where the node did not commit it) and
-// sums, over G width-G shuffles under the group's mask, the voting rights (P.c_weights, indexed by the source lane) of the
-// nodes with a time <= each of its own; the group then takes the least time whose sum reaches W (sim_core.cuh
+// sums, over G width-G shuffles under the group's mask, the voting rights (P.c_weights, or on a rights sweep its set's,
+// indexed by the source lane) of the nodes with a time <= each of its own; the group then takes the least time whose sum reaches W (sim_core.cuh
 // block_threshold_time_lanes: block_threshold_time without a per-node array), and lane 0 of the group accumulates the sample or
 // the unreached block into the reduction of the per-sample kernel (LatencyReduction).
 __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __grid_constant__ Params P, uint32_t stride,
                                                                        const int32_t* times, const uint32_t* set_of,
-                                                                       uint32_t G, uint32_t W, int64_t width, uint32_t bins,
+                                                                       const SweepSetRights* rights, uint32_t G, const uint32_t* W,
+                                                                       int64_t width, uint32_t bins,
                                                                        int64_t from, int64_t until, lbft_latency_summary* sum,
                                                                        unsigned long long* unreached_out,
                                                                        unsigned long long* hist, uint32_t* bad) {
@@ -895,8 +910,10 @@ __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __g
     const uint32_t gmask = G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (warp_lane & ~(G - 1));
     const uint32_t n0 = j, n1 = j + 32;  // (n1 < N only when N > 32, i.e. G == 32)
     const uint32_t cc0 = n0 < N ? cc[n0] : 0u, cc1 = n1 < N ? cc[n1] : 0u;
+    const uint32_t* w = rights ? rights[red.g].rights.weights : P.c_weights;  // (red.g: the instance's set on a sweep)
+    const uint32_t Wg = W[red.g];
     auto time_of = [&](uint32_t k, uint32_t r) -> int64_t {
-      return block_threshold_time_lanes(L, G, gmask, j, cc0, cc1, t_inst, P.c_weights, k, r, W);
+      return block_threshold_time_lanes(L, G, gmask, j, cc0, cc1, t_inst, w, k, r, Wg);
     };
     const bool ok = block_latency_samples_of(
         L, P.state + (size_t)tile * L.total_words * stride + lane, stride, cc, P.out_lc_round + (size_t)inst * N, t_inst, from, until,
@@ -917,21 +934,21 @@ static int need_commit_times(lbft_sim* s) {
   return LBFT_OK;
 }
 
-// lbft_latency_stats (threshold 0: the per-sample overload of lbft_latency_stats_kernel) and lbft_block_latency_stats (the
-// threshold overload), once their arguments are checked.  The buffer holds [groups] summaries, [groups] unreached counts and
-// the [groups][num_bins] bins, which lbft_latency_init_kernel sets in one pass; unreached is NULL for a per-sample call.
-static int latency_stats(lbft_sim* s, const lbft_latency_spec* spec, uint64_t threshold, lbft_latency_summary* out,
+// lbft_latency_stats (thresholds NULL: the per-sample overload of lbft_latency_stats_kernel) and lbft_block_latency_stats /
+// lbft_block_latency_stats_groups (the threshold overload, thresholds[groups]), once their arguments are checked.  The buffer
+// holds [groups] summaries, [groups] unreached counts and the [groups][num_bins] bins, which lbft_latency_init_kernel sets in
+// one pass, then the [groups] thresholds; unreached is NULL for a per-sample call.
+static int latency_stats(lbft_sim* s, const lbft_latency_spec* spec, const uint64_t* thresholds, lbft_latency_summary* out,
                          uint64_t* unreached, uint64_t* hist) {
   if (int r = need_idle(s)) return r;
   CUDA_TRY(cudaSetDevice(s->device));
   const uint32_t groups = latency_groups(s->hs), bins = spec->num_bins;
-  const size_t hist_len = (size_t)groups * bins;
-  if (int r = grow_buffer(s->d_lat, s->lat_bytes, groups * sizeof(lbft_latency_summary) + (groups + hist_len) * sizeof(uint64_t),
-                          "latency-statistics buffer"))
-    return r;
+  const size_t hist_len = (size_t)groups * bins, counts_bytes = groups * sizeof(lbft_latency_summary) + (groups + hist_len) * sizeof(uint64_t);
+  if (int r = grow_buffer(s->d_lat, s->lat_bytes, counts_bytes + groups * sizeof(uint32_t), "latency-statistics buffer")) return r;
   lbft_latency_summary* d_sum = reinterpret_cast<lbft_latency_summary*>(s->d_lat);
   unsigned long long* d_unreached = reinterpret_cast<unsigned long long*>(s->d_lat + groups * sizeof(lbft_latency_summary));
   unsigned long long* d_hist = d_unreached + groups;
+  uint32_t* d_thresholds = reinterpret_cast<uint32_t*>(s->d_lat + counts_bytes);
   const size_t init_blocks = (groups + hist_len + 255) / 256;
   lbft_latency_init_kernel<<<(unsigned)(init_blocks < 4096 ? init_blocks : 4096), 256, 0, s->stream>>>(d_sum, groups, d_unreached,
                                                                                                        groups + hist_len);
@@ -939,7 +956,8 @@ static int latency_stats(lbft_sim* s, const lbft_latency_spec* spec, uint64_t th
   CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
   const uint32_t* set_of = s->hs.sel.sweep ? s->d_set_of : nullptr;
   const size_t smem = bins <= kLatSharedBins ? bins * sizeof(uint32_t) : 0;
-  if (threshold == 0) {
+  std::vector<uint32_t> W;  // (lives until finish_chain_check has synchronised the stream)
+  if (!thresholds) {
     lbft_latency_stats_kernel<<<(s->I + kLatBlock - 1) / kLatBlock, kLatBlock, smem, s->stream>>>(
         s->P, s->stride, s->d_times, set_of, spec->bin_width, bins, spec->proposed_from, spec->proposed_until, d_sum, d_hist,
         s->d_error);
@@ -947,8 +965,10 @@ static int latency_stats(lbft_sim* s, const lbft_latency_spec* spec, uint64_t th
     uint32_t G = 1;  // lanes per instance: the smallest power of two >= min(N, 32)
     while (G < s->N && G < 32) G <<= 1;
     const uint32_t per_block = kLatBlock / G;
+    W.assign(thresholds, thresholds + groups);  // (checked: each at most 64 * 2^24)
+    CUDA_TRY(cudaMemcpyAsync(d_thresholds, W.data(), groups * sizeof(uint32_t), cudaMemcpyHostToDevice, s->stream));
     lbft_latency_stats_kernel<<<(s->I + per_block - 1) / per_block, kLatBlock, smem, s->stream>>>(
-        s->P, s->stride, s->d_times, set_of, G, (uint32_t)threshold, spec->bin_width, bins, spec->proposed_from,
+        s->P, s->stride, s->d_times, set_of, rights_table(s), G, d_thresholds, spec->bin_width, bins, spec->proposed_from,
         spec->proposed_until, d_sum, d_unreached, d_hist, s->d_error);
   }
   CUDA_TRY(cudaGetLastError());
@@ -986,7 +1006,7 @@ int lbft_latency_stats(lbft_sim* s, const lbft_latency_spec* spec, lbft_latency_
   if (!s || !spec || !out) return set_error(LBFT_ERR_INVALID, "sim, spec and out must not be NULL");
   if (int r = need_commit_times(s)) return r;
   if (const char* e = latency_spec_error(s->hs, *spec)) return set_error(LBFT_ERR_INVALID, e);
-  return latency_stats(s, spec, 0, out, nullptr, hist);
+  return latency_stats(s, spec, nullptr, out, nullptr, hist);
 }
 
 int lbft_block_latency_stats(lbft_sim* s, const lbft_latency_spec* spec, uint64_t threshold, lbft_latency_summary* out,
@@ -995,7 +1015,17 @@ int lbft_block_latency_stats(lbft_sim* s, const lbft_latency_spec* spec, uint64_
   if (int r = need_commit_times(s)) return r;
   if (const char* e = latency_spec_error(s->hs, *spec)) return set_error(LBFT_ERR_INVALID, e);
   if (const char* e = block_latency_threshold_error(s->hs, threshold)) return set_error(LBFT_ERR_INVALID, e);
-  return latency_stats(s, spec, threshold, out, unreached, hist);
+  const std::vector<uint64_t> thresholds(latency_groups(s->hs), threshold);
+  return latency_stats(s, spec, thresholds.data(), out, unreached, hist);
+}
+
+int lbft_block_latency_stats_groups(lbft_sim* s, const lbft_latency_spec* spec, const uint64_t* thresholds, lbft_latency_summary* out,
+                                    uint64_t* unreached, uint64_t* hist) {
+  if (!s || !spec || !out || !thresholds) return set_error(LBFT_ERR_INVALID, "sim, spec, thresholds and out must not be NULL");
+  if (int r = need_commit_times(s)) return r;
+  if (const char* e = latency_spec_error(s->hs, *spec)) return set_error(LBFT_ERR_INVALID, e);
+  if (const char* e = block_latency_thresholds_error(s->hs, thresholds)) return set_error(LBFT_ERR_INVALID, e);
+  return latency_stats(s, spec, thresholds, out, unreached, hist);
 }
 
 int lbft_round_switches(lbft_sim* s, uint32_t instance, lbft_round_switch* out, size_t cap, size_t* n) {

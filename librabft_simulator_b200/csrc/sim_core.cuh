@@ -314,6 +314,47 @@ LBFT_HD uint64_t silent_mask_behind(const SweepSet* set) {
 #endif
 }
 
+// The rights record behind parameter set `set` in a rights sweep's table (SweepSetRights; Core::weight / quorum / leader), read
+// the same way: author a's voting right, the quorum and where the set's leader table starts.
+static_assert(offsetof(SweepSetRights, rights) == 80 && offsetof(SweepRights, leader_off) == 4 && offsetof(SweepRights, weights) == 8,
+              "the immediates below");
+LBFT_HD uint32_t weight_behind(const SweepSet* set, uint32_t a) {
+#if defined(__CUDA_ARCH__)
+  uint32_t v;
+  asm volatile("ld.global.nc.u32 %0, [%1+88];" : "=r"(v) : "l"(reinterpret_cast<const uint32_t*>(set) + a));
+  return v;
+#else
+  return reinterpret_cast<const SweepSetRights*>(set)->rights.weights[a];
+#endif
+}
+LBFT_HD uint32_t quorum_behind(const SweepSet* set) {
+#if defined(__CUDA_ARCH__)
+  uint32_t v;
+  asm volatile("ld.global.nc.u32 %0, [%1+80];" : "=r"(v) : "l"(set));
+  return v;
+#else
+  return reinterpret_cast<const SweepSetRights*>(set)->rights.quorum;
+#endif
+}
+LBFT_HD uint32_t leader_off_behind(const SweepSet* set) {
+#if defined(__CUDA_ARCH__)
+  uint32_t v;
+  asm volatile("ld.global.nc.u32 %0, [%1+84];" : "=r"(v) : "l"(set));
+  return v;
+#else
+  return reinterpret_cast<const SweepSetRights*>(set)->rights.leader_off;
+#endif
+}
+
+static_assert(offsetof(SweepParams, P) == 0, "Core::sweep_records: a sweep kernel's Params heads its SweepParams");
+
+// Set s of a sweep's device table, whose entries are SweepSet, SweepSetFaults or SweepSetRights by `records` (bit 0: a fault
+// record follows each set, bit 1: a rights record follows that).
+LBFT_HD const SweepSet* sweep_set_at(const SweepSet* sets, uint32_t s, uint32_t records) {
+  const size_t pitch = (records & 2) ? sizeof(SweepSetRights) : ((records & 1) ? sizeof(SweepSetFaults) : sizeof(SweepSet));
+  return reinterpret_cast<const SweepSet*>(reinterpret_cast<const char*>(sets) + pitch * s);
+}
+
 // Partition plan (EXTENSION, SURVEY App. D.3): the windows open at `clock` and the next clock at which that set changes.
 // Out of line: it runs at most twice per window per run, and inlined into every send site it costs the kernels that never
 // see a partition ~5 % of their code.  packed: the open windows' author masks themselves, 16 bits per window (<= 4 windows,
@@ -651,7 +692,8 @@ struct Core {
   const double* zf;
   const double* thr;  // delay thresholds (shared-memory copy on the device when it fits; SW: the instance's set's, bind_set)
   const SweepSet* sw = nullptr;  // SW: the instance's parameter set
-  bool faults = false;           // SW: a fault sweep: `sw` points into a SweepSetFaults table (bind_faults)
+  uint32_t records = 0;          // SW, host: the records behind `sw` (sweep_set_at): bit 0 faults (bind_faults), bit 1 rights
+                                 // (bind_rights); the device reads them from the launch's parameter block instead (sweep_records)
   using Queue = QueueFor<QMODE, Mem, G, KS>;
   Queue q;                 // given its shared memory by the constructor (QMODE 2: sk / sd, or the host harness's stand-in) and init (km)
   uint32_t* km = nullptr;  // KS: the calendar's occupancy words in shared memory, a column per lane, set by the kernel
@@ -697,34 +739,63 @@ struct Core {
   // The fault model: the launch's (Params, Layout), or on a fault sweep the record of the instance's set (bind_faults).
   // SW: on a fault sweep (SweepParams::faults), the set bound by bind_set is the head of a SweepSetFaults entry whose fault
   // record follows it; before init.  The sweep kernels sit at their register bound: a record pointer, or a silent mask, held
-  // through the event loop spills there and slows every sweep.  So nothing is held but this flag (uniform over the launch):
+  // through the event loop spills there and slows every sweep.  So nothing is held (the flag: sweep_records):
   // the record is read at a fixed offset from `sw`, the silent mask where a node is tested (is_silent), and the window count
   // only enters the plan drawn at init.
-  LBFT_HD void bind_faults(bool fault_sweep) { faults = fault_sweep; }
+  LBFT_HD void bind_faults(bool fault_sweep) { records = (records & ~1u) | (fault_sweep ? 1u : 0u); }
+  // SW: which records follow the bound set.  On the device `P` is the head of the launch's SweepParams (every sweep kernel binds
+  // Core to S.P), so the flags are constant-bank reads of SweepParams::faults / rights: nothing is held through the event loop,
+  // where the sweep kernels sit at their 128-register bound.  (The host harness binds a bare Params and sets `records`.)
+  LBFT_HD uint32_t sweep_records() const {
+#if defined(__CUDA_ARCH__)
+    const SweepParams& S = *reinterpret_cast<const SweepParams*>(&P);
+    return (S.faults ? 1u : 0u) | (S.rights ? 2u : 0u);
+#else
+    return records;
+#endif
+  }
+  LBFT_HD bool faults() const { return sweep_records() & 1; }
   LBFT_HD const SweepFaults& fault_record() const { return reinterpret_cast<const SweepSetFaults*>(sw)->faults; }
   // Whether the instance may have silent nodes, and whether node n is one.  On a fault sweep P.silent_mask is the union of
   // the sets' silent nodes (HostSetup::build_sweep), so the launch-uniform test skips the record wherever no set has any.
   LBFT_HD bool any_silent() const { return P.silent_mask; }
   LBFT_HD bool is_silent(uint32_t n) const {
-    if constexpr (SW) return ((P.silent_mask >> n) & 1) && (!faults || ((silent_mask_behind(sw) >> n) & 1));
+    if constexpr (SW) return ((P.silent_mask >> n) & 1) && (!faults() || ((silent_mask_behind(sw) >> n) & 1));
     else return (P.silent_mask >> n) & 1;
   }
   // SW: whether run() drops an event of `kind` for `receiver` from `sender` unhandled (a silent receiver handles nothing, and a
   // silent sender's request is not answered), with one load of the mask.
   LBFT_HD bool sweep_silent_drop(uint32_t kind, uint32_t receiver, uint32_t sender) const {
-    const uint64_t mask = faults ? silent_mask_behind(sw) : P.silent_mask;
+    const uint64_t mask = faults() ? silent_mask_behind(sw) : P.silent_mask;
     return ((mask >> receiver) | (kind == EV_REQUEST ? mask >> sender : 0)) & 1;
   }
   // The plan's window count and length, read when init() draws the plan.  A set never has more windows than the layout;
   // init() leaves the layout's windows past the set's count empty ([0, 0): never open), so partitioned() and the send path stay
   // keyed on L.part_windows, as packed_plan() is.
   LBFT_HD uint32_t part_windows() const {
-    if constexpr (SW) return faults ? fault_record().part_windows : L.part_windows;
+    if constexpr (SW) return faults() ? fault_record().part_windows : L.part_windows;
     else return L.part_windows;
   }
   LBFT_HD uint32_t part_max_len() const {
-    if constexpr (SW) return faults ? fault_record().part_max_len : P.part_max_len;
+    if constexpr (SW) return faults() ? fault_record().part_max_len : P.part_max_len;
     else return P.part_max_len;
+  }
+  // The voting rights: the launch's (Params), or on a rights sweep the record of the instance's set (bind_rights), which sits
+  // behind its fault record (SweepSetRights: a rights sweep is a fault sweep too).  As with the faults, the loop holds nothing
+  // new (sweep_records): the weight and the quorum are loaded where a vote or a timeout is tallied, the leader table's
+  // offset where a leader is read (round_leader) (once per round change, and in finalize).
+  LBFT_HD void bind_rights(bool rights_sweep) { records = (records & ~2u) | (rights_sweep ? 2u : 0u); }
+  LBFT_HD uint32_t weight(uint32_t a) const {
+    if constexpr (SW) return (sweep_records() & 2) ? weight_behind(sw, a) : P.c_weights[a];
+    else return P.c_weights[a];
+  }
+  LBFT_HD uint32_t quorum() const {
+    if constexpr (SW) return (sweep_records() & 2) ? quorum_behind(sw) : P.quorum;
+    else return P.quorum;
+  }
+  LBFT_HD uint32_t round_leader(uint32_t r) const {
+    if constexpr (SW) return (sweep_records() & 2) ? P.leader[leader_off_behind(sw) + r] : P.leader[r];
+    else return P.leader[r];
   }
 
   // ------------------------------------------------------------------------------------------
@@ -1175,8 +1246,8 @@ struct Core {
     if ((d.vmask >> author) & 1) return;
     d.vmask |= (mask_t)1 << author;
     if (election(d) == 0) {
-      d.f[F_BALLOT] += P.c_weights[author];
-      if (d.f[F_BALLOT] >= P.quorum) set_election(d, 1);
+      d.f[F_BALLOT] += weight(author);
+      if (d.f[F_BALLOT] >= quorum()) set_election(d, 1);
     }
   }
   // Record::QuorumCertificate — verify :330-389, insert :500-526
@@ -1205,8 +1276,8 @@ struct Core {
     if ((d.tmask >> author) & 1) return;
     d.tmask |= (mask_t)1 << author;
     put_timeout_hcbr(d, author, hcbr);
-    d.f[F_TOW] += P.c_weights[author];
-    if (d.f[F_TOW] >= P.quorum) {
+    d.f[F_TOW] += weight(author);
+    if (d.f[F_TOW] >= quorum()) {
       d.tcmask = d.tmask;
       copy_timeout_hcbr_to_tc(d);
       d.f[F_TC_ROUND] = d.f[F_CUR];
@@ -1328,7 +1399,7 @@ struct Core {
     if (new_epoch || active > d.f[F_PMR]) {
       d.f[F_PMR] = active;
       d.f[F_PM_START] = (uint32_t)clk;
-      uint32_t ld = P.leader[active];
+      uint32_t ld = round_leader(active);
       d.f[F_FLAGS] = (d.f[F_FLAGS] & ~(0xffu << FL_LEADER_SHIFT)) | (ld << FL_LEADER_SHIFT);
       uint32_t base = d.f[F_HCR] > 0 ? d.f[F_HCR] + 2 : 0;  // duration(), :111-124
       if (!(active > base)) { status |= ST_INVARIANT; base = active - 1; }
@@ -1383,7 +1454,7 @@ struct Core {
     // ---- check_for_new_quorum_certificate (record_store.rs:702-738) and QC broadcast, node.rs:277-283
     if (election(d) == 1) {
       uint32_t r = d.f[F_CUR];
-      if (P.leader[r] == n) {
+      if (round_leader(r) == n) {
         set_election(d, 2);
         // likewise at most one QC per round: the election is Closed until the round advances (debug check only)
 #ifdef LBFT_CHECK_C1
@@ -1977,7 +2048,7 @@ struct Core {
         uint32_t r = m.ld(scratch + k);
         uint32_t c0 = m.ld(L.chain_base + 2 * r);
         int32_t tm = (int32_t)m.ld(L.chain_base + 2 * r + 1);
-        h.write_u64(P.leader[multi() ? r % L.rspan : r]);
+        h.write_u64(round_leader(multi() ? r % L.rspan : r));
         h.write_u64(c0 >> 16);
         h.write_u64((uint64_t)(int64_t)tm);
       }

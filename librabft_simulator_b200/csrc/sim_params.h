@@ -271,15 +271,31 @@ struct SweepSetFaults {
   SweepFaults faults;
 };
 
+// The voting rights of one parameter set of a rights sweep (lbft_create_sweep_rights): what Params::c_weights, quorum and
+// leader give every instance of a plain handle.  The set's leader table starts at Params::leader[leader_off]; sets with equal
+// rights share one table.
+struct SweepRights {
+  uint32_t quorum;
+  uint32_t leader_off;
+  uint32_t weights[64];  // 0 past num_nodes
+};
+// One entry of a rights sweep's device table: the set, its fault record (its own faults, or the configuration's shared ones)
+// and its rights record, each at a fixed offset from the set pointer an instance holds (sim_core.cuh Core::bind_rights).
+struct SweepSetRights {
+  SweepSetFaults sf;
+  SweepRights rights;
+};
+
 // The parameter block of a sweep handle's kernels (lbft_create_sweep): instance i runs with sets[set_of[i]], and
 // P.delay_thr / P.duration / P.period are the concatenated tables of all sets.  (A block of its own rather than fields
 // appended to Params, so that no other kernel's parameters move.)
 struct SweepParams {
   Params P;
   const uint32_t* set_of;  // [num_instances]
-  const SweepSet* sets;    // [num_sets]; a fault sweep (lbft_create_sweep_faults): the sets of a SweepSetFaults [num_sets] table
-  uint32_t faults;         // 1: a fault sweep, whose instances take their silent nodes and partition plan from their set's record
-  uint32_t pad;
+  const SweepSet* sets;    // [num_sets]; a fault sweep (lbft_create_sweep_faults): the sets of a SweepSetFaults [num_sets] table;
+                           // a rights sweep (lbft_create_sweep_rights): of a SweepSetRights [num_sets] table
+  uint32_t faults;         // 1: a fault or rights sweep, whose instances take their silent nodes and partition plan from their set's record
+  uint32_t rights;         // 1: a rights sweep, whose instances take their voting rights, quorum and leaders from their set's record
 };
 
 }  // namespace lbft

@@ -67,13 +67,16 @@ class LatencyStats:
 class BlockLatencyStats(LatencyStats):
     """Block-latency statistics per group at a voting-rights threshold (``BatchResult.block_latency_stats``): the fields of
     ``LatencyStats``, where a sample is one block's latency from its proposal to the time the nodes that committed it reach
-    ``threshold`` voting rights, plus ``unreached[groups]``, the blocks that never reached it, and the resolved integer
-    ``threshold``."""
+    the group's threshold in voting rights, plus ``unreached[groups]``, the blocks that never reached it, the resolved integer
+    ``thresholds[groups]``, and ``threshold``: their common value, or None when the groups' thresholds differ (a named
+    threshold on a sweep whose sets carry different voting rights)."""
 
     def __init__(self, summary, unreached, hist, bin_width, threshold):
         super().__init__(summary, hist, bin_width)
         self.unreached = unreached
-        self.threshold = int(threshold)
+        t = np.asarray(threshold, dtype=np.int64).reshape(-1)
+        self.thresholds = np.broadcast_to(t, (len(unreached),)).copy() if t.size == 1 else t
+        self.threshold = int(t[0]) if (t == t[0]).all() else None
 
 
 def resolve_threshold(threshold, total):
@@ -527,15 +530,26 @@ class BatchSimulator:
         """The sum of the voting rights of the committee (each node holds 1 unless ``voting_rights`` says otherwise)."""
         return self.num_nodes if self.voting_rights is None else int(self.voting_rights.sum())
 
+    def group_voting_rights(self):
+        """The total voting rights of each group of ``latency_stats`` / ``block_latency_stats``, as an int64 array: the one
+        group of a plain simulator holds ``total_voting_rights()``."""
+        return np.full(1, self.total_voting_rights(), dtype=np.int64)
+
     def block_latency_stats(self, threshold="quorum", num_bins=1024, bin_width=1, proposed_from=0, proposed_until=None):
         """``lbft_block_latency_stats``: per-group block-latency statistics at a voting-rights threshold as a
-        ``BlockLatencyStats`` (see ``BatchResult.block_latency_stats``)."""
-        w = resolve_threshold(threshold, self.total_voting_rights())
+        ``BlockLatencyStats`` (see ``BatchResult.block_latency_stats``).  A named threshold is resolved per group, with the
+        group's total voting rights; where the groups' totals differ it goes through ``lbft_block_latency_stats_groups``."""
         spec, summary, hist = self._latency_buffers(num_bins, bin_width, proposed_from, proposed_until)
         unreached = np.zeros(summary.shape[0], dtype=np.uint64)
-        _lib.check(self._lib.lbft_block_latency_stats(self._handle, ctypes.byref(spec), ctypes.c_uint64(min(max(w, 0), (1 << 64) - 1)),
-                                                      ctypes.c_void_p(summary.ctypes.data), ctypes.c_void_p(unreached.ctypes.data),
-                                                      ctypes.c_void_p(hist.ctypes.data) if hist.size else None))
+        totals = self.group_voting_rights()
+        out = (ctypes.c_void_p(summary.ctypes.data), ctypes.c_void_p(unreached.ctypes.data),
+               ctypes.c_void_p(hist.ctypes.data) if hist.size else None)
+        if isinstance(threshold, str) and (totals != totals[0]).any():
+            w = np.array([resolve_threshold(threshold, int(t)) for t in totals], dtype=np.uint64)
+            _lib.check(self._lib.lbft_block_latency_stats_groups(self._handle, ctypes.byref(spec), ctypes.c_void_p(w.ctypes.data), *out))
+        else:
+            w = resolve_threshold(threshold, int(totals[0]))
+            _lib.check(self._lib.lbft_block_latency_stats(self._handle, ctypes.byref(spec), ctypes.c_uint64(min(max(w, 0), (1 << 64) - 1)), *out))
         return BlockLatencyStats(summary, unreached, hist, spec.bin_width, w)
 
     def round_switches(self, instance):
@@ -578,10 +592,16 @@ class FaultSet:
 @dataclass(frozen=True)
 class ParamSet:
     """One point of a parameter sweep: the network delay and ``NodeConfig`` of the instances assigned to it
-    (main.rs --mean / --variance and --delta / --gamma / --lambda / --target_commit_interval), and its fault model."""
+    (main.rs --mean / --variance and --delta / --gamma / --lambda / --target_commit_interval), its fault model, and its
+    voting rights: a tuple of one int per node, or None for 1 per node (``BatchSimulator``'s ``voting_rights``)."""
     network_delay: RandomDelay = RandomDelay()
     node_config: NodeConfig = NodeConfig()
     faults: FaultSet = FaultSet()
+    voting_rights: tuple = None
+
+    def __post_init__(self):
+        if self.voting_rights is not None:  # (a list or array compares, and hashes, as a tuple)
+            object.__setattr__(self, "voting_rights", tuple(int(w) for w in self.voting_rights))
 
     def to_c(self):
         d, n = self.network_delay, self.node_config
@@ -595,8 +615,10 @@ class SweepSimulator(BatchSimulator):
     ``param_sets[set_of_instance[i]]``; everything else (committee, voting rights, ``commands_per_epoch``, capacities,
     device) is shared and passed as for ``BatchSimulator``.  Silent nodes and partitions are shared too, unless a set carries
     a ``FaultSet`` of its own: then every set has its own (``lbft_create_sweep_faults``) and the shared ``silent`` /
-    ``partition_*`` arguments must be left unset.  Every result of instance i is what a ``BatchSimulator`` with that set's
-    delay, node config and faults computes for it.  Running, re-seeding (the set assignment stays), streaming and reading
+    ``partition_*`` arguments must be left unset.  Likewise the voting rights: when a set carries its own
+    (``lbft_create_sweep_rights``), every set has its own (1 per node where left None) and ``voting_rights`` must be left
+    unset.  Every result of instance i is what a ``BatchSimulator`` with that set's delay, node config, faults and voting
+    rights computes for it.  Running, re-seeding (the set assignment stays), streaming and reading
     results work as on a ``BatchSimulator``."""
 
     def __init__(self, seeds, num_nodes, param_sets, set_of_instance, **shared):
@@ -607,38 +629,75 @@ class SweepSimulator(BatchSimulator):
             raise ValueError("set_of_instance needs one entry per seed (%d)" % self.num_instances)
 
     @classmethod
-    def grid(cls, seeds_per_point, delays, node_configs, num_nodes=4, faults=None, **shared):
+    def grid(cls, seeds_per_point, delays, node_configs, num_nodes=4, faults=None, voting_rights=None, **shared):
         """The Cartesian product ``delays x node_configs`` (point p = i * len(node_configs) + j), each point run over the
         same seeds (``seeds_per_point``: a sequence of seeds, or a count k for seeds 0..k-1) in a contiguous block of
         instances: point p holds instances [p * k, (p + 1) * k).  ``set_of_instance`` and ``param_sets`` say which is which.
         ``faults``, a list of ``FaultSet``, adds a third, fastest-varying axis: point p = (i * len(node_configs) + j) *
-        len(faults) + f, so ``latency_stats().mean().reshape(len(delays), len(node_configs), len(faults))`` is the cube."""
+        len(faults) + f, so ``latency_stats().mean().reshape(len(delays), len(node_configs), len(faults))`` is the cube.
+        ``voting_rights``, a list of rows of one voting right per node, adds a fastest-varying axis after that (after
+        ``node_configs`` when ``faults`` is None): ``block_latency_stats("quorum").mean().reshape(len(delays),
+        len(node_configs), len(faults), len(voting_rights))``."""
         seeds = np.arange(seeds_per_point, dtype=np.uint64) if np.isscalar(seeds_per_point) else \
             np.asarray(seeds_per_point, dtype=np.uint64).reshape(-1)
         sets = [ParamSet(d, n) for d in delays for n in node_configs] if faults is None else \
             [ParamSet(d, n, f) for d in delays for n in node_configs for f in faults]
+        if voting_rights is not None:
+            sets = [ParamSet(p.network_delay, p.node_config, p.faults, v) for p in sets for v in voting_rights]
         k = seeds.shape[0]
         return cls(np.tile(seeds, len(sets)), num_nodes, sets, np.repeat(np.arange(len(sets), dtype=np.uint32), k), **shared)
 
     def create(self, max_clock):
-        """``lbft_create_sweep``, or ``lbft_create_sweep_faults`` when some set has faults: validate every set, build the
-        per-set host tables, allocate device state."""
+        """``lbft_create_sweep``, or ``lbft_create_sweep_faults`` when some set has faults, or ``lbft_create_sweep_rights``
+        when some set has voting rights: validate every set, build the per-set host tables, allocate device state."""
         per_set = any(p.faults != FaultSet() for p in self.param_sets)
         if per_set and (self.silent is not None or self.partition_windows or self.partition_max_len):
             raise ValueError("a sweep takes silent nodes and partitions either per set (ParamSet.faults) or shared (silent / "
                              "partition_windows / partition_max_len), not both")
+        rights = self._rights_table()
+        if rights is not None and self.voting_rights is not None:
+            raise ValueError("a sweep takes voting rights either per set (ParamSet.voting_rights) or shared (voting_rights), not both")
         self.close()
         handle = ctypes.c_void_p()
         cfg = self.make_config(max_clock)
         sets = (_lib.LbftParamSet * max(1, len(self.param_sets)))(*[p.to_c() for p in self.param_sets])
         so = ctypes.c_void_p(self.set_of_instance.ctypes.data)
-        if per_set:
-            faults = (_lib.LbftFaultSet * len(self.param_sets))(*[p.faults.to_c() for p in self.param_sets])
+        faults = (_lib.LbftFaultSet * len(self.param_sets))(*[p.faults.to_c() for p in self.param_sets]) if per_set else None
+        if rights is not None:
+            _lib.check(self._lib.lbft_create_sweep_rights(ctypes.byref(cfg), sets, faults, ctypes.c_void_p(rights.ctypes.data),
+                                                          len(self.param_sets), so, ctypes.byref(handle)))
+        elif per_set:
             _lib.check(self._lib.lbft_create_sweep_faults(ctypes.byref(cfg), sets, faults, len(self.param_sets), so, ctypes.byref(handle)))
         else:
             _lib.check(self._lib.lbft_create_sweep(ctypes.byref(cfg), sets, len(self.param_sets), so, ctypes.byref(handle)))
         self._handle = handle
         return self
+
+    def _rights_table(self):
+        """The [num_sets][num_nodes] voting rights of a rights sweep (1 per node where a set leaves them None), or None when
+        no set carries any."""
+        if all(p.voting_rights is None for p in self.param_sets):
+            return None
+        rows = [(1,) * self.num_nodes if p.voting_rights is None else p.voting_rights for p in self.param_sets]
+        if any(len(r) != self.num_nodes for r in rows):
+            raise ValueError("ParamSet.voting_rights needs one entry per node (%d)" % self.num_nodes)
+        return np.ascontiguousarray(rows, dtype=np.uint64)
+
+    def total_voting_rights(self):
+        """The sum of the voting rights of the committee; on a sweep whose sets carry their own voting rights, their common
+        total (``ValueError`` when the sets' totals differ: see ``group_voting_rights``)."""
+        totals = self.group_voting_rights()
+        if (totals != totals[0]).any():
+            raise ValueError("the parameter sets of this sweep have different total voting rights: use group_voting_rights()")
+        return int(totals[0])
+
+    def group_voting_rights(self):
+        """The total voting rights of each parameter set (a group of the latency statistics), as an int64 array: its own
+        row's total on a rights sweep, the shared committee's otherwise."""
+        rights = self._rights_table()
+        if rights is None:
+            return np.full(len(self.param_sets), super().total_voting_rights(), dtype=np.int64)
+        return rights.sum(axis=1).astype(np.int64)
 
 
 def format_round_switches_csv(num_nodes, switches):
