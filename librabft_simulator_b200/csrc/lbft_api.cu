@@ -10,6 +10,7 @@
 
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <string>
 #include <vector>
@@ -45,122 +46,146 @@ static int set_error(int code, const std::string& msg) {
       return set_error(LBFT_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e_));             \
   } while (0)
 
-// Pinned host mirrors of one run's summaries.  There are two sets: an asynchronous run fills the one the getters are not
-// reading, so the results of run k stay readable while run k+1 is in flight (lbft_run_async / lbft_wait).
-struct HostResults {
-  uint32_t* commit_counts = nullptr;
-  uint32_t* lc_round = nullptr;
-  uint64_t* last_state = nullptr;
-  uint32_t* counters = nullptr;
-  uint32_t* status = nullptr;
-  uint32_t* rounds = nullptr;
-  uint32_t* error = nullptr;  // [1] OR of the status words with an error bit
+// The owners of a handle's CUDA resources: each frees what it holds when it is destroyed.  Memory is the only code that
+// allocates or frees the handle's memory: on the device (Pinned false) or pinned on the host (true).
+template <bool Pinned>
+class Memory {
+ public:
+  Memory() = default;
+  Memory(const Memory&) = delete;
+  Memory& operator=(const Memory&) = delete;
+  ~Memory() { release(); }
+  // Replaces what it holds by `bytes` of new memory; holds nothing when that fails.  A failed allocation is reported by the
+  // return value alone: the runtime's record of it is cleared, so that the next launch's error check does not see it.
+  cudaError_t alloc(size_t bytes) {
+    release();
+    void* p = nullptr;
+    const cudaError_t e = Pinned ? cudaMallocHost(&p, bytes) : cudaMalloc(&p, bytes);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      return e;
+    }
+    p_ = static_cast<unsigned char*>(p);
+    bytes_ = bytes;
+    return cudaSuccess;
+  }
+  size_t bytes() const { return bytes_; }
+  template <class T = unsigned char>
+  T* at(size_t offset = 0) const { return reinterpret_cast<T*>(p_ + offset); }
+
+ private:
+  void release() {
+    if (Pinned) cudaFreeHost(p_);
+    else cudaFree(p_);
+    p_ = nullptr;
+    bytes_ = 0;
+  }
+  unsigned char* p_ = nullptr;
+  size_t bytes_ = 0;
+};
+using DeviceMemory = Memory<false>;
+using PinnedMemory = Memory<true>;
+
+// A stream or an event, created into `h` and destroyed with its owner.
+template <class H, cudaError_t (*Destroy)(H)>
+struct Owned {
+  H h = nullptr;
+  Owned() = default;
+  Owned(const Owned&) = delete;
+  Owned& operator=(const Owned&) = delete;
+  ~Owned() {
+    if (h) Destroy(h);
+  }
+  operator H() const { return h; }
+};
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+
+// The per-run results, in the order of the outputs block and of its pinned host mirrors.  The first three regions are
+// lbft_device_buffer(5) (include/lbft.h).  Only the first holds 8-byte words, so no region needs padding.
+enum Output { OUT_LAST_STATE, OUT_COMMIT_COUNTS, OUT_ROUNDS, OUT_LC_ROUND, OUT_COUNTERS, OUT_STATUS, OUT_ERROR, OUT_END };
+class OutputLayout {
+ public:
+  OutputLayout(size_t I = 0, size_t N = 0) {
+    const size_t bytes[OUT_END] = {I * N * sizeof(uint64_t), I * N * sizeof(uint32_t), I * sizeof(uint32_t),
+                                   I * N * sizeof(uint32_t), I * 12 * sizeof(uint32_t), I * sizeof(uint32_t),
+                                   sizeof(uint32_t)};  // (error: the OR of the status words with an error bit)
+    for (int r = 0; r < OUT_END; r++) at_[r + 1] = at_[r] + bytes[r];
+  }
+  size_t offset(Output r) const { return at_[r]; }
+  size_t bytes(Output r) const { return at_[r + 1] - at_[r]; }
+  size_t total() const { return at_[OUT_END]; }
+
+ private:
+  size_t at_[OUT_END + 1] = {};
 };
 
 struct lbft_sim {
   HostSetup hs;
-  Params P{};
+  Params P{};  // its device pointers point into `inputs`, `state` and `outputs`
   int device = 0;
   uint32_t I = 0, N = 0;
   uint32_t stride = 32;  // instances per tile (the lane-interleaving factor of the state layout)
-  std::vector<uint64_t> seeds_host;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[6] = {};
-  // device buffers
-  uint64_t* d_seeds = nullptr;
-  double* d_zx = nullptr;
-  double* d_zf = nullptr;
-  uint8_t* d_leader = nullptr;
-  int32_t* d_duration = nullptr;
-  int32_t* d_period = nullptr;
-  uint32_t* d_weights = nullptr;
-  double* d_delay_thr = nullptr;
-  uint64_t* d_sets = nullptr;    // sweep handles only: HostSetup::set_table (each set with the records HostSetup::records names)
-  uint32_t* d_set_of = nullptr;  // sweep handles only
-  uint32_t* d_state = nullptr;
-  uint32_t* d_commit_counts = nullptr;
-  uint32_t* d_lc_round = nullptr;
-  uint64_t* d_last_state = nullptr;
-  uint32_t* d_counters = nullptr;
-  uint32_t* d_status = nullptr;
-  uint32_t* d_rounds = nullptr;
-  uint32_t* d_error = nullptr;
-  // d_last_state, d_commit_counts and d_rounds are carved out of ONE allocation, in this order, so that the per-instance
-  // summaries a multi-GPU caller all-gathers travel in a single collective (lbft_device_buffer(5))
-  unsigned char* d_summary = nullptr;
-  size_t summary_bytes = 0;
-  // the read-out buffers, allocated on first use and grown by grow_buffer: each with its size in bytes
-  lbft_commit* d_logs = nullptr;  // lbft_commit_logs: [I][cap]
-  size_t logs_bytes = 0;
-  int32_t* d_times = nullptr;    // LBFT_FLAG_COMMIT_TIMES: the commit-time table [I][N + 1][round_cap] (sim_core.cuh Core CT)
-  int64_t* d_times_out = nullptr;  // lbft_commit_times: [I][N][cap] committed, then [I][cap] proposed
-  size_t times_bytes = 0;
-  unsigned char* d_lat = nullptr;  // lbft_latency_stats / lbft_block_latency_stats: summaries, unreached counts and bins
-  size_t lat_bytes = 0;
+  Stream stream;
+  Event ev[6];
+  // Device memory counted in lbft_memory_info:
+  //  * inputs: the seeds, then the launch-invariant tables (create_on_device);
+  //  * outputs: the per-run results (regions);
+  //  * state: the instance state, an allocation of its own, which the bench kernel's 128-bit lane-block accesses rely on;
+  //  * times: LBFT_FLAG_COMMIT_TIMES' commit-time table [I][N + 1][round_cap] (sim_core.cuh Core CT), never cleared.
+  DeviceMemory inputs, outputs, state, times;
+  OutputLayout regions;
+  const uint64_t* sets = nullptr;    // sweep handles only, in `inputs`: HostSetup::set_table
+  const uint32_t* set_of = nullptr;  // sweep handles only, in `inputs`
+  // the read-out buffers, allocated on first use and grown by grow_buffer
+  DeviceMemory logs;       // lbft_commit_logs: [I][cap]
+  DeviceMemory times_out;  // lbft_commit_times: [I][N][cap] committed, then [I][cap] proposed
+  DeviceMemory lat;        // lbft_latency_stats / lbft_block_latency_stats: summaries, unreached counts and bins
   uint64_t device_bytes = 0;
-  // pinned host staging: two seed buffers (lbft_set_seeds never writes the one an in-flight upload reads) and two
-  // result sets (see HostResults)
-  uint64_t* h_seeds[2] = {nullptr, nullptr};
+  // pinned host staging: two seed buffers (lbft_set_seeds never writes the one an in-flight upload reads) and two mirrors
+  // of `outputs` (an asynchronous run fills the one the getters are not reading, so the results of run k stay readable while
+  // run k+1 is in flight: lbft_run_async / lbft_wait)
+  PinnedMemory h_seeds[2];
   int seed_set = 0;        // buffer holding the most recently set seeds
   int seed_inflight = -1;  // buffer an in-flight upload is reading, -1 if none
-  HostResults res[2];
+  PinnedMemory res[2];
   int done = 0;            // result set the getters read
   bool pending = false;    // an lbft_run_async has not been waited for
-  bool pending_download = false;  // ... and it includes the device->host copies
   bool uploaded = false, ran = false, downloaded = false;
   bool started = false;     // resumable handles: a staged run is in progress, the next launch restores the instances
   int64_t next_stop = 0;    // stop clock of the next launch (max_clock unless set by lbft_run_until)
   int64_t last_stop = -1;   // stop clock of the last launch
   lbft_timing timing{};
-};
 
-template <class T>
-static cudaError_t dev_alloc(lbft_sim* s, T** p, size_t count) {
-  cudaError_t e = cudaMalloc((void**)p, count * sizeof(T));
-  if (e == cudaSuccess) s->device_bytes += count * sizeof(T);
-  return e;
-}
-
-static void free_all(lbft_sim* s) {
-  if (!s) return;
-  cudaSetDevice(s->device);
-  if (s->stream) cudaStreamSynchronize(s->stream);  // an lbft_run_async may still be in flight
-  cudaFree(s->d_seeds); cudaFree(s->d_zx); cudaFree(s->d_zf); cudaFree(s->d_leader); cudaFree(s->d_duration);
-  cudaFree(s->d_period); cudaFree(s->d_weights); cudaFree(s->d_delay_thr); cudaFree(s->d_state); cudaFree(s->d_summary);
-  cudaFree(s->d_lc_round); cudaFree(s->d_counters); cudaFree(s->d_status);
-  cudaFree(s->d_error); cudaFree(s->d_logs); cudaFree(s->d_sets); cudaFree(s->d_set_of);
-  cudaFree(s->d_times); cudaFree(s->d_times_out); cudaFree(s->d_lat);
-  for (int b = 0; b < 2; b++) {
-    cudaFreeHost(s->h_seeds[b]);
-    HostResults& r = s->res[b];
-    cudaFreeHost(r.commit_counts); cudaFreeHost(r.lc_round); cudaFreeHost(r.last_state); cudaFreeHost(r.counters);
-    cudaFreeHost(r.status); cudaFreeHost(r.rounds); cudaFreeHost(r.error);
+  // The members free their resources after this, with the handle's device current.  (One process may drive several GPUs.)
+  ~lbft_sim() {
+    if (!stream) return;  // nothing was created on the device
+    cudaSetDevice(device);
+    cudaStreamSynchronize(stream);  // an lbft_run_async may still be in flight
   }
-  for (auto& e : s->ev)
-    if (e) cudaEventDestroy(e);
-  if (s->stream) cudaStreamDestroy(s->stream);
-  delete s;
-}
+  // Allocates one of the four blocks above, counted in device_bytes.
+  cudaError_t dev_alloc(DeviceMemory& m, size_t bytes) {
+    const cudaError_t e = m.alloc(bytes);
+    if (e == cudaSuccess) device_bytes += bytes;
+    return e;
+  }
+  // Region r of the finished run's results, in the host mirror the getters read.
+  template <class T>
+  const T* result(Output r) const { return res[done].at<T>(regions.offset(r)); }
+};
 
 // The three phases of a run, enqueued on the handle's stream without waiting.
 static int enqueue_upload(lbft_sim* s) {
   CUDA_TRY(cudaEventRecord(s->ev[0], s->stream));
-  CUDA_TRY(cudaMemcpyAsync(s->d_seeds, s->h_seeds[s->seed_set], s->I * sizeof(uint64_t), cudaMemcpyHostToDevice, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(s->inputs.at(), s->h_seeds[s->seed_set].at(), s->I * sizeof(uint64_t), cudaMemcpyHostToDevice, s->stream));
   CUDA_TRY(cudaEventRecord(s->ev[1], s->stream));
   s->seed_inflight = s->seed_set;
   return LBFT_OK;
 }
 static int enqueue_kernel(lbft_sim* s);
-static int enqueue_download(lbft_sim* s, HostResults& r) {
-  const size_t I = s->I, N = s->N;
+static int enqueue_download(lbft_sim* s, PinnedMemory& r) {
   CUDA_TRY(cudaEventRecord(s->ev[4], s->stream));
-  CUDA_TRY(cudaMemcpyAsync(r.commit_counts, s->d_commit_counts, I * N * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(r.lc_round, s->d_lc_round, I * N * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(r.last_state, s->d_last_state, I * N * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(r.counters, s->d_counters, I * 12 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(r.status, s->d_status, I * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(r.rounds, s->d_rounds, I * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(r.error, s->d_error, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(r.at(), s->outputs.at(), s->regions.total(), cudaMemcpyDeviceToHost, s->stream));
   CUDA_TRY(cudaEventRecord(s->ev[5], s->stream));
   return LBFT_OK;
 }
@@ -191,18 +216,17 @@ static int finish_kernel(lbft_sim* s) {
 static int finish_download(lbft_sim* s, int set) {
   float ms = 0;
   CUDA_TRY(cudaEventElapsedTime(&ms, s->ev[4], s->ev[5]));
-  const size_t I = s->I, N = s->N;
   s->timing.d2h_ms = ms;
-  s->timing.d2h_bytes = I * N * (2 * sizeof(uint32_t) + sizeof(uint64_t)) + I * 14 * sizeof(uint32_t) + sizeof(uint32_t);
+  s->timing.d2h_bytes = s->regions.total();
   s->done = set;
   s->downloaded = true;
-  const HostResults& r = s->res[set];
-  if (*r.error & LBFT_ST_ERROR_MASK) {
-    for (size_t i = 0; i < I; i++)
-      if (r.status[i] & LBFT_ST_ERROR_MASK) {
+  const uint32_t* status = s->result<uint32_t>(OUT_STATUS);
+  if (*s->result<uint32_t>(OUT_ERROR) & LBFT_ST_ERROR_MASK) {
+    for (size_t i = 0; i < s->I; i++)
+      if (status[i] & LBFT_ST_ERROR_MASK) {
         char buf[360];
         snprintf(buf, sizeof buf, "instance %zu ended with status 0x%x (see lbft_status; raise round_cap/queue_cap/payload_cap%s)", i,
-                 r.status[i], (r.status[i] & LBFT_ST_QUEUE_OVERFLOW) ? "; QUEUE_OVERFLOW also means the queue mode ran out of creation "
+                 status[i], (status[i] & LBFT_ST_QUEUE_OVERFLOW) ? "; QUEUE_OVERFLOW also means the queue mode ran out of creation "
                  "stamps: queue_cap > 512 selects a queue with wider stamps" : "");
         return set_error(LBFT_ERR_CAPACITY, buf);
       }
@@ -215,7 +239,7 @@ static int need_idle(lbft_sim* s) {
   return LBFT_OK;
 }
 
-static int create_on_device(lbft_sim* s, const lbft_config* config, lbft_sim** out_sim);
+static int create_on_device(std::unique_ptr<lbft_sim> s, const lbft_config* config, lbft_sim** out_sim);
 
 // The body of the lbft_create* entry points: build(hs) fills the host setup of a new handle, or returns false with hs.error set;
 // then the device half.  (The host tables can be large: a rights sweep keeps a leader table per distinct row of rights.)
@@ -223,21 +247,16 @@ template <class Build>
 static int create_handle(const lbft_config* config, lbft_sim** out_sim, Build build) {
   if (!config || !out_sim) return set_error(LBFT_ERR_INVALID, "config and out_sim must not be NULL");
   *out_sim = nullptr;
-  lbft_sim* s = new (std::nothrow) lbft_sim();
+  std::unique_ptr<lbft_sim> s(new (std::nothrow) lbft_sim());
   if (!s) return set_error(LBFT_ERR_NOMEM, "out of host memory");
   bool built = false;
   try {
     built = build(s->hs);
   } catch (const std::bad_alloc&) {
-    delete s;
     return set_error(LBFT_ERR_NOMEM, "out of host memory for the handle's host tables");
   }
-  if (!built) {
-    std::string e = s->hs.error;
-    delete s;
-    return set_error(LBFT_ERR_INVALID, e);
-  }
-  return create_on_device(s, config, out_sim);
+  if (!built) return set_error(LBFT_ERR_INVALID, s->hs.error);
+  return create_on_device(std::move(s), config, out_sim);
 }
 
 extern "C" {
@@ -276,103 +295,82 @@ int lbft_create_sweep_rights(const lbft_config* config, const lbft_param_set* se
 
 }  // extern "C"
 
-// The device half of the lbft_create* entry points, once the host setup `s->hs` is built: takes ownership of `s`.
-static int create_on_device(lbft_sim* s, const lbft_config* config, lbft_sim** out_sim) {
+// The device half of the lbft_create* entry points, once the host setup `s->hs` is built.  On failure the partial handle is
+// deleted, and its owners free what it holds.
+static int create_on_device(std::unique_ptr<lbft_sim> s, const lbft_config* config, lbft_sim** out_sim) {
   s->I = config->num_instances;
   s->N = config->num_nodes;
   s->device = config->device;
   s->stride = (uint32_t)s->hs.sel.tile;
-  s->seeds_host.assign(config->seeds, config->seeds + s->I);
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) {
-    delete s;
+  if (e != cudaSuccess || ndev == 0)
     return set_error(LBFT_ERR_CUDA, std::string("no usable CUDA device (there is no CPU fallback): ") + cudaGetErrorString(e));
-  }
-  if (s->device < 0 || s->device >= ndev) {
-    delete s;
-    return set_error(LBFT_ERR_INVALID, "device ordinal out of range");
-  }
-#define CREATE_TRY(expr)                                                                      \
-  do {                                                                                        \
-    cudaError_t e2_ = (expr);                                                                 \
-    if (e2_ != cudaSuccess) {                                                                 \
-      std::string m_ = std::string(#expr) + ": " + cudaGetErrorString(e2_);                 \
-      free_all(s);                                                                            \
-      return set_error(e2_ == cudaErrorMemoryAllocation ? LBFT_ERR_NOMEM : LBFT_ERR_CUDA, m_); \
-    }                                                                                         \
+  if (s->device < 0 || s->device >= ndev) return set_error(LBFT_ERR_INVALID, "device ordinal out of range");
+#define CREATE_TRY(expr)                                                                                         \
+  do {                                                                                                           \
+    cudaError_t e2_ = (expr);                                                                                    \
+    if (e2_ != cudaSuccess)                                                                                      \
+      return set_error(e2_ == cudaErrorMemoryAllocation ? LBFT_ERR_NOMEM : LBFT_ERR_CUDA,                        \
+                       std::string(#expr) + ": " + cudaGetErrorString(e2_));                                     \
   } while (0)
   CREATE_TRY(cudaSetDevice(s->device));
-  CREATE_TRY(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
-  for (auto& evt : s->ev) CREATE_TRY(cudaEventCreate(&evt));
-  const Layout& L = s->hs.params.L;
+  CREATE_TRY(cudaStreamCreateWithFlags(&s->stream.h, cudaStreamNonBlocking));
+  for (auto& evt : s->ev) CREATE_TRY(cudaEventCreate(&evt.h));
+  const HostSetup& hs = s->hs;
   const size_t I = s->I, N = s->N, tiles = (I + s->stride - 1) / s->stride;
-  CREATE_TRY(dev_alloc(s, &s->d_seeds, I));
-  CREATE_TRY(dev_alloc(s, &s->d_zx, 257));
-  CREATE_TRY(dev_alloc(s, &s->d_zf, 257));
-  CREATE_TRY(dev_alloc(s, &s->d_leader, s->hs.leader.size()));
-  CREATE_TRY(dev_alloc(s, &s->d_duration, s->hs.duration.size()));
-  CREATE_TRY(dev_alloc(s, &s->d_period, s->hs.period.size()));
-  CREATE_TRY(dev_alloc(s, &s->d_weights, N));
-  if (!s->hs.delay_thr.empty()) CREATE_TRY(dev_alloc(s, &s->d_delay_thr, s->hs.delay_thr.size()));
-  CREATE_TRY(dev_alloc(s, &s->d_state, tiles * L.total_words * s->stride));
-  s->summary_bytes = I * N * sizeof(uint64_t) + I * N * sizeof(uint32_t) + I * sizeof(uint32_t);
-  CREATE_TRY(dev_alloc(s, &s->d_summary, s->summary_bytes));
-  s->d_last_state = reinterpret_cast<uint64_t*>(s->d_summary);
-  s->d_commit_counts = reinterpret_cast<uint32_t*>(s->d_summary + I * N * sizeof(uint64_t));
-  s->d_rounds = s->d_commit_counts + I * N;
-  CREATE_TRY(dev_alloc(s, &s->d_lc_round, I * N));
-  CREATE_TRY(dev_alloc(s, &s->d_counters, I * 12));
-  CREATE_TRY(dev_alloc(s, &s->d_status, I));
-  CREATE_TRY(dev_alloc(s, &s->d_error, 1));
-  if (s->hs.sel.ct) CREATE_TRY(dev_alloc(s, &s->d_times, I * (N + 1) * L.round_cap));  // (never cleared: see Core CT)
+  // The inputs block: the seeds (uploaded by every run), then the launch-invariant tables, uploaded here in one copy.  The
+  // regions are ordered by element size, so none needs padding; a table that is empty has no region and a null pointer.
+  const std::vector<uint64_t> set_table = hs.set_table();  // (empty on a plain handle)
+  const size_t seeds_bytes = I * sizeof(uint64_t);
+  std::vector<unsigned char> tables;
+  auto stage = [&](const auto& v) {  // -> the region's offset in the block
+    const size_t at = seeds_bytes + tables.size();
+    const unsigned char* b = reinterpret_cast<const unsigned char*>(v.data());
+    tables.insert(tables.end(), b, b + v.size() * sizeof(v[0]));
+    return at;
+  };
+  const size_t zig_x = stage(hs.zig_x), zig_f = stage(hs.zig_f), delay_thr = stage(hs.delay_thr), sets = stage(set_table),
+               duration = stage(hs.duration), period = stage(hs.period), weights = stage(hs.weights), set_of = stage(hs.set_of),
+               leader = stage(hs.leader);
+  CREATE_TRY(s->dev_alloc(s->inputs, seeds_bytes + tables.size()));
+  CREATE_TRY(cudaMemcpy(s->inputs.at(seeds_bytes), tables.data(), tables.size(), cudaMemcpyHostToDevice));
+  s->regions = OutputLayout(I, N);
+  CREATE_TRY(s->dev_alloc(s->outputs, s->regions.total()));
+  CREATE_TRY(s->dev_alloc(s->state, tiles * hs.params.L.total_words * s->stride * sizeof(uint32_t)));
+  if (hs.sel.ct) CREATE_TRY(s->dev_alloc(s->times, I * (N + 1) * hs.params.L.round_cap * sizeof(int32_t)));
   for (int b = 0; b < 2; b++) {
-    HostResults& r = s->res[b];
-    CREATE_TRY(cudaMallocHost((void**)&s->h_seeds[b], I * sizeof(uint64_t)));
-    CREATE_TRY(cudaMallocHost((void**)&r.commit_counts, I * N * sizeof(uint32_t)));
-    CREATE_TRY(cudaMallocHost((void**)&r.lc_round, I * N * sizeof(uint32_t)));
-    CREATE_TRY(cudaMallocHost((void**)&r.last_state, I * N * sizeof(uint64_t)));
-    CREATE_TRY(cudaMallocHost((void**)&r.counters, I * 12 * sizeof(uint32_t)));
-    CREATE_TRY(cudaMallocHost((void**)&r.status, I * sizeof(uint32_t)));
-    CREATE_TRY(cudaMallocHost((void**)&r.rounds, I * sizeof(uint32_t)));
-    CREATE_TRY(cudaMallocHost((void**)&r.error, sizeof(uint32_t)));
-  }
-  memcpy(s->h_seeds[0], s->seeds_host.data(), I * sizeof(uint64_t));
-  // launch-invariant tables
-  CREATE_TRY(cudaMemcpy(s->d_zx, s->hs.zig_x.data(), 257 * sizeof(double), cudaMemcpyHostToDevice));
-  CREATE_TRY(cudaMemcpy(s->d_zf, s->hs.zig_f.data(), 257 * sizeof(double), cudaMemcpyHostToDevice));
-  CREATE_TRY(cudaMemcpy(s->d_leader, s->hs.leader.data(), s->hs.leader.size(), cudaMemcpyHostToDevice));
-  CREATE_TRY(cudaMemcpy(s->d_duration, s->hs.duration.data(), s->hs.duration.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-  CREATE_TRY(cudaMemcpy(s->d_period, s->hs.period.data(), s->hs.period.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-  CREATE_TRY(cudaMemcpy(s->d_weights, s->hs.weights.data(), N * sizeof(uint32_t), cudaMemcpyHostToDevice));
-  if (s->d_delay_thr)
-    CREATE_TRY(cudaMemcpy(s->d_delay_thr, s->hs.delay_thr.data(), s->hs.delay_thr.size() * sizeof(double), cudaMemcpyHostToDevice));
-  if (!s->hs.sets.empty()) {
-    const std::vector<uint64_t> table = s->hs.set_table();
-    CREATE_TRY(dev_alloc(s, &s->d_sets, table.size()));
-    CREATE_TRY(cudaMemcpy(s->d_sets, table.data(), table.size() * sizeof(uint64_t), cudaMemcpyHostToDevice));
-    CREATE_TRY(dev_alloc(s, &s->d_set_of, I));
-    CREATE_TRY(cudaMemcpy(s->d_set_of, s->hs.set_of.data(), I * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    CREATE_TRY(s->h_seeds[b].alloc(seeds_bytes));
+    CREATE_TRY(s->res[b].alloc(s->regions.total()));
   }
 #undef CREATE_TRY
-  s->P = s->hs.params;
-  s->P.seeds = s->d_seeds;
-  s->P.zig_x = s->d_zx;
-  s->P.zig_f = s->d_zf;
-  s->P.leader = s->d_leader;
-  s->P.duration = s->d_duration;
-  s->P.period = s->d_period;
-  s->P.weights = s->d_weights;
-  s->P.delay_thr = s->d_delay_thr;
-  s->P.state = s->d_state;
-  s->P.out_commit_counts = s->d_commit_counts;
-  s->P.out_lc_round = s->d_lc_round;
-  s->P.out_last_state = s->d_last_state;
-  s->P.out_counters = s->d_counters;
-  s->P.out_status = s->d_status;
-  s->P.out_rounds = s->d_rounds;
-  s->P.out_error = s->d_error;
-  *out_sim = s;
+  memcpy(s->h_seeds[0].at(), config->seeds, seeds_bytes);
+  Params& P = s->P;
+  P = hs.params;
+  const DeviceMemory& in = s->inputs;
+  P.seeds = in.at<uint64_t>();
+  P.zig_x = in.at<double>(zig_x);
+  P.zig_f = in.at<double>(zig_f);
+  P.delay_thr = hs.delay_thr.empty() ? nullptr : in.at<double>(delay_thr);
+  P.duration = in.at<int32_t>(duration);
+  P.period = in.at<int32_t>(period);
+  P.weights = in.at<uint32_t>(weights);
+  P.leader = in.at<uint8_t>(leader);
+  if (!set_table.empty()) {
+    s->sets = in.at<uint64_t>(sets);
+    s->set_of = in.at<uint32_t>(set_of);
+  }
+  P.state = s->state.at<uint32_t>();
+  const DeviceMemory& out = s->outputs;
+  const OutputLayout& at = s->regions;
+  P.out_last_state = out.at<uint64_t>(at.offset(OUT_LAST_STATE));
+  P.out_commit_counts = out.at<uint32_t>(at.offset(OUT_COMMIT_COUNTS));
+  P.out_rounds = out.at<uint32_t>(at.offset(OUT_ROUNDS));
+  P.out_lc_round = out.at<uint32_t>(at.offset(OUT_LC_ROUND));
+  P.out_counters = out.at<uint32_t>(at.offset(OUT_COUNTERS));
+  P.out_status = out.at<uint32_t>(at.offset(OUT_STATUS));
+  P.out_error = out.at<uint32_t>(at.offset(OUT_ERROR));
+  *out_sim = s.release();
   return LBFT_OK;
 }
 
@@ -382,7 +380,7 @@ int lbft_set_seeds(lbft_sim* s, const uint64_t* seeds) {
   if (!s || !seeds) return set_error(LBFT_ERR_INVALID, "NULL argument");
   // never the buffer an in-flight upload is reading (lbft_run_async): the caller may stage run k+1 while run k runs
   const int b = s->seed_set != s->seed_inflight ? s->seed_set : 1 - s->seed_set;
-  memcpy(s->h_seeds[b], seeds, (size_t)s->I * sizeof(uint64_t));
+  memcpy(s->h_seeds[b].at(), seeds, (size_t)s->I * sizeof(uint64_t));
   s->seed_set = b;
   s->uploaded = false;
   s->started = false;
@@ -391,16 +389,16 @@ int lbft_set_seeds(lbft_sim* s, const uint64_t* seeds) {
 
 int lbft_device_buffer(lbft_sim* s, uint32_t which, void** device_ptr, size_t* bytes) {
   if (!s || !device_ptr || !bytes) return set_error(LBFT_ERR_INVALID, "NULL argument");
-  const size_t I = s->I, N = s->N;
-  switch (which) {
-    case 0: *device_ptr = s->d_commit_counts; *bytes = I * N * sizeof(uint32_t); break;
-    case 1: *device_ptr = s->d_last_state; *bytes = I * N * sizeof(uint64_t); break;
-    case 2: *device_ptr = s->d_counters; *bytes = I * 12 * sizeof(uint32_t); break;
-    case 3: *device_ptr = s->d_status; *bytes = I * sizeof(uint32_t); break;
-    case 4: *device_ptr = s->d_rounds; *bytes = I * sizeof(uint32_t); break;
-    case 5: *device_ptr = s->d_summary; *bytes = s->summary_bytes; break;
-    default: return set_error(LBFT_ERR_INVALID, "unknown buffer id");
+  if (which > 5) return set_error(LBFT_ERR_INVALID, "unknown buffer id");
+  if (which == 5) {  // the first three regions
+    *device_ptr = s->outputs.at();
+    *bytes = s->regions.offset(OUT_LC_ROUND);
+    return LBFT_OK;
   }
+  static const Output ids[5] = {OUT_COMMIT_COUNTS, OUT_LAST_STATE, OUT_COUNTERS, OUT_STATUS, OUT_ROUNDS};
+  const Output r = ids[which];
+  *device_ptr = s->outputs.at(s->regions.offset(r));
+  *bytes = s->regions.bytes(r);
   return LBFT_OK;
 }
 
@@ -483,19 +481,19 @@ int lbft_run_until(lbft_sim* s, int64_t stop_clock) {
 
 // A rights sweep's device table (lbft_create_sweep_rights), or null: the read-outs take each instance's leaders and weights from it.
 static const SweepSetRights* rights_table(const lbft_sim* s) {
-  return s->hs.rights.empty() ? nullptr : reinterpret_cast<const SweepSetRights*>(s->d_sets);
+  return s->hs.rights.empty() ? nullptr : reinterpret_cast<const SweepSetRights*>(s->sets);
 }
 
 static int enqueue_kernel(lbft_sim* s) {
   s->P.stop_clock = (int32_t)(s->P.resumable ? s->next_stop : (int64_t)s->P.max_clock);
   s->P.run_flags = (s->P.resumable && s->started) ? 1u : 0u;
-  CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
+  CUDA_TRY(cudaMemsetAsync(s->P.out_error, 0, sizeof(uint32_t), s->stream));
   CUDA_TRY(cudaEventRecord(s->ev[2], s->stream));
   const KernelSel& k = s->hs.sel;
   const uint32_t records = s->hs.records();
-  const SweepParams sp{s->P, s->d_set_of, reinterpret_cast<const SweepSet*>(s->d_sets), records & 1u, (records >> 1) & 1u};
-  const CtParams<Params> cp{s->P, s->d_times};
-  const CtParams<SweepParams> csp{sp, s->d_times};
+  const SweepParams sp{s->P, s->set_of, reinterpret_cast<const SweepSet*>(s->sets), records & 1u, (records >> 1) & 1u};
+  const CtParams<Params> cp{s->P, s->times.at<int32_t>()};
+  const CtParams<SweepParams> csp{sp, s->times.at<int32_t>()};
   cudaError_t e = k.ct ? (k.sweep ? (k.wide ? launch_ct_sweep_wide(k, csp, s->stream) : launch_ct_sweep_thread(k, csp, s->stream))
                                   : (k.wide ? launch_ct_wide(k, cp, s->stream) : launch_ct_thread(k, cp, s->stream)))
                   : k.sweep ? (k.wide ? launch_sweep_wide(k, sp, s->stream) : launch_sweep_thread(k, sp, s->stream))
@@ -537,13 +535,12 @@ uint64_t config_digest(const lbft_sim* s) {
   if (!s->hs.delay_thr.empty()) h = fnv1a(h, s->hs.delay_thr.data(), s->hs.delay_thr.size() * sizeof(double));
   return h;
 }
-size_t state_bytes(const lbft_sim* s) { return (size_t)((s->I + s->stride - 1) / s->stride) * s->P.L.total_words * s->stride * sizeof(uint32_t); }
 }  // namespace
 
 int lbft_snapshot_size(lbft_sim* s, size_t* bytes) {
   if (!s || !bytes) return set_error(LBFT_ERR_INVALID, "NULL argument");
   if (!s->P.resumable) return set_error(LBFT_ERR_STATE, "not a resumable handle: set LBFT_FLAG_RESUMABLE in lbft_config.flags");
-  *bytes = sizeof(SnapshotHeader) + state_bytes(s);
+  *bytes = sizeof(SnapshotHeader) + s->state.bytes();
   return LBFT_OK;
 }
 
@@ -556,7 +553,7 @@ int lbft_snapshot_save(lbft_sim* s, void* buf, size_t cap) {
   CUDA_TRY(cudaSetDevice(s->device));
   SnapshotHeader h{kSnapMagic, LBFT_ABI_VERSION, s->I, s->N, s->P.L.total_words, s->P.max_clock, s->last_stop, config_digest(s)};
   memcpy(buf, &h, sizeof h);
-  CUDA_TRY(cudaMemcpy(static_cast<char*>(buf) + sizeof h, s->d_state, state_bytes(s), cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(static_cast<char*>(buf) + sizeof h, s->P.state, s->state.bytes(), cudaMemcpyDeviceToHost));
   return LBFT_OK;
 }
 
@@ -572,7 +569,7 @@ int lbft_snapshot_load(lbft_sim* s, const void* buf, size_t bytes) {
     return set_error(LBFT_ERR_INVALID, "the snapshot was taken from a differently configured simulator");
   if (int r = need_idle(s)) return r;
   CUDA_TRY(cudaSetDevice(s->device));
-  CUDA_TRY(cudaMemcpy(s->d_state, static_cast<const char*>(buf) + sizeof h, state_bytes(s), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(s->P.state, static_cast<const char*>(buf) + sizeof h, s->state.bytes(), cudaMemcpyHostToDevice));
   s->started = true;   // the next lbft_run_until restores the instances from their save areas
   s->uploaded = true;  // the seeds are not needed any more
   s->ran = false;
@@ -588,31 +585,17 @@ static int need_results(lbft_sim* s, const void* out) {
   if (!s->downloaded) return set_error(LBFT_ERR_STATE, "results are not available: call lbft_run (or lbft_download) first");
   return LBFT_OK;
 }
-int lbft_commit_counts(lbft_sim* s, uint32_t* out) {
-  if (int r = need_results(s, out)) return r;
-  memcpy(out, s->res[s->done].commit_counts, (size_t)s->I * s->N * sizeof(uint32_t));
+// Copies region r of the finished run's results to `out`.
+static int read_result(lbft_sim* s, Output r, void* out) {
+  if (int e = need_results(s, out)) return e;
+  memcpy(out, s->result<unsigned char>(r), s->regions.bytes(r));
   return LBFT_OK;
 }
-int lbft_last_states(lbft_sim* s, uint64_t* out) {
-  if (int r = need_results(s, out)) return r;
-  memcpy(out, s->res[s->done].last_state, (size_t)s->I * s->N * sizeof(uint64_t));
-  return LBFT_OK;
-}
-int lbft_counters(lbft_sim* s, lbft_instance_counters* out) {
-  if (int r = need_results(s, out)) return r;
-  memcpy(out, s->res[s->done].counters, (size_t)s->I * 12 * sizeof(uint32_t));
-  return LBFT_OK;
-}
-int lbft_active_rounds(lbft_sim* s, uint32_t* out) {
-  if (int r = need_results(s, out)) return r;
-  memcpy(out, s->res[s->done].rounds, (size_t)s->I * sizeof(uint32_t));  // == lbft_instance_counters.max_active_round
-  return LBFT_OK;
-}
-int lbft_status(lbft_sim* s, uint32_t* out) {
-  if (int r = need_results(s, out)) return r;
-  memcpy(out, s->res[s->done].status, (size_t)s->I * sizeof(uint32_t));
-  return LBFT_OK;
-}
+int lbft_commit_counts(lbft_sim* s, uint32_t* out) { return read_result(s, OUT_COMMIT_COUNTS, out); }
+int lbft_last_states(lbft_sim* s, uint64_t* out) { return read_result(s, OUT_LAST_STATE, out); }
+int lbft_counters(lbft_sim* s, lbft_instance_counters* out) { return read_result(s, OUT_COUNTERS, out); }
+int lbft_active_rounds(lbft_sim* s, uint32_t* out) { return read_result(s, OUT_ROUNDS, out); }  // == counters' max_active_round
+int lbft_status(lbft_sim* s, uint32_t* out) { return read_result(s, OUT_STATUS, out); }
 int lbft_timing_info(lbft_sim* s, lbft_timing* out) {
   if (!s || !out) return set_error(LBFT_ERR_INVALID, "NULL argument");
   *out = s->timing;
@@ -643,14 +626,14 @@ int lbft_commit_log(lbft_sim* s, uint32_t instance, uint32_t node, lbft_commit* 
   const Layout& L = s->P.L;
   std::vector<uint32_t> chain(2 * (size_t)L.round_cap);
   const uint32_t S = s->stride, tile = instance / S, lane = instance % S;
-  const uint32_t* src = s->d_state + ((size_t)tile * L.total_words + L.chain_base) * S + lane;
+  const uint32_t* src = s->P.state + ((size_t)tile * L.total_words + L.chain_base) * S + lane;
   CUDA_TRY(cudaMemcpy2D(chain.data(), sizeof(uint32_t), src, S * sizeof(uint32_t), sizeof(uint32_t), chain.size(), cudaMemcpyDeviceToHost));
-  uint32_t lc = s->res[s->done].lc_round[(size_t)instance * s->N + node];
-  uint32_t count = s->res[s->done].commit_counts[(size_t)instance * s->N + node];
+  uint32_t lc = s->result<uint32_t>(OUT_LC_ROUND)[(size_t)instance * s->N + node];
+  uint32_t count = s->result<uint32_t>(OUT_COMMIT_COUNTS)[(size_t)instance * s->N + node];
   // epochs > 1: the parent of an epoch's first block is the block whose state is the epoch's initial state
   std::vector<uint32_t> einit(L.epochs, 0);
   if (L.epochs > 1)
-    CUDA_TRY(cudaMemcpy2D(einit.data(), sizeof(uint32_t), s->d_state + ((size_t)tile * L.total_words + L.einit_base) * S + lane,
+    CUDA_TRY(cudaMemcpy2D(einit.data(), sizeof(uint32_t), s->P.state + ((size_t)tile * L.total_words + L.einit_base) * S + lane,
                           S * sizeof(uint32_t), sizeof(uint32_t), L.epochs, cudaMemcpyDeviceToHost));
   std::vector<lbft_commit> log(count);
   const uint32_t leaders = rights_table(s) ? s->hs.rights[s->hs.set_of[instance]].leader_off : 0u;  // the instance's leader table
@@ -673,23 +656,18 @@ int lbft_commit_log(lbft_sim* s, uint32_t instance, uint32_t node, lbft_commit* 
 }  // extern "C"
 
 // A read-out buffer grown to at least `bytes` on first use (its contents are not kept); `label` names it in the error.
-template <class T>
-static int grow_buffer(T*& buf, size_t& held, size_t bytes, const char* label) {
-  if (bytes <= held) return LBFT_OK;
-  cudaFree(buf);
-  buf = nullptr;
-  held = 0;
-  cudaError_t e = cudaMalloc((void**)&buf, bytes);
+static int grow_buffer(DeviceMemory& buf, size_t bytes, const char* label) {
+  if (bytes <= buf.bytes()) return LBFT_OK;
+  cudaError_t e = buf.alloc(bytes);
   if (e != cudaSuccess) return set_error(LBFT_ERR_NOMEM, std::string(label) + ": " + cudaGetErrorString(e));
-  held = bytes;
   return LBFT_OK;
 }
 
 // The end of a bulk read-out, once its copies are enqueued: waits for them and fails the call if the kernel counted, in
-// d_error, instances whose node logs are not prefixes of one chain.
+// out_error, instances whose node logs are not prefixes of one chain.
 static int finish_chain_check(lbft_sim* s) {
   uint32_t bad = 0;
-  CUDA_TRY(cudaMemcpyAsync(&bad, s->d_error, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(&bad, s->P.out_error, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
   CUDA_TRY(cudaStreamSynchronize(s->stream));
   if (!bad) return LBFT_OK;
   char buf[160];
@@ -735,16 +713,16 @@ int lbft_commit_logs(lbft_sim* s, lbft_commit* out, size_t cap, uint32_t* lens) 
   if (int r = need_idle(s)) return r;
   CUDA_TRY(cudaSetDevice(s->device));
   const size_t bytes = (size_t)s->I * cap * sizeof(lbft_commit);
-  if (int r = grow_buffer(s->d_logs, s->logs_bytes, bytes, "commit-log buffer")) return r;
+  if (int r = grow_buffer(s->logs, bytes, "commit-log buffer")) return r;
   // rows beyond a log's length are zero
-  CUDA_TRY(cudaMemsetAsync(s->d_logs, 0, bytes, s->stream));
-  CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
-  lbft_commit_logs_kernel<<<(s->I + 127) / 128, 128, 0, s->stream>>>(s->P, s->stride, s->d_set_of, rights_table(s), s->d_logs,
-                                                                       (uint32_t)cap, s->d_error);
+  CUDA_TRY(cudaMemsetAsync(s->logs.at(), 0, bytes, s->stream));
+  CUDA_TRY(cudaMemsetAsync(s->P.out_error, 0, sizeof(uint32_t), s->stream));
+  lbft_commit_logs_kernel<<<(s->I + 127) / 128, 128, 0, s->stream>>>(s->P, s->stride, s->set_of, rights_table(s), s->logs.at<lbft_commit>(),
+                                                                       (uint32_t)cap, s->P.out_error);
   CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemcpyAsync(out, s->d_logs, bytes, cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(out, s->logs.at(), bytes, cudaMemcpyDeviceToHost, s->stream));
   const int r = finish_chain_check(s);  // (the lengths are returned when the chain check fails too)
-  if (lens && r != LBFT_ERR_CUDA) memcpy(lens, s->res[s->done].commit_counts, (size_t)s->I * s->N * sizeof(uint32_t));
+  if (lens && r != LBFT_ERR_CUDA) memcpy(lens, s->result<uint32_t>(OUT_COMMIT_COUNTS), s->regions.bytes(OUT_COMMIT_COUNTS));
   return r;
 }
 
@@ -944,23 +922,23 @@ static int latency_stats(lbft_sim* s, const lbft_latency_spec* spec, const uint6
   CUDA_TRY(cudaSetDevice(s->device));
   const uint32_t groups = latency_groups(s->hs), bins = spec->num_bins;
   const size_t hist_len = (size_t)groups * bins, counts_bytes = groups * sizeof(lbft_latency_summary) + (groups + hist_len) * sizeof(uint64_t);
-  if (int r = grow_buffer(s->d_lat, s->lat_bytes, counts_bytes + groups * sizeof(uint32_t), "latency-statistics buffer")) return r;
-  lbft_latency_summary* d_sum = reinterpret_cast<lbft_latency_summary*>(s->d_lat);
-  unsigned long long* d_unreached = reinterpret_cast<unsigned long long*>(s->d_lat + groups * sizeof(lbft_latency_summary));
+  if (int r = grow_buffer(s->lat, counts_bytes + groups * sizeof(uint32_t), "latency-statistics buffer")) return r;
+  lbft_latency_summary* d_sum = s->lat.at<lbft_latency_summary>();
+  unsigned long long* d_unreached = s->lat.at<unsigned long long>(groups * sizeof(lbft_latency_summary));
   unsigned long long* d_hist = d_unreached + groups;
-  uint32_t* d_thresholds = reinterpret_cast<uint32_t*>(s->d_lat + counts_bytes);
+  uint32_t* d_thresholds = s->lat.at<uint32_t>(counts_bytes);
   const size_t init_blocks = (groups + hist_len + 255) / 256;
   lbft_latency_init_kernel<<<(unsigned)(init_blocks < 4096 ? init_blocks : 4096), 256, 0, s->stream>>>(d_sum, groups, d_unreached,
                                                                                                        groups + hist_len);
   CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
-  const uint32_t* set_of = s->hs.sel.sweep ? s->d_set_of : nullptr;
+  CUDA_TRY(cudaMemsetAsync(s->P.out_error, 0, sizeof(uint32_t), s->stream));
+  const uint32_t* set_of = s->hs.sel.sweep ? s->set_of : nullptr;
   const size_t smem = bins <= kLatSharedBins ? bins * sizeof(uint32_t) : 0;
   std::vector<uint32_t> W;  // (lives until finish_chain_check has synchronised the stream)
   if (!thresholds) {
     lbft_latency_stats_kernel<<<(s->I + kLatBlock - 1) / kLatBlock, kLatBlock, smem, s->stream>>>(
-        s->P, s->stride, s->d_times, set_of, spec->bin_width, bins, spec->proposed_from, spec->proposed_until, d_sum, d_hist,
-        s->d_error);
+        s->P, s->stride, s->times.at<int32_t>(), set_of, spec->bin_width, bins, spec->proposed_from, spec->proposed_until, d_sum, d_hist,
+        s->P.out_error);
   } else {
     uint32_t G = 1;  // lanes per instance: the smallest power of two >= min(N, 32)
     while (G < s->N && G < 32) G <<= 1;
@@ -968,8 +946,8 @@ static int latency_stats(lbft_sim* s, const lbft_latency_spec* spec, const uint6
     W.assign(thresholds, thresholds + groups);  // (checked: each at most 64 * 2^24)
     CUDA_TRY(cudaMemcpyAsync(d_thresholds, W.data(), groups * sizeof(uint32_t), cudaMemcpyHostToDevice, s->stream));
     lbft_latency_stats_kernel<<<(s->I + per_block - 1) / per_block, kLatBlock, smem, s->stream>>>(
-        s->P, s->stride, s->d_times, set_of, rights_table(s), G, d_thresholds, spec->bin_width, bins, spec->proposed_from,
-        spec->proposed_until, d_sum, d_unreached, d_hist, s->d_error);
+        s->P, s->stride, s->times.at<int32_t>(), set_of, rights_table(s), G, d_thresholds, spec->bin_width, bins, spec->proposed_from,
+        spec->proposed_until, d_sum, d_unreached, d_hist, s->P.out_error);
   }
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaMemcpyAsync(out, d_sum, groups * sizeof(lbft_latency_summary), cudaMemcpyDeviceToHost, s->stream));
@@ -990,12 +968,12 @@ int lbft_commit_times(lbft_sim* s, int64_t* committed, int64_t* proposed, size_t
   if (int r = need_idle(s)) return r;
   CUDA_TRY(cudaSetDevice(s->device));
   const size_t I = s->I, N = s->N;
-  if (int r = grow_buffer(s->d_times_out, s->times_bytes, I * (N + 1) * cap * sizeof(int64_t), "commit-time buffer")) return r;
-  int64_t* d_committed = s->d_times_out;
-  int64_t* d_proposed = s->d_times_out + I * N * cap;
-  CUDA_TRY(cudaMemsetAsync(s->d_error, 0, sizeof(uint32_t), s->stream));
-  lbft_commit_times_kernel<<<(s->I + 127) / 128, 128, 0, s->stream>>>(s->P, s->stride, s->d_times, (uint32_t)cap, d_committed,
-                                                                        d_proposed, s->d_error);
+  if (int r = grow_buffer(s->times_out, I * (N + 1) * cap * sizeof(int64_t), "commit-time buffer")) return r;
+  int64_t* d_committed = s->times_out.at<int64_t>();
+  int64_t* d_proposed = d_committed + I * N * cap;
+  CUDA_TRY(cudaMemsetAsync(s->P.out_error, 0, sizeof(uint32_t), s->stream));
+  lbft_commit_times_kernel<<<(s->I + 127) / 128, 128, 0, s->stream>>>(s->P, s->stride, s->times.at<int32_t>(), (uint32_t)cap, d_committed,
+                                                                        d_proposed, s->P.out_error);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaMemcpyAsync(committed, d_committed, I * N * cap * sizeof(int64_t), cudaMemcpyDeviceToHost, s->stream));
   if (proposed) CUDA_TRY(cudaMemcpyAsync(proposed, d_proposed, I * cap * sizeof(int64_t), cudaMemcpyDeviceToHost, s->stream));
@@ -1039,7 +1017,7 @@ int lbft_round_switches(lbft_sim* s, uint32_t instance, lbft_round_switch* out, 
   const uint32_t row = L.round_cap + 1;
   std::vector<uint32_t> table((size_t)s->N * row);
   const uint32_t S = s->stride, tile = instance / S, lane = instance % S;
-  const uint32_t* src = s->d_state + ((size_t)tile * L.total_words + rs_table_base(L)) * S + lane;
+  const uint32_t* src = s->P.state + ((size_t)tile * L.total_words + rs_table_base(L)) * S + lane;
   CUDA_TRY(cudaMemcpy2D(table.data(), sizeof(uint32_t), src, S * sizeof(uint32_t), sizeof(uint32_t), table.size(), cudaMemcpyDeviceToHost));
   size_t k = 0;
   for (uint32_t node = 0; node < s->N; node++)
@@ -1053,6 +1031,6 @@ int lbft_round_switches(lbft_sim* s, uint32_t instance, lbft_round_switch* out, 
   return LBFT_OK;
 }
 
-void lbft_destroy(lbft_sim* s) { free_all(s); }
+void lbft_destroy(lbft_sim* s) { delete s; }
 
 }  // extern "C"

@@ -52,17 +52,27 @@ def test_rerun_is_deterministic_and_reseeding_changes_results(oracle):
 
 
 def test_device_buffer_view_matches_host_results():
+    """Every id of lbft_device_buffer views the finished run's results: 0 commit counts, 1 last states, 2 counters, 3 status,
+    4 active rounds, and 5 the block of 1, 0 and 4, decoded by ShardedResult as the all-gather's receiver decodes it."""
     import torch
+    from librabft_simulator_b200.distributed import ShardedResult, _DeviceView
     seeds = np.arange(40, 104, dtype=np.uint64)
     sim = make(seeds).create(1000)
     res = sim.run()
-    ptr, nbytes = sim.device_buffer(0)
-    assert nbytes == 64 * 4 * 4
 
-    class Cai:
-        __cuda_array_interface__ = {"shape": (64 * 4,), "typestr": "<i4", "data": (ptr, False), "version": 2}
-    t = torch.as_tensor(Cai(), device="cuda:0").cpu().numpy().astype(np.uint32).reshape(64, 4)
-    np.testing.assert_array_equal(t, res.commit_counts)
+    def view(which, nbytes_want):
+        ptr, nbytes = sim.device_buffer(which)
+        assert nbytes == nbytes_want, which
+        return torch.as_tensor(_DeviceView(ptr, (nbytes,), "|u1"), device="cuda:0").cpu().numpy()
+    np.testing.assert_array_equal(view(0, 64 * 4 * 4).view(np.uint32).reshape(64, 4), res.commit_counts)
+    np.testing.assert_array_equal(view(1, 64 * 4 * 8).view(np.uint64).reshape(64, 4), res.last_committed_states)
+    np.testing.assert_array_equal(view(2, 64 * 12 * 4).view(np.uint32).reshape(64, 12), res.counters)
+    np.testing.assert_array_equal(view(3, 64 * 4).view(np.uint32), res.status)
+    np.testing.assert_array_equal(view(4, 64 * 4).view(np.uint32), res.active_rounds)
+    block = ShardedResult(None, view(5, 64 * 4 * 12 + 64 * 4), 64, 4, 0, 64)
+    np.testing.assert_array_equal(block.commit_counts, res.commit_counts)
+    np.testing.assert_array_equal(block.last_committed_states, res.last_committed_states)
+    np.testing.assert_array_equal(block.active_rounds, res.active_rounds)
     sim.close()
 
 
