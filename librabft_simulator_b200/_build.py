@@ -3,8 +3,9 @@
 * ``csrc/liblbft_b200.so`` — the product: sm_90a (H100) CUDA kernels + the C ABI of ``include/lbft.h``.
 * ``oracle/liblbft_oracle.so``, ``tests/hostcore/libhostcore.so``, ``tests/hostcore/libhostcore_sweep.so``,
   ``tests/hostcore/libhostcore_ct.so``, ``tests/hostcore/libhostcore_latency.so``, ``tests/hostcore/libhostcore_fault.so``, ``tests/hostcore/libhostcore_rights.so``,
-  ``tests/hostcore/libhostcore_block_latency.so`` and ``tests/hostcore/libhostcore_lane_block.so`` — test infrastructure only; so is ``tests/gpuprobe/libblock_threshold_probe.so``,
-  a CUDA probe of one device function.
+  ``tests/hostcore/libhostcore_block_latency.so``, ``tests/hostcore/libhostcore_lane_block.so`` and ``tests/hostcore/libhostcore_sampler.so`` — test
+  infrastructure only; so are ``tests/gpuprobe/libblock_threshold_probe.so`` and ``tests/gpuprobe/libsampler_probe.so``, CUDA probes of device
+  functions.
 All artefacts are built in-tree and git-ignored.
 """
 import os
@@ -25,8 +26,10 @@ FAULT_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_fault.so")
 RIGHTS_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_rights.so")
 BLOCK_LATENCY_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_block_latency.so")
 LANE_BLOCK_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_lane_block.so")
+SAMPLER_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_sampler.so")
 GPUPROBE_DIR = os.path.join(ROOT, "tests", "gpuprobe")
 BLOCK_THRESHOLD_PROBE_PATH = os.path.join(GPUPROBE_DIR, "libblock_threshold_probe.so")
+SAMPLER_PROBE_PATH = os.path.join(GPUPROBE_DIR, "libsampler_probe.so")
 
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
@@ -220,6 +223,32 @@ def build_block_threshold_probe(force=False):
     return BLOCK_THRESHOLD_PROBE_PATH
 
 
+def _sampler_sources(main):
+    return [main, os.path.join(GPUPROBE_DIR, "sampler_ops.cuh"), os.path.join(ROOT, "include", "lbft.h")] + [
+        os.path.join(CSRC, f) for f in PRODUCT_HEADERS]
+
+
+def build_sampler_probe(force=False):
+    """The device sampler (sim_core.cuh Core's RNG, range draws, ziggurat and delay lookup) on records with explicit states
+    (tests/gpuprobe/sampler_probe.cu), with the product's nvcc flags: test infrastructure, never linked into the product
+    library."""
+    srcs = _sampler_sources(os.path.join(GPUPROBE_DIR, "sampler_probe.cu"))
+    if not force and _newer(SAMPLER_PROBE_PATH, srcs):
+        return SAMPLER_PROBE_PATH
+    _run([nvcc_path()] + NVCC_FLAGS + ["-shared", "-o", SAMPLER_PROBE_PATH, "sampler_probe.cu"], GPUPROBE_DIR)
+    return SAMPLER_PROBE_PATH
+
+
+def build_sampler_hostcore(force=False):
+    """The host-compiled twin of the sampler probe (tests/hostcore/sampler_hostcore.cpp): test infrastructure."""
+    srcs = _sampler_sources(os.path.join(HOSTCORE_DIR, "sampler_hostcore.cpp"))
+    if not force and _newer(SAMPLER_HOSTCORE_PATH, srcs):
+        return SAMPLER_HOSTCORE_PATH
+    _run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-DLBFT_CHECK_C1",
+          "-o", SAMPLER_HOSTCORE_PATH, "sampler_hostcore.cpp"], HOSTCORE_DIR)
+    return SAMPLER_HOSTCORE_PATH
+
+
 def build_rights_hostcore(force=False):
     """The SW and SW + CT cores of rights sweeps over the product's host setup and set table (tests/hostcore/rights_hostcore.cpp,
     which compiles fault_hostcore.cpp and ct_hostcore.cpp into itself): test infrastructure."""
@@ -236,4 +265,5 @@ def build_rights_hostcore(force=False):
 def build_all(force=False):
     return (build_product(force), build_oracle(force), build_hostcore(force), build_sweep_hostcore(force), build_ct_hostcore(force),
             build_latency_hostcore(force), build_fault_hostcore(force), build_block_latency_hostcore(force),
-            build_lane_block_hostcore(force), build_block_threshold_probe(force), build_rights_hostcore(force))
+            build_lane_block_hostcore(force), build_block_threshold_probe(force), build_rights_hostcore(force),
+            build_sampler_probe(force), build_sampler_hostcore(force))

@@ -595,7 +595,9 @@ struct HostSetup {
       double v = std::exp(mu + sigma * z);
       return v >= 9.0e18 ? INT64_MAX : (int64_t)v;
     };
-    const double ZMAX = 14.0;  // |z| <= R + 52*ln(2)/R ~ 13.52 for the 256-layer ziggurat with 52-bit uniforms
+    // |z| <= 12.2254 for the 256-layer ziggurat: the tail returns R - ln(a)/R only once -2 ln(b) >= (ln(a)/R)^2, and
+    // -2 ln(b) <= 106 ln(2) for an Open01 b >= 2^-53 (tests/rng_support.py largest_deviate)
+    const double ZMAX = 14.0;
     int64_t kmax = D(ZMAX);
     if (kmax < 1 || kmax > 4096) return;  // too wide: keep the exp() path
     auto key = [](double d) { int64_t b; memcpy(&b, &d, 8); return b < 0 ? INT64_MIN - b : b; };  // monotone map

@@ -41,6 +41,17 @@ struct LaunchShape {
 // 32-entry pitch); the state layout interleaves TILE instances.
 // The records behind each set of a sweep's table (sim_core.cuh sweep_set_at): bit 0 faults, bit 1 rights.
 __host__ __device__ __forceinline__ uint32_t sweep_records(const SweepParams& S) { return (S.faults ? 1u : 0u) | (S.rights ? 2u : 0u); }
+// Where a thread kernel's instances read the delay thresholds (Core::thr) from: the block's shared-memory copy `s_thr`, filled
+// here by the block's threads, when the launch has a table of at most kThrSmem entries (returns true); the table in global
+// memory otherwise, and always on a sweep (SW: the instances of one warp may belong to different sets, Core::bind_set).  The
+// caller publishes the copy with a __syncthreads before the first read.
+template <bool SW>
+__device__ __forceinline__ bool place_delay_thresholds(const Params& P, double* s_thr) {
+  const bool thr_fits = !SW && P.delay_kmax != 0 && P.delay_kmax + 2 <= kThrSmem;
+  if (thr_fits)
+    for (uint32_t i = threadIdx.x; i < P.delay_kmax + 2; i += blockDim.x) s_thr[i] = P.delay_thr[i];
+  return thr_fits;
+}
 // The body of both thread kernels (lbft_event_loop_kernel, lbft_sweep_event_loop_kernel), given the kernel's shared memory.
 // SW (sweep handles): the instance's parameter set supplies the delay model and NodeConfig, on a fault sweep (`records` bit 0:
 // `sets` heads a SweepSetFaults table) the silent nodes and partition plan, and on a rights sweep (bit 1: a SweepSetRights table)
@@ -56,9 +67,7 @@ __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, d
     s_zx[i] = P.zig_x[i];
     s_zf[i] = P.zig_f[i];
   }
-  const bool thr_fits = !SW && P.delay_kmax != 0 && P.delay_kmax + 2 <= kThrSmem;
-  if (thr_fits)
-    for (uint32_t i = threadIdx.x; i < P.delay_kmax + 2; i += blockDim.x) s_thr[i] = P.delay_thr[i];
+  const bool thr_fits = place_delay_thresholds<SW>(P, s_thr);
   __syncthreads();
   const uint32_t gthread = blockIdx.x * blockDim.x + threadIdx.x;
   const uint32_t tile = gthread >> 5, lane = gthread & 31;

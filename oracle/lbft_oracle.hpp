@@ -241,7 +241,10 @@ struct RandomDelay {
   }
   int64_t sample(Xoshiro256StarStar& rng) const {
     if (kind == 1) return lo + (int64_t)gen_range_u64(rng, (uint64_t)(hi - lo + 1));
-    double n = standard_normal(rng);
+    return lognormal_of(standard_normal(rng));
+  }
+  // The LogNormal delay of the standard normal deviate n.
+  int64_t lognormal_of(double n) const {
     double v = std::exp(mu + sigma * n);  // Normal: mean + std_dev * n; LogNormal: exp
     return (int64_t)v;                    // simulator.rs:117 `v as i64`
   }

@@ -271,6 +271,67 @@ void lbfo_round_durations(int64_t delta, double gamma, double lambda, int64_t* d
   }
 }
 
+// One call of the sampler from an explicit Xoshiro256** state (tests/rng_support.py REC; the device's side of it is the sampler
+// probe's record): s in / out, arg the seed, n or the bits of z / x, result the integer result or the bits of a double.
+struct SamplerRec {
+  uint64_t s[4];
+  uint64_t arg, result;
+  uint32_t op, set, draws, status;
+};
+static_assert(sizeof(SamplerRec) == 64, "tests/rng_support.py REC");
+static uint64_t f64_bits(double d) {
+  uint64_t b;
+  memcpy(&b, &d, 8);
+  return b;
+}
+
+// Runs recs[0..n) through the oracle's Xoshiro256StarStar, gen_range_u32 / u64, standard_normal and RandomDelay of `c`'s delay
+// model, or of sets[rec.set]'s when sets is not NULL.  Ops: 0 seed_from_u64(arg), 1 next_u64, 2 gen_range_u32(arg),
+// 3 gen_range_u64(arg), 4 standard_normal, 5 the LogNormal delay of z = arg, 6 RandomDelay::sample, 7 exp(arg), 8 log(arg)
+// (the host libm).  status is always 0.  0, or -1 (lbfo_last_error).
+int lbfo_sampler(const lbft_config* c, const lbft_param_set* sets, uint32_t num_sets, SamplerRec* recs, size_t n) {
+  std::vector<RandomDelay> models;
+  for (uint32_t s = 0; s < (sets ? num_sets : 1u); s++) {
+    lbft_config cs = *c;
+    if (sets) {
+      cs.delay_kind = sets[s].delay_kind;
+      cs.delay_mean = sets[s].delay_mean;
+      cs.delay_variance = sets[s].delay_variance;
+      cs.delay_lo = sets[s].delay_lo;
+      cs.delay_hi = sets[s].delay_hi;
+    }
+    SimConfig sc;
+    if (!make_cfg(&cs, sc, g_err)) return -1;
+    models.push_back(sc.delay);
+  }
+  for (size_t i = 0; i < n; i++) {
+    SamplerRec& r = recs[i];
+    if (r.set >= models.size() || r.op > 8) { g_err = "record " + std::to_string(i) + ": set or op out of range"; return -1; }
+    const RandomDelay& d = models[r.set];
+    Xoshiro256StarStar rng;
+    memcpy(rng.s, r.s, sizeof r.s);
+    double x;
+    memcpy(&x, &r.arg, 8);
+    uint64_t v = 0;
+    switch (r.op) {
+      case 0: rng = Xoshiro256StarStar::seed_from_u64(r.arg); break;
+      case 1: v = rng.next_u64(); break;
+      case 2: v = gen_range_u32(rng, (uint32_t)r.arg); break;
+      case 3: v = gen_range_u64(rng, r.arg); break;
+      case 4: v = f64_bits(standard_normal(rng)); break;
+      case 5: v = (uint64_t)d.lognormal_of(x); break;
+      case 6: v = (uint64_t)d.sample(rng); break;
+      case 7: v = f64_bits(std::exp(x)); break;
+      case 8: v = f64_bits(std::log(x)); break;
+    }
+    memcpy(r.s, rng.s, sizeof r.s);
+    r.result = v;
+    r.draws = (uint32_t)rng.draws;
+    r.status = 0;
+  }
+  return 0;
+}
+
 int lbfo_selftest(char* buf, size_t cap);  // oracle_selftest.cpp
 
 }  // extern "C"
