@@ -206,6 +206,23 @@ int lbft_create_sweep_rights(const lbft_config* config, const lbft_param_set* se
                              const uint64_t* voting_rights, uint32_t num_sets, const uint32_t* set_of_instance,
                              lbft_sim** out_sim);
 
+/* A committee sweep: lbft_create_sweep_rights with the committee size per parameter set as well.  config->num_nodes is the
+ * layout's committee, and the stride of every per-node output; set s runs committee_sizes[s] (1..config->num_nodes) nodes.
+ * voting_rights[s * num_nodes + n] is node n's voting right in set s, 0 for n >= committee_sizes[s]; voting_rights may be NULL:
+ * then each node of a set's committee holds 1.  For its nodes 0..n_s-1 (n_s = committee_sizes[set_of_instance[i]]) every output
+ * of instance i (with the exceptions of lbft_create_sweep_faults) is what lbft_create + lbft_run give it with num_nodes = n_s,
+ * sets[s], faults[s] (or the shared faults) and row s of voting_rights truncated to n_s substituted into `config`.  Its other
+ * nodes are absent: commit count, last committed round and state key 0, lbft_commit_logs length 0 and lbft_commit_log 0 rows,
+ * lbft_commit_times entries -1.  The layout and kernel are what lbft_create_sweep_rights picks for the same call.  Refused
+ * (LBFT_ERR_INVALID, before any device work; the error names the set): whatever lbft_create_sweep_rights refuses (but a NULL
+ * voting_rights), NULL committee_sizes, a size of 0 or above num_nodes, a row with a non-zero entry at or past its set's size,
+ * a silent node (a set's silent_mask bit, or with faults NULL a config->silent entry) at or past a set's size, and a set whose
+ * substituted configuration lbft_create refuses.  lbft_block_latency_stats(_groups) weigh each group with its set's rights,
+ * so "all" and "quorum" are per committee. */
+int lbft_create_sweep_committees(const lbft_config* config, const lbft_param_set* sets, const lbft_fault_set* faults,
+                                 const uint64_t* voting_rights, const uint32_t* committee_sizes, uint32_t num_sets,
+                                 const uint32_t* set_of_instance, lbft_sim** out_sim);
+
 /* Simulator::new for every instance followed by loop_until(max_clock) (simulator.rs:200-250,
  * 380-475): copies the seeds host->device, runs the event-loop kernel to completion, copies the
  * per-node summaries (commit counts, last-committed-state keys, counters, status) device->host.

@@ -9,6 +9,7 @@
 // Pure C++ (no CUDA) so the CPU debugging harness in tests/hostcore can share it.  Written
 // independently of oracle/ (the oracle is the checker, not a dependency).
 #pragma once
+#include <algorithm>
 #include <cmath>
 #include <cstddef>
 #include <cstdint>
@@ -369,6 +370,7 @@ struct HostSetup {
   std::vector<uint32_t> set_of;   // sweep handles: [num_instances] the set of each instance
   std::vector<SweepFaults> faults;  // fault and rights sweeps: one record per parameter set (build_sweep_faults / _rights); empty otherwise
   std::vector<SweepRights> rights;  // rights sweeps: one record per parameter set (build_sweep_rights); empty otherwise
+  bool committees = false;          // a committee sweep (build_sweep_committees): each set's fault record carries its committee size
   std::string error;
   KernelSel sel{};
 
@@ -399,8 +401,13 @@ struct HostSetup {
   // record, with one leader table per distinct row of `vr` appended to `leader` (set 0's first, where a plain handle has its
   // own); `faults` gets each set's fault record, the configuration's shared faults when `fs` is null; and weights, Params'
   // quorum and c_weights are set 0's.
+  //
+  // A committee sweep (lbft_create_sweep_committees, `sizes` not null: [num_sets], with `vr`): a rights sweep whose set s runs a
+  // committee of sizes[s] <= num_nodes nodes, validated as a plain configuration of that many nodes.  c.num_nodes stays the
+  // layout's committee, so layout and kernel are the rights sweep's; each row of `vr` is 0 past its set's committee, and each
+  // set's fault record carries the size.
   bool build_sweep(const lbft_config& c, const lbft_param_set* ps, uint32_t num_sets, const uint32_t* set_of_instance,
-                   const lbft_fault_set* fs = nullptr, const uint64_t* vr = nullptr) {
+                   const lbft_fault_set* fs = nullptr, const uint64_t* vr = nullptr, const uint32_t* sizes = nullptr) {
     if (c.struct_size != sizeof(lbft_config)) return fail("lbft_config.struct_size does not match this library (ABI mismatch)");
     if (!ps || !set_of_instance) return fail("sets and set_of_instance must not be NULL");
     if (num_sets == 0 || num_sets > c.num_instances || num_sets > 65536u) return fail("num_sets must be in 1..min(num_instances, 65536)");
@@ -410,19 +417,27 @@ struct HostSetup {
     if (fs && (c.silent || c.partition_windows || c.partition_max_len))
       return fail("a fault sweep takes its silent nodes and partitions per set only: lbft_config.silent must be NULL and "
                   "partition_windows / partition_max_len 0");
-    if (vr && c.voting_rights)
+    if ((vr || sizes) && c.voting_rights)
       return fail("a rights sweep takes its voting rights per set only: lbft_config.voting_rights must be NULL");
     uint32_t fastest = 0, windows = 0;
     for (uint32_t s = 0; s < num_sets; s++) {
       uint8_t silent[64];
       lbft_config cs = fs ? with_faults(with_set(c, ps[s]), fs[s], silent) : with_set(c, ps[s]);
       if (vr) cs.voting_rights = vr + (size_t)s * c.num_nodes;
-      const char* e = config_error(cs);
-      if (!e && fs && c.num_nodes < 64 && (fs[s].silent_mask >> c.num_nodes)) e = "silent_mask has a bit at or above num_nodes";
+      const char* e = sizes ? committee_error(c, cs, sizes[s]) : nullptr;
+      if (!e && sizes) cs.num_nodes = sizes[s];
+      if (!e) e = config_error(cs);
+      if (!e && fs && cs.num_nodes < 64 && (fs[s].silent_mask >> cs.num_nodes)) e = "silent_mask has a bit at or above num_nodes";
       if (e || ps[s].reserved)
         return fail(("parameter set " + std::to_string(s) + ": " + (ps[s].reserved ? "reserved must be 0" : e)).c_str());
       if (mean_delay(cs) < mean_delay(with_set(c, ps[fastest]))) fastest = s;
       if (fs && fs[s].partition_windows > windows) windows = fs[s].partition_windows;
+    }
+    std::vector<uint64_t> ones;  // a committee sweep without rights: 1 for each node of a set's committee (validated above)
+    if (sizes && !vr) {
+      ones.assign((size_t)num_sets * c.num_nodes, 0);
+      for (uint32_t s = 0; s < num_sets; s++) std::fill_n(ones.begin() + (size_t)s * c.num_nodes, sizes[s], 1);
+      vr = ones.data();
     }
     lbft_config cf = with_set(c, ps[fastest]);
     if (fs) cf.partition_windows = windows;
@@ -439,13 +454,16 @@ struct HostSetup {
     if (fs) {
       faults.resize(num_sets);
       for (uint32_t s = 0; s < num_sets; s++) {
-        faults[s] = SweepFaults{fs[s].silent_mask, fs[s].partition_windows, fs[s].partition_max_len};
+        faults[s] = SweepFaults{fs[s].silent_mask, (uint16_t)fs[s].partition_windows, 0, fs[s].partition_max_len};
         params.silent_mask |= fs[s].silent_mask;  // the union: the kernels' launch-uniform "any silent node" test
       }
     } else if (vr) {
-      faults.assign(num_sets, SweepFaults{params.silent_mask, params.L.part_windows, params.part_max_len});
+      faults.assign(num_sets, SweepFaults{params.silent_mask, (uint16_t)params.L.part_windows, 0, params.part_max_len});
     }
+    if (sizes)
+      for (uint32_t s = 0; s < num_sets; s++) faults[s].num_nodes = (uint16_t)sizes[s];
     if (vr) add_rights(vr, num_sets);
+    committees = sizes != nullptr;
     sel = select_kernel(cf, tile, params, true);
     return true;
   }
@@ -464,8 +482,17 @@ struct HostSetup {
     return build_sweep(c, ps, num_sets, set_of_instance, fs, vr);
   }
 
-  // Which records follow each set in the sweep's device table (sim_core.cuh sweep_set_at): bit 0 faults, bit 1 rights.
-  uint32_t records() const { return (faults.empty() ? 0u : 1u) | (rights.empty() ? 0u : 2u); }
+  // A committee sweep (lbft_create_sweep_committees): build_sweep_rights with each set's committee size, its voting rights
+  // (row s of `vr`, or 1 for each of its nodes when `vr` is null) and its faults when `fs` is not null.
+  bool build_sweep_committees(const lbft_config& c, const lbft_param_set* ps, const lbft_fault_set* fs, const uint64_t* vr,
+                              const uint32_t* sizes, uint32_t num_sets, const uint32_t* set_of_instance) {
+    if (!sizes) return fail("committee_sizes must not be NULL");
+    return build_sweep(c, ps, num_sets, set_of_instance, fs, vr, sizes);
+  }
+
+  // Which records follow each set in the sweep's device table (sim_core.cuh sweep_set_at): bit 0 faults, bit 1 rights, and bit
+  // 2 on a committee sweep, whose fault records carry the committee sizes (the entries are those of a rights sweep).
+  uint32_t records() const { return (faults.empty() ? 0u : 1u) | (rights.empty() ? 0u : 2u) | (committees ? 4u : 0u); }
 
   // A sweep's device table of parameter sets, the bytes the runtime uploads: `sets`, each followed by its fault record and then
   // its rights record where records() has them (SweepSet, SweepSetFaults or SweepSetRights entries).
@@ -527,7 +554,8 @@ struct HostSetup {
   }
 
   // A rights sweep's records (`vr`: [num_sets][num_nodes], checked by config_error): per set its weights and quorum, and one
-  // leader table per distinct row.  Set 0's table is the one build_shared made.
+  // leader table per distinct row.  Set 0's table is the one build_shared made.  A committee sweep's rows are 0 past each set's
+  // committee, which pick_author's scan never reaches: each table is the set's plain committee's.
   void add_rights(const uint64_t* vr, uint32_t num_sets) {
     const uint32_t N = params.L.num_nodes;
     std::map<std::vector<uint32_t>, uint32_t> table_of;
@@ -643,6 +671,18 @@ struct HostSetup {
       zig_f[i] = lit(f(xs[i]));
     }
     params.zig_r = lit(R);
+  }
+
+  // A committee sweep's checks on set s beyond those of a plain configuration of its size n (`cs`: the set's configuration with
+  // the layout's num_nodes): null when valid.
+  static const char* committee_error(const lbft_config& c, const lbft_config& cs, uint32_t n) {
+    if (c.num_nodes > 64) return "num_nodes must be in 1..64";
+    if (n < 1 || n > c.num_nodes) return "committee size must be in 1..lbft_config.num_nodes (the layout's committee)";
+    for (uint32_t k = n; k < c.num_nodes; k++) {
+      if (cs.voting_rights && cs.voting_rights[k]) return "voting_rights has a non-zero entry at or past the set's committee size";
+      if (cs.silent && cs.silent[k]) return "a silent node is at or past the set's committee size";
+    }
+    return nullptr;
   }
 
   bool fail(const char* msg) {

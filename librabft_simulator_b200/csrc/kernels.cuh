@@ -4,7 +4,8 @@
 //   lbft_wide_kernel<NMAX, QMODE>                          one WARP per instance (small batches, large committees)
 //   lbft_sweep_event_loop_kernel / lbft_sweep_wide_kernel  the same bodies for sweep handles (lbft_create_sweep: per-instance
 //                                                          delay model and NodeConfig; lbft_create_sweep_faults: and faults;
-//                                                          lbft_create_sweep_rights: and voting rights)
+//                                                          lbft_create_sweep_rights: and voting rights;
+//                                                          lbft_create_sweep_committees: and committee size)
 //   lbft_ct_*_kernel                                       the same bodies with the commit-time stores (LBFT_FLAG_COMMIT_TIMES),
 //                                                          a twin of every one-shot single-epoch plain and sweep kernel
 //
@@ -39,8 +40,6 @@ struct LaunchShape {
 // each other's code paths, so a warp of 8 instances finishes far sooner than a warp of 32, and four times as many warps hide
 // each other's latency.  Plain kernels over the calendar queue and the shared-memory queue (whose columns keep their
 // 32-entry pitch); the state layout interleaves TILE instances.
-// The records behind each set of a sweep's table (sim_core.cuh sweep_set_at): bit 0 faults, bit 1 rights.
-__host__ __device__ __forceinline__ uint32_t sweep_records(const SweepParams& S) { return (S.faults ? 1u : 0u) | (S.rights ? 2u : 0u); }
 // Where a thread kernel's instances read the delay thresholds (Core::thr) from: the block's shared-memory copy `s_thr`, filled
 // here by the block's threads, when the launch has a table of at most kThrSmem entries (returns true); the table in global
 // memory otherwise, and always on a sweep (SW: the instances of one warp may belong to different sets, Core::bind_set).  The
@@ -55,8 +54,8 @@ __device__ __forceinline__ bool place_delay_thresholds(const Params& P, double* 
 // The body of both thread kernels (lbft_event_loop_kernel, lbft_sweep_event_loop_kernel), given the kernel's shared memory.
 // SW (sweep handles): the instance's parameter set supplies the delay model and NodeConfig, on a fault sweep (`records` bit 0:
 // `sets` heads a SweepSetFaults table) the silent nodes and partition plan, and on a rights sweep (bit 1: a SweepSetRights table)
-// the voting rights, quorum and leaders; its thresholds are read through L1 from the concatenated table, as the instances of one
-// warp may belong to different sets.
+// the voting rights, quorum and leaders, and on a committee sweep (bit 2, a rights sweep too) the committee size; its thresholds
+// are read through L1 from the concatenated table, as the instances of one warp may belong to different sets.
 // CT: the commit-time stores (sim_core.cuh Core CT) into `times`, [num_instances][N + 1][round_cap].
 template <int NMAX, int QMODE, int FX, bool REC, bool RES, bool EP, bool TDS, int TILE, bool SW, bool CT = false>
 __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, double* s_zf, double* s_thr, uint32_t* s_queue,
@@ -95,6 +94,7 @@ __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, d
     core.bind_set(sweep_set_at(sets, set_of[inst], records));
     core.bind_faults(records & 1);
     core.bind_rights(records & 2);
+    core.bind_committee(records & 4);
   }
   if (RES && (P.run_flags & 1u)) core.restore_regs();  // a later lbft_run_until: continue where the last launch stopped
   else core.init(P.seeds[inst]);
@@ -174,6 +174,7 @@ __device__ __forceinline__ void wide_body(const Params& P, uint32_t* s_wide, con
     core.bind_set(sweep_set_at(sets, set_of[inst], records));
     core.bind_faults(records & 1);
     core.bind_rights(records & 2);
+    core.bind_committee(records & 4);
   }
   core.init(P.seeds[inst]);
   core.run();

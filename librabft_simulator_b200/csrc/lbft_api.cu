@@ -293,6 +293,14 @@ int lbft_create_sweep_rights(const lbft_config* config, const lbft_param_set* se
                        [&](HostSetup& hs) { return hs.build_sweep_rights(*config, sets, faults, voting_rights, num_sets, set_of_instance); });
 }
 
+int lbft_create_sweep_committees(const lbft_config* config, const lbft_param_set* sets, const lbft_fault_set* faults,
+                                 const uint64_t* voting_rights, const uint32_t* committee_sizes, uint32_t num_sets,
+                                 const uint32_t* set_of_instance, lbft_sim** out_sim) {
+  return create_handle(config, out_sim, [&](HostSetup& hs) {
+    return hs.build_sweep_committees(*config, sets, faults, voting_rights, committee_sizes, num_sets, set_of_instance);
+  });
+}
+
 }  // extern "C"
 
 // The device half of the lbft_create* entry points, once the host setup `s->hs` is built.  On failure the partial handle is
@@ -491,7 +499,7 @@ static int enqueue_kernel(lbft_sim* s) {
   CUDA_TRY(cudaEventRecord(s->ev[2], s->stream));
   const KernelSel& k = s->hs.sel;
   const uint32_t records = s->hs.records();
-  const SweepParams sp{s->P, s->set_of, reinterpret_cast<const SweepSet*>(s->sets), records & 1u, (records >> 1) & 1u};
+  const SweepParams sp{s->P, s->set_of, reinterpret_cast<const SweepSet*>(s->sets), records & 1u, (records >> 1) & 3u};
   const CtParams<Params> cp{s->P, s->times.at<int32_t>()};
   const CtParams<SweepParams> csp{sp, s->times.at<int32_t>()};
   cudaError_t e = k.ct ? (k.sweep ? (k.wide ? launch_ct_sweep_wide(k, csp, s->stream) : launch_ct_sweep_thread(k, csp, s->stream))

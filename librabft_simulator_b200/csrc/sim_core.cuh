@@ -345,11 +345,26 @@ LBFT_HD uint32_t leader_off_behind(const SweepSet* set) {
   return reinterpret_cast<const SweepSetRights*>(set)->rights.leader_off;
 #endif
 }
+// The committee size of a committee sweep's set (Core::nodes), which its fault record carries.
+static_assert(offsetof(SweepSetFaults, faults) + offsetof(SweepFaults, num_nodes) == 74, "the immediate below");
+LBFT_HD uint32_t nodes_behind(const SweepSet* set) {
+#if defined(__CUDA_ARCH__)
+  uint16_t v;
+  asm volatile("ld.global.nc.u16 %0, [%1+74];" : "=h"(v) : "l"(set));
+  return v;
+#else
+  return reinterpret_cast<const SweepSetFaults*>(set)->faults.num_nodes;
+#endif
+}
 
 static_assert(offsetof(SweepParams, P) == 0, "Core::sweep_records: a sweep kernel's Params heads its SweepParams");
 
+// The records behind each set of a sweep's table (sweep_set_at): bit 0 faults, bit 1 rights, bit 2 the committee size (a
+// committee sweep's SweepParams::rights has bits 0 and 1 set: its table is a rights sweep's).
+LBFT_HD uint32_t sweep_records(const SweepParams& S) { return (S.faults ? 1u : 0u) | (S.rights ? 2u : 0u) | ((S.rights & 2u) << 1); }
+
 // Set s of a sweep's device table, whose entries are SweepSet, SweepSetFaults or SweepSetRights by `records` (bit 0: a fault
-// record follows each set, bit 1: a rights record follows that).
+// record follows each set, bit 1: a rights record follows that; bit 2 does not change the entry).
 LBFT_HD const SweepSet* sweep_set_at(const SweepSet* sets, uint32_t s, uint32_t records) {
   const size_t pitch = (records & 2) ? sizeof(SweepSetRights) : ((records & 1) ? sizeof(SweepSetFaults) : sizeof(SweepSet));
   return reinterpret_cast<const SweepSet*>(reinterpret_cast<const char*>(sets) + pitch * s);
@@ -693,7 +708,8 @@ struct Core {
   const double* thr;  // delay thresholds (shared-memory copy on the device when it fits; SW: the instance's set's, bind_set)
   const SweepSet* sw = nullptr;  // SW: the instance's parameter set
   uint32_t records = 0;          // SW, host: the records behind `sw` (sweep_set_at): bit 0 faults (bind_faults), bit 1 rights
-                                 // (bind_rights); the device reads them from the launch's parameter block instead (sweep_records)
+                                 // (bind_rights), bit 2 the committee size (bind_committee); the device reads them from the
+                                 // launch's parameter block instead (sweep_records)
   using Queue = QueueFor<QMODE, Mem, G, KS>;
   Queue q;                 // given its shared memory by the constructor (QMODE 2: sk / sd, or the host harness's stand-in) and init (km)
   uint32_t* km = nullptr;  // KS: the calendar's occupancy words in shared memory, a column per lane, set by the kernel
@@ -748,8 +764,7 @@ struct Core {
   // where the sweep kernels sit at their 128-register bound.  (The host harness binds a bare Params and sets `records`.)
   LBFT_HD uint32_t sweep_records() const {
 #if defined(__CUDA_ARCH__)
-    const SweepParams& S = *reinterpret_cast<const SweepParams*>(&P);
-    return (S.faults ? 1u : 0u) | (S.rights ? 2u : 0u);
+    return lbft::sweep_records(*reinterpret_cast<const SweepParams*>(&P));
 #else
     return records;
 #endif
@@ -797,7 +812,15 @@ struct Core {
     if constexpr (SW) return (sweep_records() & 2) ? P.leader[leader_off_behind(sw) + r] : P.leader[r];
     else return P.leader[r];
   }
-
+  // The instance's committee: nodes 0..nodes()-1 run, the layout's others (L.num_nodes, which keeps shaping the state, the
+  // masks and every per-node output) stay absent.  The layout's on every handle but a committee sweep (bind_committee), whose
+  // set's fault record carries it.  As with the rights, nothing is held through the loop: it is loaded where the committee is
+  // walked (init's draws, finalize, and the cut of run()'s fan-out lists).
+  LBFT_HD void bind_committee(bool committee_sweep) { records = (records & ~4u) | (committee_sweep ? 4u : 0u); }
+  LBFT_HD uint32_t nodes() const {
+    if constexpr (SW) return (sweep_records() & 4) ? nodes_behind(sw) : L.num_nodes;
+    else return L.num_nodes;
+  }
   // ------------------------------------------------------------------------------------------
   // RNG (rand_xoshiro 0.6.0 / rand 0.8.3 / rand_distr 0.4.0)
   // ------------------------------------------------------------------------------------------
@@ -1782,11 +1805,12 @@ struct Core {
       uint64_t k0 = s0, k1 = s1, k2 = s2, k3 = s3;
       uint32_t kd = draws;
       seed_rng(seed ^ 0xD1B54A32D192ED03ULL, s0, s1, s2, s3);
-      uint64_t nsub = N >= 64 ? 0xfffffffffffffffeULL : ((1ULL << N) - 2);
+      const uint32_t n = nodes();  // (the author masks are drawn over the instance's committee)
+      uint64_t nsub = n >= 64 ? 0xfffffffffffffffeULL : ((1ULL << n) - 2);
       for (uint32_t k = 0; k < part_windows(); k++) {
         int64_t t0 = (int64_t)gen_range_u64((uint64_t)P.max_clock + 1);
         int64_t len = 1 + (int64_t)gen_range_u64(part_max_len() ? part_max_len() : 1);
-        uint64_t mask = N >= 2 ? 1 + gen_range_u64(nsub) : 0;
+        uint64_t mask = n >= 2 ? 1 + gen_range_u64(nsub) : 0;
         m.st(L.part_base + 4 * k, (uint32_t)t0);
         m.st(L.part_base + 4 * k + 1, (uint32_t)(t0 + len));
         m.st(L.part_base + 4 * k + 2, (uint32_t)mask);
@@ -1798,8 +1822,9 @@ struct Core {
       s0 = k0; s1 = k1; s2 = k2; s3 = k3;
       draws = kd;
     }
+    const uint32_t present = nodes();
 #pragma unroll 1
-    for (uint32_t n = 0; n < N; n++) {
+    for (uint32_t n = 0; n < present; n++) {
       int32_t startup = sample_delay() + 1;
       uint32_t b = nbase(n);
       node_st(b, F_STARTUP, (uint32_t)startup);
@@ -1940,6 +1965,15 @@ struct Core {
         } else {
           if (query_pending) list.fill_others(N, receiver);
         }
+        // A committee sweep: the lists above cover the layout's committee, ascending, so the instance's committee's are their first
+        // nodes() - 1 entries (a list of one is addressed to a node of the committee, so it stays; a list cut to none sends
+        // nothing, as an empty one).  One cut here rather than a committee bound at each fill: that bound, live in the loop,
+        // cost the sweep kernels spills.
+        if constexpr (SW)
+          if (sweep_records() & 4) {
+            const uint32_t others = nodes_behind(sw) - 1;
+            if (list.len > others) list.len = others;
+          }
         for (uint32_t i = list.len; i-- > 1;) list.swap(i, gen_range_u32(i + 1));  // SliceRandom::shuffle
         if (list.len == 0) continue;
         HcbrRegs hc;
@@ -2031,7 +2065,13 @@ struct Core {
     const uint32_t N = L.num_nodes;
     const uint32_t scratch = RES ? res_area_base(L, REC) + RES_REG_WORDS : L.heap_time;
     uint32_t max_round = 0;
-    for (uint32_t n = 0; n < N; n++) {
+    const uint32_t present = nodes();
+    for (uint32_t n = present; n < N; n++) {  // a committee sweep's absent nodes: the outputs of a node that never committed
+      P.out_commit_counts[(size_t)inst * N + n] = 0;
+      P.out_lc_round[(size_t)inst * N + n] = 0;
+      P.out_last_state[(size_t)inst * N + n] = 0;
+    }
+    for (uint32_t n = 0; n < present; n++) {
       uint32_t b = nbase(n);
       uint32_t commits = node_ld(b, F_COMMITS), lc = node_ld(b, F_LC_ROUND), pmr = node_ld(b, F_PMR);
       if (pmr > max_round) max_round = pmr;

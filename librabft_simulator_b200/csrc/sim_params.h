@@ -259,9 +259,13 @@ struct Params {
 // The fault model of one parameter set of a fault sweep (lbft_create_sweep_faults): what Params::silent_mask, Layout::part_windows
 // and Params::part_max_len give every instance of a plain handle.  part_windows is at most the layout's (the partition region
 // is sized for the largest count of any set).
+// num_nodes: on a committee sweep (lbft_create_sweep_committees, whose sets all carry fault and rights records) the set's
+// committee, at most the layout's (Layout::num_nodes); 0 on every other sweep.  (16 bits each: part_windows never exceeds
+// 64, and the record keeps its 16 bytes, so no sweep's table grows.)
 struct SweepFaults {
   uint64_t silent_mask;
-  uint32_t part_windows;
+  uint16_t part_windows;
+  uint16_t num_nodes;
   uint32_t part_max_len;
 };
 // One entry of a fault sweep's device table of parameter sets: the set, and its fault record right behind it, so that an
@@ -295,7 +299,8 @@ struct SweepParams {
   const SweepSet* sets;    // [num_sets]; a fault sweep (lbft_create_sweep_faults): the sets of a SweepSetFaults [num_sets] table;
                            // a rights sweep (lbft_create_sweep_rights): of a SweepSetRights [num_sets] table
   uint32_t faults;         // 1: a fault or rights sweep, whose instances take their silent nodes and partition plan from their set's record
-  uint32_t rights;         // 1: a rights sweep, whose instances take their voting rights, quorum and leaders from their set's record
+  uint32_t rights;         // bit 0: a rights sweep, whose instances take their voting rights, quorum and leaders from their set's
+                           // record; bit 1: a committee sweep (a rights sweep too), whose instances take their committee size from it
 };
 
 }  // namespace lbft

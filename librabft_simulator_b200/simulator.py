@@ -592,12 +592,14 @@ class FaultSet:
 @dataclass(frozen=True)
 class ParamSet:
     """One point of a parameter sweep: the network delay and ``NodeConfig`` of the instances assigned to it
-    (main.rs --mean / --variance and --delta / --gamma / --lambda / --target_commit_interval), its fault model, and its
-    voting rights: a tuple of one int per node, or None for 1 per node (``BatchSimulator``'s ``voting_rights``)."""
+    (main.rs --mean / --variance and --delta / --gamma / --lambda / --target_commit_interval), its fault model, its
+    voting rights: a tuple of one int per node of the set, or None for 1 per node (``BatchSimulator``'s ``voting_rights``),
+    and its committee size: None for the simulator's ``num_nodes``."""
     network_delay: RandomDelay = RandomDelay()
     node_config: NodeConfig = NodeConfig()
     faults: FaultSet = FaultSet()
     voting_rights: tuple = None
+    num_nodes: int = None
 
     def __post_init__(self):
         if self.voting_rights is not None:  # (a list or array compares, and hashes, as a tuple)
@@ -617,9 +619,12 @@ class SweepSimulator(BatchSimulator):
     a ``FaultSet`` of its own: then every set has its own (``lbft_create_sweep_faults``) and the shared ``silent`` /
     ``partition_*`` arguments must be left unset.  Likewise the voting rights: when a set carries its own
     (``lbft_create_sweep_rights``), every set has its own (1 per node where left None) and ``voting_rights`` must be left
-    unset.  Every result of instance i is what a ``BatchSimulator`` with that set's delay, node config, faults and voting
-    rights computes for it.  Running, re-seeding (the set assignment stays), streaming and reading
-    results work as on a ``BatchSimulator``."""
+    unset.  And the committee size: when a set has its own (``ParamSet.num_nodes``, ``lbft_create_sweep_committees``),
+    ``num_nodes`` is the size of the layout every instance gets and must be at least every set's; the per-node arrays keep
+    ``num_nodes`` columns, and an instance's nodes past its set's committee read as nodes that never committed (mask them with
+    ``nodes_of_instance()``).  Every result of instance i (of its committee's nodes) is what a ``BatchSimulator`` with that
+    set's delay, node config, faults, voting rights and committee size computes for it.  Running, re-seeding (the set
+    assignment stays), streaming and reading results work as on a ``BatchSimulator``."""
 
     def __init__(self, seeds, num_nodes, param_sets, set_of_instance, **shared):
         super().__init__(seeds, num_nodes, **shared)
@@ -627,6 +632,12 @@ class SweepSimulator(BatchSimulator):
         self.set_of_instance = np.ascontiguousarray(np.asarray(set_of_instance, dtype=np.uint32).reshape(-1))
         if self.set_of_instance.shape[0] != self.num_instances:
             raise ValueError("set_of_instance needs one entry per seed (%d)" % self.num_instances)
+        for s, p in enumerate(self.param_sets):
+            if p.num_nodes is not None and not 1 <= int(p.num_nodes) <= self.num_nodes:
+                raise ValueError("parameter set %d: num_nodes (%r) must be in 1..num_nodes of the simulator (%d), the layout's "
+                                 "committee" % (s, p.num_nodes, self.num_nodes))
+        if self._committees() and self.voting_rights is not None:
+            raise ValueError("a sweep whose sets have their own committee sizes takes voting rights per set only (ParamSet.voting_rights)")
 
     @classmethod
     def grid(cls, seeds_per_point, delays, node_configs, num_nodes=4, faults=None, voting_rights=None, **shared):
@@ -637,19 +648,28 @@ class SweepSimulator(BatchSimulator):
         len(faults) + f, so ``latency_stats().mean().reshape(len(delays), len(node_configs), len(faults))`` is the cube.
         ``voting_rights``, a list of rows of one voting right per node, adds a fastest-varying axis after that (after
         ``node_configs`` when ``faults`` is None): ``block_latency_stats("quorum").mean().reshape(len(delays),
-        len(node_configs), len(faults), len(voting_rights))``."""
+        len(node_configs), len(faults), len(voting_rights))``.  ``num_nodes``, a list of committee sizes instead of one,
+        likewise adds a fastest-varying axis of committees, in a layout of the largest (it cannot be combined with a
+        ``voting_rights`` list, whose rows have a fixed length)."""
         seeds = np.arange(seeds_per_point, dtype=np.uint64) if np.isscalar(seeds_per_point) else \
             np.asarray(seeds_per_point, dtype=np.uint64).reshape(-1)
         sets = [ParamSet(d, n) for d in delays for n in node_configs] if faults is None else \
             [ParamSet(d, n, f) for d in delays for n in node_configs for f in faults]
         if voting_rights is not None:
+            if not np.isscalar(num_nodes):
+                raise ValueError("a grid takes a list of committee sizes (num_nodes) or a list of voting-rights rows, not both")
             sets = [ParamSet(p.network_delay, p.node_config, p.faults, v) for p in sets for v in voting_rights]
+        if not np.isscalar(num_nodes):
+            sizes = [int(n) for n in num_nodes]
+            sets = [ParamSet(p.network_delay, p.node_config, p.faults, None, n) for p in sets for n in sizes]
+            num_nodes = max(sizes)
         k = seeds.shape[0]
         return cls(np.tile(seeds, len(sets)), num_nodes, sets, np.repeat(np.arange(len(sets), dtype=np.uint32), k), **shared)
 
     def create(self, max_clock):
         """``lbft_create_sweep``, or ``lbft_create_sweep_faults`` when some set has faults, or ``lbft_create_sweep_rights``
-        when some set has voting rights: validate every set, build the per-set host tables, allocate device state."""
+        when some set has voting rights, or ``lbft_create_sweep_committees`` when some set has its own committee size:
+        validate every set, build the per-set host tables, allocate device state."""
         per_set = any(p.faults != FaultSet() for p in self.param_sets)
         if per_set and (self.silent is not None or self.partition_windows or self.partition_max_len):
             raise ValueError("a sweep takes silent nodes and partitions either per set (ParamSet.faults) or shared (silent / "
@@ -663,7 +683,12 @@ class SweepSimulator(BatchSimulator):
         sets = (_lib.LbftParamSet * max(1, len(self.param_sets)))(*[p.to_c() for p in self.param_sets])
         so = ctypes.c_void_p(self.set_of_instance.ctypes.data)
         faults = (_lib.LbftFaultSet * len(self.param_sets))(*[p.faults.to_c() for p in self.param_sets]) if per_set else None
-        if rights is not None:
+        if self._committees():
+            sizes = np.ascontiguousarray(self._committee_sizes(), dtype=np.uint32)
+            _lib.check(self._lib.lbft_create_sweep_committees(
+                ctypes.byref(cfg), sets, faults, None if rights is None else ctypes.c_void_p(rights.ctypes.data),
+                ctypes.c_void_p(sizes.ctypes.data), len(self.param_sets), so, ctypes.byref(handle)))
+        elif rights is not None:
             _lib.check(self._lib.lbft_create_sweep_rights(ctypes.byref(cfg), sets, faults, ctypes.c_void_p(rights.ctypes.data),
                                                           len(self.param_sets), so, ctypes.byref(handle)))
         elif per_set:
@@ -673,15 +698,33 @@ class SweepSimulator(BatchSimulator):
         self._handle = handle
         return self
 
+    def _committees(self):
+        """Whether some set has its own committee size (a committee sweep)."""
+        return any(p.num_nodes is not None for p in self.param_sets)
+
+    def _committee_sizes(self):
+        """Each set's committee size."""
+        return np.array([self.num_nodes if p.num_nodes is None else int(p.num_nodes) for p in self.param_sets], dtype=np.int64)
+
     def _rights_table(self):
-        """The [num_sets][num_nodes] voting rights of a rights sweep (1 per node where a set leaves them None), or None when
-        no set carries any."""
+        """The [num_sets][num_nodes] voting rights of a rights or committee sweep (1 per node of its committee where a set
+        leaves them None, 0 past it), or None when no set carries any."""
         if all(p.voting_rights is None for p in self.param_sets):
             return None
-        rows = [(1,) * self.num_nodes if p.voting_rights is None else p.voting_rights for p in self.param_sets]
-        if any(len(r) != self.num_nodes for r in rows):
-            raise ValueError("ParamSet.voting_rights needs one entry per node (%d)" % self.num_nodes)
-        return np.ascontiguousarray(rows, dtype=np.uint64)
+        sizes = self._committee_sizes()
+        rows = np.zeros((len(self.param_sets), self.num_nodes), dtype=np.uint64)
+        for s, p in enumerate(self.param_sets):
+            row = (1,) * int(sizes[s]) if p.voting_rights is None else p.voting_rights
+            if len(row) != sizes[s]:
+                raise ValueError("ParamSet.voting_rights needs one entry per node of the set (%d)" % sizes[s])
+            rows[s, :len(row)] = row
+        return rows
+
+    def nodes_of_instance(self):
+        """The committee size of each instance, as an int64 array [num_instances]: its set's, where the per-node arrays have
+        ``num_nodes`` columns.  ``np.arange(sim.num_nodes) < sim.nodes_of_instance()[:, None]`` masks the nodes an instance
+        has."""
+        return self._committee_sizes()[self.set_of_instance]
 
     def total_voting_rights(self):
         """The sum of the voting rights of the committee; on a sweep whose sets carry their own voting rights, their common
@@ -693,11 +736,13 @@ class SweepSimulator(BatchSimulator):
 
     def group_voting_rights(self):
         """The total voting rights of each parameter set (a group of the latency statistics), as an int64 array: its own
-        row's total on a rights sweep, the shared committee's otherwise."""
+        row's total on a rights sweep, its committee's on a committee sweep, the shared committee's otherwise."""
         rights = self._rights_table()
-        if rights is None:
-            return np.full(len(self.param_sets), super().total_voting_rights(), dtype=np.int64)
-        return rights.sum(axis=1).astype(np.int64)
+        if rights is not None:
+            return rights.sum(axis=1).astype(np.int64)
+        if self._committees():
+            return self._committee_sizes()
+        return np.full(len(self.param_sets), super().total_voting_rights(), dtype=np.int64)
 
 
 def format_round_switches_csv(num_nodes, switches):
