@@ -94,9 +94,11 @@ typedef struct lbft_instance_counters {
   uint32_t scheduled;         /* Simulator.event_count: creation stamps handed out                     */
   uint32_t max_active_round;  /* max over nodes of ActiveRound::active_round() (simulator.rs:86-88)     */
   uint32_t rng_draws;         /* Xoshiro256** next_u64 calls on the instance stream                    */
-  uint32_t max_queue;         /* high-water mark of the device event queue (implementation-specific)   */
+  uint32_t max_queue;         /* high-water mark of the device event queue: the smallest queue_cap     *
+                               * with which the instance completes (the read-out floor aside)         */
   uint32_t scheduled_notify;  /* DataSyncNotifyEvents handed a creation stamp (simulator.rs:348-354)    */
-  uint32_t max_payloads;      /* high-water mark of in-flight notification snapshots (implementation)   */
+  uint32_t max_payloads;      /* high-water mark of in-flight notification snapshots: the smallest     *
+                               * payload_cap with which the instance completes                        */
   uint32_t timers_elided;     /* duplicate timers accounted as cancelled without being queued (impl.)  */
 } lbft_instance_counters;
 
