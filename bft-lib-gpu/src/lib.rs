@@ -166,6 +166,9 @@ pub mod ffi {
         pub fn lbft_create_sweep_committees(config: *const LbftConfig, sets: *const lbft_param_set, faults: *const lbft_fault_set,
                                             voting_rights: *const u64, committee_sizes: *const u32, num_sets: u32,
                                             set_of_instance: *const u32, out_sim: *mut *mut LbftSim) -> c_int;
+        pub fn lbft_create_sweep_links(config: *const LbftConfig, sets: *const lbft_param_set, faults: *const lbft_fault_set,
+                                       voting_rights: *const u64, committee_sizes: *const u32, link_latency: *const u32,
+                                       num_sets: u32, set_of_instance: *const u32, out_sim: *mut *mut LbftSim) -> c_int;
         pub fn lbft_destroy(sim: *mut LbftSim);
         pub fn lbft_set_seeds(sim: *mut LbftSim, seeds: *const u64) -> c_int;
         pub fn lbft_run(sim: *mut LbftSim) -> c_int;

@@ -225,6 +225,23 @@ int lbft_create_sweep_committees(const lbft_config* config, const lbft_param_set
                                  const uint64_t* voting_rights, const uint32_t* committee_sizes, uint32_t num_sets,
                                  const uint32_t* set_of_instance, lbft_sim** out_sim);
 
+/* A links sweep: the most general sweep, with a matrix of link latencies per parameter set as well.  link_latency[(s * N + a)
+ * * N + b] (N = config->num_nodes, the layout's committee) is M_s[a][b], whole milliseconds in 0..65535: every network event
+ * (notification, request, response) an instance of set s schedules from sender a to receiver b (the event's sender and receiver,
+ * the pair its partition test looks at) is due at clock + delay + M_s[a][b], where delay is drawn from the set's delay model
+ * exactly as without links.  The partition test, the silent-receiver elision and the drop past max_clock see that time.  The
+ * startup delay of Simulator::new and the timers get no link term.  faults, voting_rights and committee_sizes may each be NULL;
+ * the rules are those of lbft_create_sweep_faults, lbft_create_sweep_rights and lbft_create_sweep_committees, and where faults
+ * or voting_rights is NULL the configuration's shared value applies to every set.  A set whose matrix is all zero computes what
+ * the same set computes without links, counters included.  The layout and kernel are what the same call without link_latency
+ * picks: the matrices enter no kernel choice.  Sets with equal matrices share one device table of N x N u16 (lbft_memory_info
+ * counts them).  Refused (LBFT_ERR_INVALID, before any device work; the error names the set): whatever the corresponding sweep
+ * refuses, NULL link_latency, an entry above 65535, and a non-zero entry in a row or column at or past the set's committee
+ * size. */
+int lbft_create_sweep_links(const lbft_config* config, const lbft_param_set* sets, const lbft_fault_set* faults,
+                            const uint64_t* voting_rights, const uint32_t* committee_sizes, const uint32_t* link_latency,
+                            uint32_t num_sets, const uint32_t* set_of_instance, lbft_sim** out_sim);
+
 /* Simulator::new for every instance followed by loop_until(max_clock) (simulator.rs:200-250,
  * 380-475): copies the seeds host->device, runs the event-loop kernel to completion, copies the
  * per-node summaries (commit counts, last-committed-state keys, counters, status) device->host.

@@ -3,7 +3,7 @@
 * ``csrc/liblbft_b200.so`` — the product: sm_90a (H100) CUDA kernels + the C ABI of ``include/lbft.h``.
 * ``oracle/liblbft_oracle.so``, ``tests/hostcore/libhostcore.so``, ``tests/hostcore/libhostcore_sweep.so``,
   ``tests/hostcore/libhostcore_ct.so``, ``tests/hostcore/libhostcore_latency.so``, ``tests/hostcore/libhostcore_fault.so``, ``tests/hostcore/libhostcore_rights.so``,
-  ``tests/hostcore/libhostcore_committee.so``,
+  ``tests/hostcore/libhostcore_committee.so``, ``tests/hostcore/libhostcore_link.so``,
   ``tests/hostcore/libhostcore_block_latency.so``, ``tests/hostcore/libhostcore_lane_block.so`` and ``tests/hostcore/libhostcore_sampler.so`` — test
   infrastructure only; so are ``tests/gpuprobe/libblock_threshold_probe.so`` and ``tests/gpuprobe/libsampler_probe.so``, CUDA probes of device
   functions.
@@ -26,6 +26,7 @@ LATENCY_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_latency.so")
 FAULT_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_fault.so")
 RIGHTS_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_rights.so")
 COMMITTEE_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_committee.so")
+LINK_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_link.so")
 BLOCK_LATENCY_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_block_latency.so")
 LANE_BLOCK_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_lane_block.so")
 SAMPLER_HOSTCORE_PATH = os.path.join(HOSTCORE_DIR, "libhostcore_sampler.so")
@@ -278,8 +279,23 @@ def build_committee_hostcore(force=False):
     return COMMITTEE_HOSTCORE_PATH
 
 
+def build_link_hostcore(force=False):
+    """The SW and SW + CT cores of links sweeps over the product's host setup and set table, and the oracle with link latencies
+    (tests/hostcore/link_hostcore.cpp with tests/hostcore/link_oracle.hpp, which compiles committee_hostcore.cpp,
+    rights_hostcore.cpp, fault_hostcore.cpp and ct_hostcore.cpp into itself): test infrastructure."""
+    srcs = [os.path.join(HOSTCORE_DIR, f) for f in ("link_hostcore.cpp", "link_oracle.hpp", "committee_hostcore.cpp", "rights_hostcore.cpp",
+                                                   "fault_hostcore.cpp", "ct_hostcore.cpp")] + [
+        os.path.join(ROOT, "include", "lbft.h")] + [os.path.join(CSRC, f) for f in ("sim_core.cuh", "sim_params.h", "host_setup.hpp")] + [
+        os.path.join(ORACLE_DIR, f) for f in ("oracle_capi.cpp", "lbft_oracle.hpp")]
+    if not force and _newer(LINK_HOSTCORE_PATH, srcs):
+        return LINK_HOSTCORE_PATH
+    _run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-DLBFT_CHECK_C1",
+          "-o", LINK_HOSTCORE_PATH, "link_hostcore.cpp"], HOSTCORE_DIR)
+    return LINK_HOSTCORE_PATH
+
+
 def build_all(force=False):
     return (build_product(force), build_oracle(force), build_hostcore(force), build_sweep_hostcore(force), build_ct_hostcore(force),
             build_latency_hostcore(force), build_fault_hostcore(force), build_block_latency_hostcore(force),
             build_lane_block_hostcore(force), build_block_threshold_probe(force), build_rights_hostcore(force),
-            build_committee_hostcore(force), build_sampler_probe(force), build_sampler_hostcore(force))
+            build_committee_hostcore(force), build_link_hostcore(force), build_sampler_probe(force), build_sampler_hostcore(force))

@@ -371,6 +371,8 @@ struct HostSetup {
   std::vector<SweepFaults> faults;  // fault and rights sweeps: one record per parameter set (build_sweep_faults / _rights); empty otherwise
   std::vector<SweepRights> rights;  // rights sweeps: one record per parameter set (build_sweep_rights); empty otherwise
   bool committees = false;          // a committee sweep (build_sweep_committees): each set's fault record carries its committee size
+  std::vector<uint16_t> links;      // links sweeps: the distinct N x N link-latency matrices of the sets (build_sweep_links)
+  std::vector<uint32_t> link_off;   // links sweeps: one record per parameter set, where its matrix starts in `links`; empty otherwise
   std::string error;
   KernelSel sel{};
 
@@ -406,8 +408,16 @@ struct HostSetup {
   // committee of sizes[s] <= num_nodes nodes, validated as a plain configuration of that many nodes.  c.num_nodes stays the
   // layout's committee, so layout and kernel are the rights sweep's; each row of `vr` is 0 past its set's committee, and each
   // set's fault record carries the size.
+  //
+  // A links sweep (lbft_create_sweep_links, `lk` not null: [num_sets][num_nodes][num_nodes]): a rights sweep (a committee sweep
+  // when `sizes` is not null) whose set s adds lk[s][a][b] to the time of every network event from a to b.  With `vr` null each
+  // set gets the configuration's shared rights (1 per node of its committee when it has none).  Layout and kernel do not depend
+  // on the matrices: the stamp-width and queue-mode tests are sized by the shortest mean delay, which over-estimates the event
+  // rate of a network slowed by its links, so they stay safe (and an overrun still surfaces as LBFT_ERR_CAPACITY).  `links` gets
+  // one matrix per distinct one, `link_off` each set's.
   bool build_sweep(const lbft_config& c, const lbft_param_set* ps, uint32_t num_sets, const uint32_t* set_of_instance,
-                   const lbft_fault_set* fs = nullptr, const uint64_t* vr = nullptr, const uint32_t* sizes = nullptr) {
+                   const lbft_fault_set* fs = nullptr, const uint64_t* vr = nullptr, const uint32_t* sizes = nullptr,
+                   const uint32_t* lk = nullptr) {
     if (c.struct_size != sizeof(lbft_config)) return fail("lbft_config.struct_size does not match this library (ABI mismatch)");
     if (!ps || !set_of_instance) return fail("sets and set_of_instance must not be NULL");
     if (num_sets == 0 || num_sets > c.num_instances || num_sets > 65536u) return fail("num_sets must be in 1..min(num_instances, 65536)");
@@ -428,15 +438,19 @@ struct HostSetup {
       if (!e && sizes) cs.num_nodes = sizes[s];
       if (!e) e = config_error(cs);
       if (!e && fs && cs.num_nodes < 64 && (fs[s].silent_mask >> cs.num_nodes)) e = "silent_mask has a bit at or above num_nodes";
+      if (!e && lk) e = links_error(lk + (size_t)s * c.num_nodes * c.num_nodes, c.num_nodes, cs.num_nodes);
       if (e || ps[s].reserved)
         return fail(("parameter set " + std::to_string(s) + ": " + (ps[s].reserved ? "reserved must be 0" : e)).c_str());
       if (mean_delay(cs) < mean_delay(with_set(c, ps[fastest]))) fastest = s;
       if (fs && fs[s].partition_windows > windows) windows = fs[s].partition_windows;
     }
-    std::vector<uint64_t> ones;  // a committee sweep without rights: 1 for each node of a set's committee (validated above)
-    if (sizes && !vr) {
+    // a committee or links sweep without rights: the shared rights, or 1, for each node of a set's committee (validated above)
+    std::vector<uint64_t> ones;
+    if ((sizes || lk) && !vr) {
       ones.assign((size_t)num_sets * c.num_nodes, 0);
-      for (uint32_t s = 0; s < num_sets; s++) std::fill_n(ones.begin() + (size_t)s * c.num_nodes, sizes[s], 1);
+      for (uint32_t s = 0; s < num_sets; s++)
+        for (uint32_t n = 0; n < (sizes ? sizes[s] : c.num_nodes); n++)
+          ones[(size_t)s * c.num_nodes + n] = c.voting_rights ? c.voting_rights[n] : 1;
       vr = ones.data();
     }
     lbft_config cf = with_set(c, ps[fastest]);
@@ -463,6 +477,7 @@ struct HostSetup {
     if (sizes)
       for (uint32_t s = 0; s < num_sets; s++) faults[s].num_nodes = (uint16_t)sizes[s];
     if (vr) add_rights(vr, num_sets);
+    if (lk) add_links(lk, num_sets);
     committees = sizes != nullptr;
     sel = select_kernel(cf, tile, params, true);
     return true;
@@ -490,22 +505,42 @@ struct HostSetup {
     return build_sweep(c, ps, num_sets, set_of_instance, fs, vr, sizes);
   }
 
-  // Which records follow each set in the sweep's device table (sim_core.cuh sweep_set_at): bit 0 faults, bit 1 rights, and bit
-  // 2 on a committee sweep, whose fault records carry the committee sizes (the entries are those of a rights sweep).
-  uint32_t records() const { return (faults.empty() ? 0u : 1u) | (rights.empty() ? 0u : 2u) | (committees ? 4u : 0u); }
+  // A links sweep (lbft_create_sweep_links): build_sweep with each set's link-latency matrix (lk[s], [num_nodes][num_nodes]),
+  // its voting rights (row s of `vr`, or the shared ones when `vr` is null), its faults when `fs` is not null and its committee
+  // size when `sizes` is not null.
+  bool build_sweep_links(const lbft_config& c, const lbft_param_set* ps, const lbft_fault_set* fs, const uint64_t* vr,
+                         const uint32_t* sizes, const uint32_t* lk, uint32_t num_sets, const uint32_t* set_of_instance) {
+    if (!lk) return fail("link_latency must not be NULL");
+    return build_sweep(c, ps, num_sets, set_of_instance, fs, vr, sizes, lk);
+  }
 
-  // A sweep's device table of parameter sets, the bytes the runtime uploads: `sets`, each followed by its fault record and then
-  // its rights record where records() has them (SweepSet, SweepSetFaults or SweepSetRights entries).
+  // Which records follow each set in the sweep's device table (sim_core.cuh sweep_set_at): bit 0 faults, bit 1 rights, bit 2 on
+  // a committee sweep, whose fault records carry the committee sizes (the entries are those of a rights sweep), and bit 3 the
+  // links records of a links sweep.
+  uint32_t records() const {
+    return (faults.empty() ? 0u : 1u) | (rights.empty() ? 0u : 2u) | (committees ? 4u : 0u) | (link_off.empty() ? 0u : 8u);
+  }
+
+  // A sweep's device table of parameter sets, the bytes the runtime uploads: `sets`, each followed by its fault record, its
+  // rights record and its links record where records() has them (SweepSet, SweepSetFaults, SweepSetRights or SweepSetLinks
+  // entries).
   std::vector<uint64_t> set_table() const {
     const uint32_t rec = records();
-    const size_t pitch = (rec & 2) ? sizeof(SweepSetRights) : ((rec & 1) ? sizeof(SweepSetFaults) : sizeof(SweepSet));
-    static_assert(sizeof(SweepSet) % 8 == 0 && sizeof(SweepSetFaults) % 8 == 0 && sizeof(SweepSetRights) % 8 == 0, "whole words");
+    const size_t pitch = (rec & 8)   ? sizeof(SweepSetLinks)
+                         : (rec & 2) ? sizeof(SweepSetRights)
+                                     : ((rec & 1) ? sizeof(SweepSetFaults) : sizeof(SweepSet));
+    static_assert(sizeof(SweepSet) % 8 == 0 && sizeof(SweepSetFaults) % 8 == 0 && sizeof(SweepSetRights) % 8 == 0 &&
+                      sizeof(SweepSetLinks) % 8 == 0, "whole words");
     std::vector<uint64_t> t(sets.size() * pitch / 8);
     for (size_t k = 0; k < sets.size(); k++) {
       char* e = reinterpret_cast<char*>(t.data()) + k * pitch;
       memcpy(e, &sets[k], sizeof(SweepSet));
       if (rec & 1) memcpy(e + offsetof(SweepSetFaults, faults), &faults[k], sizeof(SweepFaults));
       if (rec & 2) memcpy(e + offsetof(SweepSetRights, rights), &rights[k], sizeof(SweepRights));
+      if (rec & 8) {
+        const SweepLinks l{link_off[k], 0};
+        memcpy(e + offsetof(SweepSetLinks, links), &l, sizeof(SweepLinks));
+      }
     }
     return t;
   }
@@ -571,6 +606,24 @@ struct HostSetup {
       r.quorum = quorum_of(total);
       r.leader_off = it->second;
       for (uint32_t n = 0; n < N; n++) r.weights[n] = row[n];
+    }
+  }
+
+  // A links sweep's records (`lk`: [num_sets][N][N], checked by links_error): one matrix of u16 per distinct one in `links`, and
+  // where each set's starts in `link_off`.
+  void add_links(const uint32_t* lk, uint32_t num_sets) {
+    const size_t NN = (size_t)params.L.num_nodes * params.L.num_nodes;
+    std::map<std::vector<uint16_t>, uint32_t> off_of;
+    link_off.assign(num_sets, 0);
+    std::vector<uint16_t> m(NN);
+    for (uint32_t s = 0; s < num_sets; s++) {
+      for (size_t k = 0; k < NN; k++) m[k] = (uint16_t)lk[s * NN + k];
+      auto it = off_of.find(m);
+      if (it == off_of.end()) {
+        it = off_of.emplace(m, (uint32_t)links.size()).first;
+        links.insert(links.end(), m.begin(), m.end());
+      }
+      link_off[s] = it->second;
     }
   }
 
@@ -682,6 +735,17 @@ struct HostSetup {
       if (cs.voting_rights && cs.voting_rights[k]) return "voting_rights has a non-zero entry at or past the set's committee size";
       if (cs.silent && cs.silent[k]) return "a silent node is at or past the set's committee size";
     }
+    return nullptr;
+  }
+
+  // A links sweep's checks on set s's matrix `m` ([N][N]) for a committee of n nodes: null when valid.
+  static const char* links_error(const uint32_t* m, uint32_t N, uint32_t n) {
+    for (uint32_t a = 0; a < N; a++)
+      for (uint32_t b = 0; b < N; b++) {
+        const uint32_t v = m[(size_t)a * N + b];
+        if (v > 65535u) return "link_latency entries must be <= 65535";
+        if (v && (a >= n || b >= n)) return "link_latency has a non-zero entry in a row or column at or past the set's committee size";
+      }
     return nullptr;
   }
 

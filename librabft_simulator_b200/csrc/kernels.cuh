@@ -5,7 +5,8 @@
 //   lbft_sweep_event_loop_kernel / lbft_sweep_wide_kernel  the same bodies for sweep handles (lbft_create_sweep: per-instance
 //                                                          delay model and NodeConfig; lbft_create_sweep_faults: and faults;
 //                                                          lbft_create_sweep_rights: and voting rights;
-//                                                          lbft_create_sweep_committees: and committee size)
+//                                                          lbft_create_sweep_committees: and committee size;
+//                                                          lbft_create_sweep_links: and link latencies)
 //   lbft_ct_*_kernel                                       the same bodies with the commit-time stores (LBFT_FLAG_COMMIT_TIMES),
 //                                                          a twin of every one-shot single-epoch plain and sweep kernel
 //
@@ -54,8 +55,9 @@ __device__ __forceinline__ bool place_delay_thresholds(const Params& P, double* 
 // The body of both thread kernels (lbft_event_loop_kernel, lbft_sweep_event_loop_kernel), given the kernel's shared memory.
 // SW (sweep handles): the instance's parameter set supplies the delay model and NodeConfig, on a fault sweep (`records` bit 0:
 // `sets` heads a SweepSetFaults table) the silent nodes and partition plan, and on a rights sweep (bit 1: a SweepSetRights table)
-// the voting rights, quorum and leaders, and on a committee sweep (bit 2, a rights sweep too) the committee size; its thresholds
-// are read through L1 from the concatenated table, as the instances of one warp may belong to different sets.
+// the voting rights, quorum and leaders, on a committee sweep (bit 2, a rights sweep too) the committee size, and on a links
+// sweep (bit 3, a SweepSetLinks table) the link latencies; its thresholds are read through L1 from the concatenated table, as the
+// instances of one warp may belong to different sets.
 // CT: the commit-time stores (sim_core.cuh Core CT) into `times`, [num_instances][N + 1][round_cap].
 template <int NMAX, int QMODE, int FX, bool REC, bool RES, bool EP, bool TDS, int TILE, bool SW, bool CT = false>
 __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, double* s_zf, double* s_thr, uint32_t* s_queue,
@@ -95,6 +97,7 @@ __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, d
     core.bind_faults(records & 1);
     core.bind_rights(records & 2);
     core.bind_committee(records & 4);
+    core.bind_links(records & 8);
   }
   if (RES && (P.run_flags & 1u)) core.restore_regs();  // a later lbft_run_until: continue where the last launch stopped
   else core.init(P.seeds[inst]);
@@ -175,6 +178,7 @@ __device__ __forceinline__ void wide_body(const Params& P, uint32_t* s_wide, con
     core.bind_faults(records & 1);
     core.bind_rights(records & 2);
     core.bind_committee(records & 4);
+    core.bind_links(records & 8);
   }
   core.init(P.seeds[inst]);
   core.run();

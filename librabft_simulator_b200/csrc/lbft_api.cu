@@ -137,6 +137,7 @@ struct lbft_sim {
   OutputLayout regions;
   const uint64_t* sets = nullptr;    // sweep handles only, in `inputs`: HostSetup::set_table
   const uint32_t* set_of = nullptr;  // sweep handles only, in `inputs`
+  const uint16_t* links = nullptr;   // links sweeps only, in `inputs`: HostSetup::links
   // the read-out buffers, allocated on first use and grown by grow_buffer
   DeviceMemory logs;       // lbft_commit_logs: [I][cap]
   DeviceMemory times_out;  // lbft_commit_times: [I][N][cap] committed, then [I][cap] proposed
@@ -301,6 +302,14 @@ int lbft_create_sweep_committees(const lbft_config* config, const lbft_param_set
   });
 }
 
+int lbft_create_sweep_links(const lbft_config* config, const lbft_param_set* sets, const lbft_fault_set* faults,
+                            const uint64_t* voting_rights, const uint32_t* committee_sizes, const uint32_t* link_latency,
+                            uint32_t num_sets, const uint32_t* set_of_instance, lbft_sim** out_sim) {
+  return create_handle(config, out_sim, [&](HostSetup& hs) {
+    return hs.build_sweep_links(*config, sets, faults, voting_rights, committee_sizes, link_latency, num_sets, set_of_instance);
+  });
+}
+
 }  // extern "C"
 
 // The device half of the lbft_create* entry points, once the host setup `s->hs` is built.  On failure the partial handle is
@@ -340,7 +349,7 @@ static int create_on_device(std::unique_ptr<lbft_sim> s, const lbft_config* conf
   };
   const size_t zig_x = stage(hs.zig_x), zig_f = stage(hs.zig_f), delay_thr = stage(hs.delay_thr), sets = stage(set_table),
                duration = stage(hs.duration), period = stage(hs.period), weights = stage(hs.weights), set_of = stage(hs.set_of),
-               leader = stage(hs.leader);
+               links = stage(hs.links), leader = stage(hs.leader);
   CREATE_TRY(s->dev_alloc(s->inputs, seeds_bytes + tables.size()));
   CREATE_TRY(cudaMemcpy(s->inputs.at(seeds_bytes), tables.data(), tables.size(), cudaMemcpyHostToDevice));
   s->regions = OutputLayout(I, N);
@@ -368,6 +377,7 @@ static int create_on_device(std::unique_ptr<lbft_sim> s, const lbft_config* conf
     s->sets = in.at<uint64_t>(sets);
     s->set_of = in.at<uint32_t>(set_of);
   }
+  if (!hs.links.empty()) s->links = in.at<uint16_t>(links);
   P.state = s->state.at<uint32_t>();
   const DeviceMemory& out = s->outputs;
   const OutputLayout& at = s->regions;
@@ -487,9 +497,13 @@ int lbft_run_until(lbft_sim* s, int64_t stop_clock) {
 
 }  // extern "C"
 
-// A rights sweep's device table (lbft_create_sweep_rights), or null: the read-outs take each instance's leaders and weights from it.
-static const SweepSetRights* rights_table(const lbft_sim* s) {
-  return s->hs.rights.empty() ? nullptr : reinterpret_cast<const SweepSetRights*>(s->sets);
+// A rights sweep's device table (lbft_create_sweep_rights), or null: the read-outs take each instance's leaders and weights from
+// it, set g's entry at sweep_set_at(table, g, records) (a links sweep's entries carry their links record too).
+static const SweepSet* rights_table(const lbft_sim* s) {
+  return s->hs.rights.empty() ? nullptr : reinterpret_cast<const SweepSet*>(s->sets);
+}
+__device__ __forceinline__ const SweepRights& rights_of(const SweepSet* table, uint32_t g, uint32_t records) {
+  return reinterpret_cast<const SweepSetRights*>(sweep_set_at(table, g, records))->rights;
 }
 
 static int enqueue_kernel(lbft_sim* s) {
@@ -499,7 +513,7 @@ static int enqueue_kernel(lbft_sim* s) {
   CUDA_TRY(cudaEventRecord(s->ev[2], s->stream));
   const KernelSel& k = s->hs.sel;
   const uint32_t records = s->hs.records();
-  const SweepParams sp{s->P, s->set_of, reinterpret_cast<const SweepSet*>(s->sets), records & 1u, (records >> 1) & 3u};
+  const SweepParams sp{s->P, s->set_of, reinterpret_cast<const SweepSet*>(s->sets), records & 1u, (records >> 1) & 3u, s->links};
   const CtParams<Params> cp{s->P, s->times.at<int32_t>()};
   const CtParams<SweepParams> csp{sp, s->times.at<int32_t>()};
   cudaError_t e = k.ct ? (k.sweep ? (k.wide ? launch_ct_sweep_wide(k, csp, s->stream) : launch_ct_sweep_thread(k, csp, s->stream))
@@ -693,14 +707,14 @@ static int finish_chain_check(lbft_sim* s) {
 // depth == its commit count, SURVEY App. C.3).  Instances where that does not hold are counted in *bad.
 // The proposer of round r is leader(r) of the instance's leader table: on a rights sweep (`rights` not null) its set's.
 // ---------------------------------------------------------------------------------------------
-__global__ void lbft_commit_logs_kernel(const __grid_constant__ Params P, uint32_t stride, const uint32_t* set_of, const SweepSetRights* rights,
-                                        lbft_commit* out, uint32_t cap, uint32_t* bad) {
+__global__ void lbft_commit_logs_kernel(const __grid_constant__ Params P, uint32_t stride, const uint32_t* set_of, const SweepSet* rights,
+                                        uint32_t records, lbft_commit* out, uint32_t cap, uint32_t* bad) {
   const uint32_t inst = blockIdx.x * blockDim.x + threadIdx.x;
   if (inst >= P.num_instances) return;
   const Layout& L = P.L;
   const uint32_t N = L.num_nodes, tile = inst / stride, lane = inst % stride;
   const uint32_t* tb = P.state + (size_t)tile * L.total_words * stride + lane;
-  const uint8_t* leader = P.leader + (rights ? rights[set_of[inst]].rights.leader_off : 0u);
+  const uint8_t* leader = P.leader + (rights ? rights_of(rights, set_of[inst], records).leader_off : 0u);
   lbft_commit* row = out + (size_t)inst * cap;
   if (!walk_commit_chain(L, tb, stride, P.out_commit_counts + (size_t)inst * N, P.out_lc_round + (size_t)inst * N,
                          [&](uint32_t k, uint32_t r, uint32_t c0) {
@@ -725,7 +739,8 @@ int lbft_commit_logs(lbft_sim* s, lbft_commit* out, size_t cap, uint32_t* lens) 
   // rows beyond a log's length are zero
   CUDA_TRY(cudaMemsetAsync(s->logs.at(), 0, bytes, s->stream));
   CUDA_TRY(cudaMemsetAsync(s->P.out_error, 0, sizeof(uint32_t), s->stream));
-  lbft_commit_logs_kernel<<<(s->I + 127) / 128, 128, 0, s->stream>>>(s->P, s->stride, s->set_of, rights_table(s), s->logs.at<lbft_commit>(),
+  lbft_commit_logs_kernel<<<(s->I + 127) / 128, 128, 0, s->stream>>>(s->P, s->stride, s->set_of, rights_table(s), s->hs.records(),
+                                                                       s->logs.at<lbft_commit>(),
                                                                        (uint32_t)cap, s->P.out_error);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaMemcpyAsync(out, s->logs.at(), bytes, cudaMemcpyDeviceToHost, s->stream));
@@ -877,7 +892,8 @@ __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __g
 // the unreached block into the reduction of the per-sample kernel (LatencyReduction).
 __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __grid_constant__ Params P, uint32_t stride,
                                                                        const int32_t* times, const uint32_t* set_of,
-                                                                       const SweepSetRights* rights, uint32_t G, const uint32_t* W,
+                                                                       const SweepSet* rights, uint32_t records, uint32_t G,
+                                                                       const uint32_t* W,
                                                                        int64_t width, uint32_t bins,
                                                                        int64_t from, int64_t until, lbft_latency_summary* sum,
                                                                        unsigned long long* unreached_out,
@@ -896,7 +912,7 @@ __global__ void __launch_bounds__(kLatBlock) lbft_latency_stats_kernel(const __g
     const uint32_t gmask = G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (warp_lane & ~(G - 1));
     const uint32_t n0 = j, n1 = j + 32;  // (n1 < N only when N > 32, i.e. G == 32)
     const uint32_t cc0 = n0 < N ? cc[n0] : 0u, cc1 = n1 < N ? cc[n1] : 0u;
-    const uint32_t* w = rights ? rights[red.g].rights.weights : P.c_weights;  // (red.g: the instance's set on a sweep)
+    const uint32_t* w = rights ? rights_of(rights, red.g, records).weights : P.c_weights;  // (red.g: the instance's set on a sweep)
     const uint32_t Wg = W[red.g];
     auto time_of = [&](uint32_t k, uint32_t r) -> int64_t {
       return block_threshold_time_lanes(L, G, gmask, j, cc0, cc1, t_inst, w, k, r, Wg);
@@ -954,7 +970,7 @@ static int latency_stats(lbft_sim* s, const lbft_latency_spec* spec, const uint6
     W.assign(thresholds, thresholds + groups);  // (checked: each at most 64 * 2^24)
     CUDA_TRY(cudaMemcpyAsync(d_thresholds, W.data(), groups * sizeof(uint32_t), cudaMemcpyHostToDevice, s->stream));
     lbft_latency_stats_kernel<<<(s->I + per_block - 1) / per_block, kLatBlock, smem, s->stream>>>(
-        s->P, s->stride, s->times.at<int32_t>(), set_of, rights_table(s), G, d_thresholds, spec->bin_width, bins, spec->proposed_from,
+        s->P, s->stride, s->times.at<int32_t>(), set_of, rights_table(s), s->hs.records(), G, d_thresholds, spec->bin_width, bins, spec->proposed_from,
         spec->proposed_until, d_sum, d_unreached, d_hist, s->P.out_error);
   }
   CUDA_TRY(cudaGetLastError());

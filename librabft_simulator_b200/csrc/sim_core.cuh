@@ -357,16 +357,34 @@ LBFT_HD uint32_t nodes_behind(const SweepSet* set) {
 #endif
 }
 
+// Where the link-latency matrix of a links sweep's set starts in SweepParams::links (Core::link_latency), read the same way.
+static_assert(offsetof(SweepSetLinks, links) == 344 && offsetof(SweepLinks, link_off) == 0, "the immediate below");
+LBFT_HD uint32_t link_off_behind(const SweepSet* set) {
+#if defined(__CUDA_ARCH__)
+  uint32_t v;
+  asm volatile("ld.global.nc.u32 %0, [%1+344];" : "=r"(v) : "l"(set));
+  return v;
+#else
+  return reinterpret_cast<const SweepSetLinks*>(set)->links.link_off;
+#endif
+}
+
 static_assert(offsetof(SweepParams, P) == 0, "Core::sweep_records: a sweep kernel's Params heads its SweepParams");
 
 // The records behind each set of a sweep's table (sweep_set_at): bit 0 faults, bit 1 rights, bit 2 the committee size (a
-// committee sweep's SweepParams::rights has bits 0 and 1 set: its table is a rights sweep's).
-LBFT_HD uint32_t sweep_records(const SweepParams& S) { return (S.faults ? 1u : 0u) | (S.rights ? 2u : 0u) | ((S.rights & 2u) << 1); }
+// committee sweep's SweepParams::rights has bits 0 and 1 set: its table is a rights sweep's), bit 3 the link latencies (a links
+// sweep's SweepParams::links is not null; its rights bit is set too).
+LBFT_HD uint32_t sweep_records(const SweepParams& S) {
+  return (S.faults ? 1u : 0u) | (S.rights ? 2u : 0u) | ((S.rights & 2u) << 1) | (S.links ? 8u : 0u);
+}
 
-// Set s of a sweep's device table, whose entries are SweepSet, SweepSetFaults or SweepSetRights by `records` (bit 0: a fault
-// record follows each set, bit 1: a rights record follows that; bit 2 does not change the entry).
+// Set s of a sweep's device table, whose entries are SweepSet, SweepSetFaults, SweepSetRights or SweepSetLinks by `records`
+// (bit 0: a fault record follows each set, bit 1: a rights record follows that, bit 3: a links record follows that; bit 2 does
+// not change the entry).
 LBFT_HD const SweepSet* sweep_set_at(const SweepSet* sets, uint32_t s, uint32_t records) {
-  const size_t pitch = (records & 2) ? sizeof(SweepSetRights) : ((records & 1) ? sizeof(SweepSetFaults) : sizeof(SweepSet));
+  const size_t pitch = (records & 8)   ? sizeof(SweepSetLinks)
+                       : (records & 2) ? sizeof(SweepSetRights)
+                                       : ((records & 1) ? sizeof(SweepSetFaults) : sizeof(SweepSet));
   return reinterpret_cast<const SweepSet*>(reinterpret_cast<const char*>(sets) + pitch * s);
 }
 
@@ -708,8 +726,8 @@ struct Core {
   const double* thr;  // delay thresholds (shared-memory copy on the device when it fits; SW: the instance's set's, bind_set)
   const SweepSet* sw = nullptr;  // SW: the instance's parameter set
   uint32_t records = 0;          // SW, host: the records behind `sw` (sweep_set_at): bit 0 faults (bind_faults), bit 1 rights
-                                 // (bind_rights), bit 2 the committee size (bind_committee); the device reads them from the
-                                 // launch's parameter block instead (sweep_records)
+                                 // (bind_rights), bit 2 the committee size (bind_committee), bit 3 the link latencies
+                                 // (bind_links); the device reads them from the launch's parameter block instead (sweep_records)
   using Queue = QueueFor<QMODE, Mem, G, KS>;
   Queue q;                 // given its shared memory by the constructor (QMODE 2: sk / sd, or the host harness's stand-in) and init (km)
   uint32_t* km = nullptr;  // KS: the calendar's occupancy words in shared memory, a column per lane, set by the kernel
@@ -820,6 +838,19 @@ struct Core {
   LBFT_HD uint32_t nodes() const {
     if constexpr (SW) return (sweep_records() & 4) ? nodes_behind(sw) : L.num_nodes;
     else return L.num_nodes;
+  }
+  // The link latency M[a][b] of a links sweep (bind_links) from sender a to receiver b, added to every network event's time
+  // (enqueue_network_event).  As with the rights, nothing is held through the loop: the set's matrix offset and the entry are
+  // loaded where the event is sent.  The table is SweepParams::links, of the launch's parameter block on the device, and of the
+  // SweepParams whose P the host harness binds.
+  LBFT_HD void bind_links(bool links_sweep) { records = (records & ~8u) | (links_sweep ? 8u : 0u); }
+  LBFT_HD uint32_t link_latency(uint32_t a, uint32_t b) const {
+    const uint16_t* table = reinterpret_cast<const SweepParams*>(&P)->links + link_off_behind(sw) + a * L.num_nodes + b;
+#if defined(__CUDA_ARCH__)
+    return __ldg(table);
+#else
+    return *table;
+#endif
   }
   // ------------------------------------------------------------------------------------------
   // RNG (rand_xoshiro 0.6.0 / rand 0.8.3 / rand_distr 0.4.0)
@@ -1727,6 +1758,11 @@ struct Core {
   }
   LBFT_HD bool enqueue_network_event(uint32_t kind, uint32_t receiver, uint32_t sender, uint32_t slot, int32_t delay) {
     int32_t t = clock + delay;
+    // A links sweep: the link latency from the sender to the receiver, after the delay draw.  No wrap: clock <= max_clock < 2^29,
+    // a delay is at most 2^29 (uniform and constant, host_setup.hpp delay_model) or 10^9 (delay_via_exp), and an entry 65535.
+    static_assert((1LL << 29) + 1000000000LL + 65535LL < (1LL << 31), "clock + delay + link latency fits in int32_t");
+    if constexpr (SW)
+      if (sweep_records() & 8) t += (int32_t)link_latency(sender, receiver);
     if (L.part_windows && partitioned(receiver, sender)) {
       stamp++;
       return false;

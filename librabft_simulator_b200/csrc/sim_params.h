@@ -290,6 +290,20 @@ struct SweepSetRights {
   SweepRights rights;
 };
 
+// The link latencies of one parameter set of a links sweep (lbft_create_sweep_links): its N x N matrix of u16 milliseconds
+// starts at SweepParams::links[link_off] (entry [sender * N + receiver], N = Layout::num_nodes); sets with equal matrices share
+// one.
+struct SweepLinks {
+  uint32_t link_off;
+  uint32_t pad;
+};
+// One entry of a links sweep's device table: a rights sweep's entry (a links sweep carries fault and rights records for every
+// set) and its links record behind it (sim_core.cuh Core::link_latency).
+struct SweepSetLinks {
+  SweepSetRights sr;
+  SweepLinks links;
+};
+
 // The parameter block of a sweep handle's kernels (lbft_create_sweep): instance i runs with sets[set_of[i]], and
 // P.delay_thr / P.duration / P.period are the concatenated tables of all sets.  (A block of its own rather than fields
 // appended to Params, so that no other kernel's parameters move.)
@@ -297,10 +311,13 @@ struct SweepParams {
   Params P;
   const uint32_t* set_of;  // [num_instances]
   const SweepSet* sets;    // [num_sets]; a fault sweep (lbft_create_sweep_faults): the sets of a SweepSetFaults [num_sets] table;
-                           // a rights sweep (lbft_create_sweep_rights): of a SweepSetRights [num_sets] table
+                           // a rights sweep (lbft_create_sweep_rights): of a SweepSetRights [num_sets] table; a links sweep
+                           // (lbft_create_sweep_links): of a SweepSetLinks [num_sets] table
   uint32_t faults;         // 1: a fault or rights sweep, whose instances take their silent nodes and partition plan from their set's record
   uint32_t rights;         // bit 0: a rights sweep, whose instances take their voting rights, quorum and leaders from their set's
                            // record; bit 1: a committee sweep (a rights sweep too), whose instances take their committee size from it
+  const uint16_t* links;   // a links sweep (a rights sweep too), whose instances add their set's link latencies to every send: the
+                           // sets' matrices (SweepLinks); null on every other sweep
 };
 
 }  // namespace lbft

@@ -594,22 +594,40 @@ class ParamSet:
     """One point of a parameter sweep: the network delay and ``NodeConfig`` of the instances assigned to it
     (main.rs --mean / --variance and --delta / --gamma / --lambda / --target_commit_interval), its fault model, its
     voting rights: a tuple of one int per node of the set, or None for 1 per node (``BatchSimulator``'s ``voting_rights``),
-    and its committee size: None for the simulator's ``num_nodes``."""
+    its committee size: None for the simulator's ``num_nodes``, and its link latencies: an ``n x n`` nested sequence of whole
+    milliseconds (``n`` the set's committee size), entry ``[a][b]`` added to the time of every message from node a to node b
+    (see ``regional_latency``), or None for none."""
     network_delay: RandomDelay = RandomDelay()
     node_config: NodeConfig = NodeConfig()
     faults: FaultSet = FaultSet()
     voting_rights: tuple = None
     num_nodes: int = None
+    link_latency: tuple = None
 
     def __post_init__(self):
         if self.voting_rights is not None:  # (a list or array compares, and hashes, as a tuple)
             object.__setattr__(self, "voting_rights", tuple(int(w) for w in self.voting_rights))
+        if self.link_latency is not None:  # (likewise, a tuple of tuples)
+            object.__setattr__(self, "link_latency", tuple(tuple(int(v) for v in row) for row in self.link_latency))
 
     def to_c(self):
         d, n = self.network_delay, self.node_config
         return _lib.LbftParamSet(delay_kind=d.kind, reserved=0, delay_mean=d.mean, delay_variance=d.variance, delay_lo=d.lo,
                                  delay_hi=d.hi, target_commit_interval=n.target_commit_interval, delta=n.delta, gamma=n.gamma,
                                  lambda_=n.lambda_)
+
+
+def regional_latency(region_of_node, latency_between_regions):
+    """The link-latency matrix (``ParamSet.link_latency``) of a committee placed in regions: ``region_of_node[a]`` is node a's
+    region, ``latency_between_regions[r][q]`` the latency in ms of a message from region r to region q (its diagonal the
+    latency within a region).  Entry ``[a][b]`` is ``latency_between_regions[region_of_node[a]][region_of_node[b]]``."""
+    regions = np.asarray(region_of_node, dtype=np.int64).reshape(-1)
+    between = np.asarray(latency_between_regions, dtype=np.int64)
+    if between.ndim != 2 or between.shape[0] != between.shape[1]:
+        raise ValueError("latency_between_regions must be a square matrix, one row and column per region")
+    if regions.size and (regions.min() < 0 or regions.max() >= between.shape[0]):
+        raise ValueError("region_of_node has a region outside 0..%d" % (between.shape[0] - 1))
+    return tuple(tuple(int(v) for v in row) for row in between[regions[:, None], regions[None, :]])
 
 
 class SweepSimulator(BatchSimulator):
@@ -623,8 +641,10 @@ class SweepSimulator(BatchSimulator):
     ``num_nodes`` is the size of the layout every instance gets and must be at least every set's; the per-node arrays keep
     ``num_nodes`` columns, and an instance's nodes past its set's committee read as nodes that never committed (mask them with
     ``nodes_of_instance()``).  Every result of instance i (of its committee's nodes) is what a ``BatchSimulator`` with that
-    set's delay, node config, faults, voting rights and committee size computes for it.  Running, re-seeding (the set
-    assignment stays), streaming and reading results work as on a ``BatchSimulator``."""
+    set's delay, node config, faults, voting rights and committee size computes for it.  And the link latencies: when a set
+    carries a matrix (``ParamSet.link_latency``, ``lbft_create_sweep_links``), every network message from node a to node b of
+    an instance of that set arrives ``link_latency[a][b]`` ms later than its drawn delay says; sets without one get zeros.
+    Running, re-seeding (the set assignment stays), streaming and reading results work as on a ``BatchSimulator``."""
 
     def __init__(self, seeds, num_nodes, param_sets, set_of_instance, **shared):
         super().__init__(seeds, num_nodes, **shared)
@@ -640,7 +660,7 @@ class SweepSimulator(BatchSimulator):
             raise ValueError("a sweep whose sets have their own committee sizes takes voting rights per set only (ParamSet.voting_rights)")
 
     @classmethod
-    def grid(cls, seeds_per_point, delays, node_configs, num_nodes=4, faults=None, voting_rights=None, **shared):
+    def grid(cls, seeds_per_point, delays, node_configs, num_nodes=4, faults=None, voting_rights=None, link_latency=None, **shared):
         """The Cartesian product ``delays x node_configs`` (point p = i * len(node_configs) + j), each point run over the
         same seeds (``seeds_per_point``: a sequence of seeds, or a count k for seeds 0..k-1) in a contiguous block of
         instances: point p holds instances [p * k, (p + 1) * k).  ``set_of_instance`` and ``param_sets`` say which is which.
@@ -650,11 +670,15 @@ class SweepSimulator(BatchSimulator):
         ``node_configs`` when ``faults`` is None): ``block_latency_stats("quorum").mean().reshape(len(delays),
         len(node_configs), len(faults), len(voting_rights))``.  ``num_nodes``, a list of committee sizes instead of one,
         likewise adds a fastest-varying axis of committees, in a layout of the largest (it cannot be combined with a
-        ``voting_rights`` list, whose rows have a fixed length)."""
+        ``voting_rights`` list, whose rows have a fixed length).  ``link_latency``, a list of ``num_nodes x num_nodes`` matrices
+        (``regional_latency``), adds the fastest-varying axis after all of those (not with a list of committee sizes: the
+        matrices have a fixed size)."""
         seeds = np.arange(seeds_per_point, dtype=np.uint64) if np.isscalar(seeds_per_point) else \
             np.asarray(seeds_per_point, dtype=np.uint64).reshape(-1)
         sets = [ParamSet(d, n) for d in delays for n in node_configs] if faults is None else \
             [ParamSet(d, n, f) for d in delays for n in node_configs for f in faults]
+        if link_latency is not None and not np.isscalar(num_nodes):
+            raise ValueError("a grid takes a list of committee sizes (num_nodes) or a list of link-latency matrices, not both")
         if voting_rights is not None:
             if not np.isscalar(num_nodes):
                 raise ValueError("a grid takes a list of committee sizes (num_nodes) or a list of voting-rights rows, not both")
@@ -663,13 +687,16 @@ class SweepSimulator(BatchSimulator):
             sizes = [int(n) for n in num_nodes]
             sets = [ParamSet(p.network_delay, p.node_config, p.faults, None, n) for p in sets for n in sizes]
             num_nodes = max(sizes)
+        if link_latency is not None:
+            sets = [ParamSet(p.network_delay, p.node_config, p.faults, p.voting_rights, None, m) for p in sets for m in link_latency]
         k = seeds.shape[0]
         return cls(np.tile(seeds, len(sets)), num_nodes, sets, np.repeat(np.arange(len(sets), dtype=np.uint32), k), **shared)
 
     def create(self, max_clock):
         """``lbft_create_sweep``, or ``lbft_create_sweep_faults`` when some set has faults, or ``lbft_create_sweep_rights``
-        when some set has voting rights, or ``lbft_create_sweep_committees`` when some set has its own committee size:
-        validate every set, build the per-set host tables, allocate device state."""
+        when some set has voting rights, or ``lbft_create_sweep_committees`` when some set has its own committee size, or
+        ``lbft_create_sweep_links`` when some set has link latencies: validate every set, build the per-set host tables,
+        allocate device state."""
         per_set = any(p.faults != FaultSet() for p in self.param_sets)
         if per_set and (self.silent is not None or self.partition_windows or self.partition_max_len):
             raise ValueError("a sweep takes silent nodes and partitions either per set (ParamSet.faults) or shared (silent / "
@@ -683,7 +710,14 @@ class SweepSimulator(BatchSimulator):
         sets = (_lib.LbftParamSet * max(1, len(self.param_sets)))(*[p.to_c() for p in self.param_sets])
         so = ctypes.c_void_p(self.set_of_instance.ctypes.data)
         faults = (_lib.LbftFaultSet * len(self.param_sets))(*[p.faults.to_c() for p in self.param_sets]) if per_set else None
-        if self._committees():
+        links = self._link_table()
+        if links is not None:
+            sizes = np.ascontiguousarray(self._committee_sizes(), dtype=np.uint32) if self._committees() else None
+            _lib.check(self._lib.lbft_create_sweep_links(
+                ctypes.byref(cfg), sets, faults, None if rights is None else ctypes.c_void_p(rights.ctypes.data),
+                None if sizes is None else ctypes.c_void_p(sizes.ctypes.data), ctypes.c_void_p(links.ctypes.data),
+                len(self.param_sets), so, ctypes.byref(handle)))
+        elif self._committees():
             sizes = np.ascontiguousarray(self._committee_sizes(), dtype=np.uint32)
             _lib.check(self._lib.lbft_create_sweep_committees(
                 ctypes.byref(cfg), sets, faults, None if rights is None else ctypes.c_void_p(rights.ctypes.data),
@@ -719,6 +753,25 @@ class SweepSimulator(BatchSimulator):
                 raise ValueError("ParamSet.voting_rights needs one entry per node of the set (%d)" % sizes[s])
             rows[s, :len(row)] = row
         return rows
+
+    def _link_table(self):
+        """The [num_sets][num_nodes][num_nodes] link latencies of a links sweep (each set's matrix in the top-left corner of its
+        committee, 0 elsewhere and for sets without one), or None when no set carries any."""
+        if all(p.link_latency is None for p in self.param_sets):
+            return None
+        sizes = self._committee_sizes()
+        out = np.zeros((len(self.param_sets), self.num_nodes, self.num_nodes), dtype=np.uint32)
+        for s, p in enumerate(self.param_sets):
+            if p.link_latency is None:
+                continue
+            m = np.asarray(p.link_latency, dtype=np.int64)
+            n = int(sizes[s])
+            if m.shape != (n, n):
+                raise ValueError("parameter set %d: link_latency must be %d x %d (the set's committee)" % (s, n, n))
+            if (m < 0).any() or (m > 65535).any():
+                raise ValueError("parameter set %d: link_latency entries must be in 0..65535 ms" % s)
+            out[s, :n, :n] = m
+        return out
 
     def nodes_of_instance(self):
         """The committee size of each instance, as an int64 array [num_instances]: its set's, where the per-node arrays have
