@@ -80,6 +80,18 @@ pub mod ffi {
     #[allow(non_camel_case_types)]
     pub type lbft_fault_set = LbftFaultSet;
 
+    /// include/lbft.h `lbft_outage`: one node's outage window in an outage sweep (`lbft_create_sweep_outages`) — the node is
+    /// down at global clock t iff `down_from <= t < down_until` (ms); an empty window is no outage
+    #[repr(C)]
+    #[derive(Clone, Copy, Default, Debug, PartialEq)]
+    pub struct LbftOutage {
+        pub down_from: i64,
+        pub down_until: i64,
+    }
+    /// The header's spelling of `LbftOutage`, as the `extern "C"` block names it.
+    #[allow(non_camel_case_types)]
+    pub type lbft_outage = LbftOutage;
+
     /// include/lbft.h `lbft_commit`: one row of `committed_history()`
     #[repr(C)]
     #[derive(Clone, Copy, Default, Debug, PartialEq)]
@@ -169,6 +181,10 @@ pub mod ffi {
         pub fn lbft_create_sweep_links(config: *const LbftConfig, sets: *const lbft_param_set, faults: *const lbft_fault_set,
                                        voting_rights: *const u64, committee_sizes: *const u32, link_latency: *const u32,
                                        num_sets: u32, set_of_instance: *const u32, out_sim: *mut *mut LbftSim) -> c_int;
+        pub fn lbft_create_sweep_outages(config: *const LbftConfig, sets: *const lbft_param_set, faults: *const lbft_fault_set,
+                                         voting_rights: *const u64, committee_sizes: *const u32, link_latency: *const u32,
+                                         outages: *const lbft_outage, num_sets: u32, set_of_instance: *const u32,
+                                         out_sim: *mut *mut LbftSim) -> c_int;
         pub fn lbft_destroy(sim: *mut LbftSim);
         pub fn lbft_set_seeds(sim: *mut LbftSim, seeds: *const u64) -> c_int;
         pub fn lbft_run(sim: *mut LbftSim) -> c_int;

@@ -242,6 +242,35 @@ int lbft_create_sweep_links(const lbft_config* config, const lbft_param_set* set
                             const uint64_t* voting_rights, const uint32_t* committee_sizes, const uint32_t* link_latency,
                             uint32_t num_sets, const uint32_t* set_of_instance, lbft_sim** out_sim);
 
+/* One node's outage in an outage sweep: the node is down at global clock t iff down_from <= t < down_until (ms).  An empty
+ * window (down_from == down_until) is no outage; down_until past max_clock is a crash-stop. */
+typedef struct lbft_outage {
+  int64_t down_from;
+  int64_t down_until;
+} lbft_outage;
+
+/* An outage sweep: a links sweep whose parameter sets also carry one outage window per node.  outages[s * N + n] (N =
+ * config->num_nodes, the layout's committee) is node n's window in set s.  An event is dropped unhandled at its pop (after the
+ * max_clock test and the clock update, where the silent test sits) when its receiver is silent or down at the pop clock, or when
+ * it is a request whose sender (the node it was sent to) is silent or down then; it still counts in processed[kind] and gives
+ * back its notification slot.  The node keeps its whole state across the window (crash-recovery with persistent storage,
+ * ConsensusNode::save_node / load_node, node.rs:211-238): nothing is scheduled at recovery, and it acts again at the first event
+ * addressed to it that pops at or after down_until, a notification or a timer it scheduled before the crash.  An empty window
+ * computes what no window computes, counters included, except that a node with a non-empty window in any set of the sweep has
+ * its duplicate timers queued rather than elided, which moves the implementation counters max_queue and timers_elided in every
+ * set; [0, > max_clock) on node n computes what a silent node n computes (max_queue, max_payloads and timers_elided aside: a
+ * silent node's incoming events are also elided at send, a down node's are queued).  faults,
+ * voting_rights, committee_sizes and link_latency may each be NULL, with the rules of lbft_create_sweep_faults,
+ * lbft_create_sweep_rights, lbft_create_sweep_committees and lbft_create_sweep_links (NULL link_latency: no link term).  The
+ * layout and kernel are what the same call without outages picks.  Sets with equal schedules share one device table of N
+ * windows (lbft_memory_info counts them).  Refused (LBFT_ERR_INVALID, before any device work; the error names the set):
+ * whatever the corresponding sweep refuses, NULL outages, down_from < 0 or down_until < down_from, and a non-empty window on a
+ * node at or past the set's committee size or on a node silent in that set (its silent_mask, or config->silent when faults is
+ * NULL). */
+int lbft_create_sweep_outages(const lbft_config* config, const lbft_param_set* sets, const lbft_fault_set* faults,
+                              const uint64_t* voting_rights, const uint32_t* committee_sizes, const uint32_t* link_latency,
+                              const lbft_outage* outages, uint32_t num_sets, const uint32_t* set_of_instance, lbft_sim** out_sim);
+
 /* Simulator::new for every instance followed by loop_until(max_clock) (simulator.rs:200-250,
  * 380-475): copies the seeds host->device, runs the event-loop kernel to completion, copies the
  * per-node summaries (commit counts, last-committed-state keys, counters, status) device->host.

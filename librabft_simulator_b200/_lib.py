@@ -38,6 +38,14 @@ class LbftFaultSet(ctypes.Structure):
     _fields_ = [("silent_mask", c_u64), ("partition_windows", c_u32), ("partition_max_len", c_u32)]
 
 
+class LbftOutage(ctypes.Structure):
+    """``lbft_outage`` of include/lbft.h: one node's outage window in an outage sweep (``lbft_create_sweep_outages``)."""
+    _fields_ = [("down_from", c_i64), ("down_until", c_i64)]
+
+
+INT64_MAX = (1 << 63) - 1
+
+
 class LbftCommit(ctypes.Structure):
     _fields_ = [("proposer", c_u32), ("index", c_u32), ("time", c_i64)]
 
@@ -76,7 +84,7 @@ ST_INVARIANT, ST_EPOCH_CHANGE, ST_DELAY_NEAR_INT, ST_TIME_OVERFLOW = 16, 32, 64,
 ST_ERROR_MASK = ST_ROUND_OVERFLOW | ST_QUEUE_OVERFLOW | ST_PAYLOAD_OVERFLOW | ST_INVARIANT | ST_TIME_OVERFLOW
 
 EXPORTS = [
-    "lbft_create", "lbft_create_sweep", "lbft_create_sweep_faults", "lbft_create_sweep_rights", "lbft_create_sweep_committees", "lbft_create_sweep_links", "lbft_run", "lbft_run_async", "lbft_wait", "lbft_commit_logs", "lbft_commit_times", "lbft_latency_stats", "lbft_block_latency_stats_groups", "lbft_block_latency_stats", "lbft_upload", "lbft_run_device", "lbft_download", "lbft_commit_counts",
+    "lbft_create", "lbft_create_sweep", "lbft_create_sweep_faults", "lbft_create_sweep_rights", "lbft_create_sweep_committees", "lbft_create_sweep_links", "lbft_create_sweep_outages", "lbft_run", "lbft_run_async", "lbft_wait", "lbft_commit_logs", "lbft_commit_times", "lbft_latency_stats", "lbft_block_latency_stats_groups", "lbft_block_latency_stats", "lbft_upload", "lbft_run_device", "lbft_download", "lbft_commit_counts",
     "lbft_last_states", "lbft_commit_log", "lbft_round_switches", "lbft_active_rounds", "lbft_counters", "lbft_status", "lbft_timing_info",
     "lbft_memory_info", "lbft_kernel_info", "lbft_run_until", "lbft_snapshot_size", "lbft_snapshot_save", "lbft_snapshot_load", "lbft_set_seeds", "lbft_device_buffer", "lbft_destroy", "lbft_last_error", "lbft_abi_version",
 ]
@@ -111,6 +119,8 @@ def load():
                                                  c_u32, P, ctypes.POINTER(P)]
     lib.lbft_create_sweep_links.argtypes = [ctypes.POINTER(LbftConfig), ctypes.POINTER(LbftParamSet), ctypes.POINTER(LbftFaultSet), P, P, P,
                                             c_u32, P, ctypes.POINTER(P)]
+    lib.lbft_create_sweep_outages.argtypes = [ctypes.POINTER(LbftConfig), ctypes.POINTER(LbftParamSet), ctypes.POINTER(LbftFaultSet), P, P, P,
+                                              ctypes.POINTER(LbftOutage), c_u32, P, ctypes.POINTER(P)]
     for name in ("lbft_run", "lbft_run_async", "lbft_wait", "lbft_upload", "lbft_run_device", "lbft_download"):
         getattr(lib, name).argtypes = [P]
     for name in ("lbft_commit_counts", "lbft_last_states", "lbft_active_rounds", "lbft_counters", "lbft_status"):

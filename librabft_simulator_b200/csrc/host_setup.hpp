@@ -373,6 +373,9 @@ struct HostSetup {
   bool committees = false;          // a committee sweep (build_sweep_committees): each set's fault record carries its committee size
   std::vector<uint16_t> links;      // links sweeps: the distinct N x N link-latency matrices of the sets (build_sweep_links)
   std::vector<uint32_t> link_off;   // links sweeps: one record per parameter set, where its matrix starts in `links`; empty otherwise
+  std::vector<SweepOutage> outages;  // outage sweeps: the distinct schedules of N windows of the sets (build_sweep_outages)
+  std::vector<uint32_t> outage_off;  // outage sweeps: one record per parameter set, where its schedule starts in `outages`
+  uint64_t down_mask = 0;            // outage sweeps: the nodes with a non-empty window in any set (SweepParams::down_mask)
   std::string error;
   KernelSel sel{};
 
@@ -415,9 +418,15 @@ struct HostSetup {
   // on the matrices: the stamp-width and queue-mode tests are sized by the shortest mean delay, which over-estimates the event
   // rate of a network slowed by its links, so they stay safe (and an overrun still surfaces as LBFT_ERR_CAPACITY).  `links` gets
   // one matrix per distinct one, `link_off` each set's.
+  //
+  // An outage sweep (lbft_create_sweep_outages, `out` not null: [num_sets][num_nodes]): a rights sweep (a committee sweep when
+  // `sizes` is not null, a links sweep too when `lk` is not null) whose set s drops the events of node n while it is down,
+  // out[s][n].  Layout and kernel do not depend on the windows: a window only filters which pops are handled.  Each window is
+  // clamped into [0, max_clock + 1] (an empty one to {0, 0}); `outages` gets one schedule per distinct one, `outage_off` each
+  // set's, and `down_mask` the nodes with a non-empty window in any set, which Params::silent_mask takes in too.
   bool build_sweep(const lbft_config& c, const lbft_param_set* ps, uint32_t num_sets, const uint32_t* set_of_instance,
                    const lbft_fault_set* fs = nullptr, const uint64_t* vr = nullptr, const uint32_t* sizes = nullptr,
-                   const uint32_t* lk = nullptr) {
+                   const uint32_t* lk = nullptr, const lbft_outage* out = nullptr) {
     if (c.struct_size != sizeof(lbft_config)) return fail("lbft_config.struct_size does not match this library (ABI mismatch)");
     if (!ps || !set_of_instance) return fail("sets and set_of_instance must not be NULL");
     if (num_sets == 0 || num_sets > c.num_instances || num_sets > 65536u) return fail("num_sets must be in 1..min(num_instances, 65536)");
@@ -439,14 +448,15 @@ struct HostSetup {
       if (!e) e = config_error(cs);
       if (!e && fs && cs.num_nodes < 64 && (fs[s].silent_mask >> cs.num_nodes)) e = "silent_mask has a bit at or above num_nodes";
       if (!e && lk) e = links_error(lk + (size_t)s * c.num_nodes * c.num_nodes, c.num_nodes, cs.num_nodes);
+      if (!e && out) e = outage_error(out + (size_t)s * c.num_nodes, c.num_nodes, cs.num_nodes, fs ? fs[s].silent_mask : silent_of(c));
       if (e || ps[s].reserved)
         return fail(("parameter set " + std::to_string(s) + ": " + (ps[s].reserved ? "reserved must be 0" : e)).c_str());
       if (mean_delay(cs) < mean_delay(with_set(c, ps[fastest]))) fastest = s;
       if (fs && fs[s].partition_windows > windows) windows = fs[s].partition_windows;
     }
-    // a committee or links sweep without rights: the shared rights, or 1, for each node of a set's committee (validated above)
+    // a committee, links or outage sweep without rights: the shared rights, or 1, for each node of a set's committee (validated above)
     std::vector<uint64_t> ones;
-    if ((sizes || lk) && !vr) {
+    if ((sizes || lk || out) && !vr) {
       ones.assign((size_t)num_sets * c.num_nodes, 0);
       for (uint32_t s = 0; s < num_sets; s++)
         for (uint32_t n = 0; n < (sizes ? sizes[s] : c.num_nodes); n++)
@@ -478,8 +488,12 @@ struct HostSetup {
       for (uint32_t s = 0; s < num_sets; s++) faults[s].num_nodes = (uint16_t)sizes[s];
     if (vr) add_rights(vr, num_sets);
     if (lk) add_links(lk, num_sets);
+    if (out) add_outages(out, num_sets);
     committees = sizes != nullptr;
     sel = select_kernel(cf, tile, params, true);
+    // the windowed nodes join the launch-uniform "any silent node" test (Core::any_silent), behind which the pop-side drop tests
+    // them: a sweep without windows keeps its mask (and an outage sweep's fault records keep each set's own silent nodes)
+    params.silent_mask |= down_mask;
     return true;
   }
 
@@ -514,11 +528,22 @@ struct HostSetup {
     return build_sweep(c, ps, num_sets, set_of_instance, fs, vr, sizes, lk);
   }
 
+  // An outage sweep (lbft_create_sweep_outages): build_sweep with each set's outage windows (out[s], [num_nodes]), its link
+  // latencies when `lk` is not null, its voting rights (row s of `vr`, or the shared ones when `vr` is null), its faults when
+  // `fs` is not null and its committee size when `sizes` is not null.
+  bool build_sweep_outages(const lbft_config& c, const lbft_param_set* ps, const lbft_fault_set* fs, const uint64_t* vr,
+                           const uint32_t* sizes, const uint32_t* lk, const lbft_outage* out, uint32_t num_sets,
+                           const uint32_t* set_of_instance) {
+    if (!out) return fail("outages must not be NULL");
+    return build_sweep(c, ps, num_sets, set_of_instance, fs, vr, sizes, lk, out);
+  }
+
   // Which records follow each set in the sweep's device table (sim_core.cuh sweep_set_at): bit 0 faults, bit 1 rights, bit 2 on
-  // a committee sweep, whose fault records carry the committee sizes (the entries are those of a rights sweep), and bit 3 the
-  // links records of a links sweep.
+  // a committee sweep, whose fault records carry the committee sizes (the entries are those of a rights sweep), bit 3 the link
+  // latencies of a links sweep and bit 4 the outage windows of an outage sweep (either puts a links record behind each set).
   uint32_t records() const {
-    return (faults.empty() ? 0u : 1u) | (rights.empty() ? 0u : 2u) | (committees ? 4u : 0u) | (link_off.empty() ? 0u : 8u);
+    return (faults.empty() ? 0u : 1u) | (rights.empty() ? 0u : 2u) | (committees ? 4u : 0u) | (link_off.empty() ? 0u : 8u) |
+           (outage_off.empty() ? 0u : 16u);
   }
 
   // A sweep's device table of parameter sets, the bytes the runtime uploads: `sets`, each followed by its fault record, its
@@ -526,7 +551,7 @@ struct HostSetup {
   // entries).
   std::vector<uint64_t> set_table() const {
     const uint32_t rec = records();
-    const size_t pitch = (rec & 8)   ? sizeof(SweepSetLinks)
+    const size_t pitch = (rec & 24)  ? sizeof(SweepSetLinks)
                          : (rec & 2) ? sizeof(SweepSetRights)
                                      : ((rec & 1) ? sizeof(SweepSetFaults) : sizeof(SweepSet));
     static_assert(sizeof(SweepSet) % 8 == 0 && sizeof(SweepSetFaults) % 8 == 0 && sizeof(SweepSetRights) % 8 == 0 &&
@@ -537,8 +562,8 @@ struct HostSetup {
       memcpy(e, &sets[k], sizeof(SweepSet));
       if (rec & 1) memcpy(e + offsetof(SweepSetFaults, faults), &faults[k], sizeof(SweepFaults));
       if (rec & 2) memcpy(e + offsetof(SweepSetRights, rights), &rights[k], sizeof(SweepRights));
-      if (rec & 8) {
-        const SweepLinks l{link_off[k], 0};
+      if (rec & 24) {
+        const SweepLinks l{(rec & 8) ? link_off[k] : 0u, (rec & 16) ? outage_off[k] : 0u};
         memcpy(e + offsetof(SweepSetLinks, links), &l, sizeof(SweepLinks));
       }
     }
@@ -624,6 +649,31 @@ struct HostSetup {
         links.insert(links.end(), m.begin(), m.end());
       }
       link_off[s] = it->second;
+    }
+  }
+
+  // An outage sweep's records (`out`: [num_sets][N], checked by outage_error): each window clamped into [0, max_clock + 1], an
+  // empty one stored as {0, 0}; one schedule per distinct one in `outages`, where each set's starts in `outage_off`, and the
+  // union of the nodes with a non-empty window in `down_mask`.  (max_clock < 2^29, config_error: the clamp fits in int32_t.)
+  void add_outages(const lbft_outage* out, uint32_t num_sets) {
+    const uint32_t N = params.L.num_nodes;
+    const int64_t end = (int64_t)params.max_clock + 1;
+    std::map<std::vector<std::pair<int32_t, int32_t>>, uint32_t> off_of;
+    outage_off.assign(num_sets, 0);
+    std::vector<std::pair<int32_t, int32_t>> w(N);
+    for (uint32_t s = 0; s < num_sets; s++) {
+      for (uint32_t n = 0; n < N; n++) {
+        const lbft_outage& o = out[(size_t)s * N + n];
+        const int32_t from = (int32_t)std::min(o.down_from, end), until = (int32_t)std::min(o.down_until, end);
+        w[n] = from < until ? std::make_pair(from, until) : std::make_pair(0, 0);
+        if (from < until) down_mask |= 1ULL << n;
+      }
+      auto it = off_of.find(w);
+      if (it == off_of.end()) {
+        it = off_of.emplace(w, (uint32_t)outages.size()).first;
+        for (const auto& v : w) outages.push_back(SweepOutage{v.first, v.second});
+      }
+      outage_off[s] = it->second;
     }
   }
 
@@ -747,6 +797,26 @@ struct HostSetup {
         if (v && (a >= n || b >= n)) return "link_latency has a non-zero entry in a row or column at or past the set's committee size";
       }
     return nullptr;
+  }
+
+  // An outage sweep's checks on set s's windows `w` ([N]) for a committee of n nodes with silent nodes `silent`: null when valid.
+  static const char* outage_error(const lbft_outage* w, uint32_t N, uint32_t n, uint64_t silent) {
+    for (uint32_t k = 0; k < N; k++) {
+      if (w[k].down_from < 0) return "outages: down_from must be >= 0";
+      if (w[k].down_until < w[k].down_from) return "outages: down_until must be >= down_from";
+      if (w[k].down_until > w[k].down_from && k >= n) return "outages has a non-empty window on a node at or past the set's committee size";
+      if (w[k].down_until > w[k].down_from && ((silent >> k) & 1)) return "outages has a non-empty window on a silent node";
+    }
+    return nullptr;
+  }
+
+  // The silent nodes of lbft_config.silent as a bit mask.
+  static uint64_t silent_of(const lbft_config& c) {
+    uint64_t m = 0;
+    if (c.silent)
+      for (uint32_t n = 0; n < c.num_nodes && n < 64; n++)
+        if (c.silent[n]) m |= 1ULL << n;
+    return m;
   }
 
   bool fail(const char* msg) {

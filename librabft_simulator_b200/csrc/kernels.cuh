@@ -6,7 +6,8 @@
 //                                                          delay model and NodeConfig; lbft_create_sweep_faults: and faults;
 //                                                          lbft_create_sweep_rights: and voting rights;
 //                                                          lbft_create_sweep_committees: and committee size;
-//                                                          lbft_create_sweep_links: and link latencies)
+//                                                          lbft_create_sweep_links: and link latencies;
+//                                                          lbft_create_sweep_outages: and node outages)
 //   lbft_ct_*_kernel                                       the same bodies with the commit-time stores (LBFT_FLAG_COMMIT_TIMES),
 //                                                          a twin of every one-shot single-epoch plain and sweep kernel
 //
@@ -56,7 +57,8 @@ __device__ __forceinline__ bool place_delay_thresholds(const Params& P, double* 
 // SW (sweep handles): the instance's parameter set supplies the delay model and NodeConfig, on a fault sweep (`records` bit 0:
 // `sets` heads a SweepSetFaults table) the silent nodes and partition plan, and on a rights sweep (bit 1: a SweepSetRights table)
 // the voting rights, quorum and leaders, on a committee sweep (bit 2, a rights sweep too) the committee size, and on a links
-// sweep (bit 3, a SweepSetLinks table) the link latencies; its thresholds are read through L1 from the concatenated table, as the
+// sweep (bit 3, a SweepSetLinks table) the link latencies, and on an outage sweep (bit 4, a SweepSetLinks table) the outage
+// windows; its thresholds are read through L1 from the concatenated table, as the
 // instances of one warp may belong to different sets.
 // CT: the commit-time stores (sim_core.cuh Core CT) into `times`, [num_instances][N + 1][round_cap].
 template <int NMAX, int QMODE, int FX, bool REC, bool RES, bool EP, bool TDS, int TILE, bool SW, bool CT = false>
@@ -98,6 +100,7 @@ __device__ __forceinline__ void event_loop_body(const Params& P, double* s_zx, d
     core.bind_rights(records & 2);
     core.bind_committee(records & 4);
     core.bind_links(records & 8);
+    core.bind_outages(records & 16);
   }
   if (RES && (P.run_flags & 1u)) core.restore_regs();  // a later lbft_run_until: continue where the last launch stopped
   else core.init(P.seeds[inst]);
@@ -179,6 +182,7 @@ __device__ __forceinline__ void wide_body(const Params& P, uint32_t* s_wide, con
     core.bind_rights(records & 2);
     core.bind_committee(records & 4);
     core.bind_links(records & 8);
+    core.bind_outages(records & 16);
   }
   core.init(P.seeds[inst]);
   core.run();

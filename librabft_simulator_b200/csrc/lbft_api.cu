@@ -138,6 +138,7 @@ struct lbft_sim {
   const uint64_t* sets = nullptr;    // sweep handles only, in `inputs`: HostSetup::set_table
   const uint32_t* set_of = nullptr;  // sweep handles only, in `inputs`
   const uint16_t* links = nullptr;   // links sweeps only, in `inputs`: HostSetup::links
+  const SweepOutage* outages = nullptr;  // outage sweeps only, in `inputs`: HostSetup::outages
   // the read-out buffers, allocated on first use and grown by grow_buffer
   DeviceMemory logs;       // lbft_commit_logs: [I][cap]
   DeviceMemory times_out;  // lbft_commit_times: [I][N][cap] committed, then [I][cap] proposed
@@ -310,6 +311,15 @@ int lbft_create_sweep_links(const lbft_config* config, const lbft_param_set* set
   });
 }
 
+int lbft_create_sweep_outages(const lbft_config* config, const lbft_param_set* sets, const lbft_fault_set* faults,
+                              const uint64_t* voting_rights, const uint32_t* committee_sizes, const uint32_t* link_latency,
+                              const lbft_outage* outages, uint32_t num_sets, const uint32_t* set_of_instance, lbft_sim** out_sim) {
+  return create_handle(config, out_sim, [&](HostSetup& hs) {
+    return hs.build_sweep_outages(*config, sets, faults, voting_rights, committee_sizes, link_latency, outages, num_sets,
+                                  set_of_instance);
+  });
+}
+
 }  // extern "C"
 
 // The device half of the lbft_create* entry points, once the host setup `s->hs` is built.  On failure the partial handle is
@@ -348,7 +358,7 @@ static int create_on_device(std::unique_ptr<lbft_sim> s, const lbft_config* conf
     return at;
   };
   const size_t zig_x = stage(hs.zig_x), zig_f = stage(hs.zig_f), delay_thr = stage(hs.delay_thr), sets = stage(set_table),
-               duration = stage(hs.duration), period = stage(hs.period), weights = stage(hs.weights), set_of = stage(hs.set_of),
+               outages = stage(hs.outages), duration = stage(hs.duration), period = stage(hs.period), weights = stage(hs.weights), set_of = stage(hs.set_of),
                links = stage(hs.links), leader = stage(hs.leader);
   CREATE_TRY(s->dev_alloc(s->inputs, seeds_bytes + tables.size()));
   CREATE_TRY(cudaMemcpy(s->inputs.at(seeds_bytes), tables.data(), tables.size(), cudaMemcpyHostToDevice));
@@ -378,6 +388,7 @@ static int create_on_device(std::unique_ptr<lbft_sim> s, const lbft_config* conf
     s->set_of = in.at<uint32_t>(set_of);
   }
   if (!hs.links.empty()) s->links = in.at<uint16_t>(links);
+  if (!hs.outages.empty()) s->outages = in.at<SweepOutage>(outages);
   P.state = s->state.at<uint32_t>();
   const DeviceMemory& out = s->outputs;
   const OutputLayout& at = s->regions;
@@ -513,7 +524,8 @@ static int enqueue_kernel(lbft_sim* s) {
   CUDA_TRY(cudaEventRecord(s->ev[2], s->stream));
   const KernelSel& k = s->hs.sel;
   const uint32_t records = s->hs.records();
-  const SweepParams sp{s->P, s->set_of, reinterpret_cast<const SweepSet*>(s->sets), records & 1u, (records >> 1) & 3u, s->links};
+  const SweepParams sp{s->P,      s->set_of,  reinterpret_cast<const SweepSet*>(s->sets), records & 1u, (records >> 1) & 3u,
+                       s->links, s->outages, s->hs.down_mask};
   const CtParams<Params> cp{s->P, s->times.at<int32_t>()};
   const CtParams<SweepParams> csp{sp, s->times.at<int32_t>()};
   cudaError_t e = k.ct ? (k.sweep ? (k.wide ? launch_ct_sweep_wide(k, csp, s->stream) : launch_ct_sweep_thread(k, csp, s->stream))

@@ -369,20 +369,33 @@ LBFT_HD uint32_t link_off_behind(const SweepSet* set) {
 #endif
 }
 
+// Where the outage windows of an outage sweep's set start in SweepParams::outages (Core::down_at), read the same way.
+static_assert(offsetof(SweepSetLinks, links) + offsetof(SweepLinks, outage_off) == 348, "the immediate below");
+LBFT_HD uint32_t outage_off_behind(const SweepSet* set) {
+#if defined(__CUDA_ARCH__)
+  uint32_t v;
+  asm volatile("ld.global.nc.u32 %0, [%1+348];" : "=r"(v) : "l"(set));
+  return v;
+#else
+  return reinterpret_cast<const SweepSetLinks*>(set)->links.outage_off;
+#endif
+}
+
 static_assert(offsetof(SweepParams, P) == 0, "Core::sweep_records: a sweep kernel's Params heads its SweepParams");
 
 // The records behind each set of a sweep's table (sweep_set_at): bit 0 faults, bit 1 rights, bit 2 the committee size (a
 // committee sweep's SweepParams::rights has bits 0 and 1 set: its table is a rights sweep's), bit 3 the link latencies (a links
-// sweep's SweepParams::links is not null; its rights bit is set too).
+// sweep's SweepParams::links is not null; its rights bit is set too), bit 4 the outage windows (an outage sweep's
+// SweepParams::outages is not null; its rights bit is set too, and its entries carry a links record whether or not bit 3 is set).
 LBFT_HD uint32_t sweep_records(const SweepParams& S) {
-  return (S.faults ? 1u : 0u) | (S.rights ? 2u : 0u) | ((S.rights & 2u) << 1) | (S.links ? 8u : 0u);
+  return (S.faults ? 1u : 0u) | (S.rights ? 2u : 0u) | ((S.rights & 2u) << 1) | (S.links ? 8u : 0u) | (S.outages ? 16u : 0u);
 }
 
 // Set s of a sweep's device table, whose entries are SweepSet, SweepSetFaults, SweepSetRights or SweepSetLinks by `records`
-// (bit 0: a fault record follows each set, bit 1: a rights record follows that, bit 3: a links record follows that; bit 2 does
-// not change the entry).
+// (bit 0: a fault record follows each set, bit 1: a rights record follows that, bit 3 or 4: a links record follows that; bit 2
+// does not change the entry).
 LBFT_HD const SweepSet* sweep_set_at(const SweepSet* sets, uint32_t s, uint32_t records) {
-  const size_t pitch = (records & 8)   ? sizeof(SweepSetLinks)
+  const size_t pitch = (records & 24)  ? sizeof(SweepSetLinks)
                        : (records & 2) ? sizeof(SweepSetRights)
                                        : ((records & 1) ? sizeof(SweepSetFaults) : sizeof(SweepSet));
   return reinterpret_cast<const SweepSet*>(reinterpret_cast<const char*>(sets) + pitch * s);
@@ -797,10 +810,14 @@ struct Core {
     else return (P.silent_mask >> n) & 1;
   }
   // SW: whether run() drops an event of `kind` for `receiver` from `sender` unhandled (a silent receiver handles nothing, and a
-  // silent sender's request is not answered), with one load of the mask.
+  // silent sender's request is not answered), with one load of the mask.  On an outage sweep the same holds for a node down at
+  // the pop clock (down_at): the host adds the windowed nodes to P.silent_mask, so this test is reached through any_silent()
+  // only on sweeps that have a silent or a windowed node, and an outage sweep carries fault records (faults()), so `mask` is
+  // still the set's silent nodes alone.
   LBFT_HD bool sweep_silent_drop(uint32_t kind, uint32_t receiver, uint32_t sender) const {
     const uint64_t mask = faults() ? silent_mask_behind(sw) : P.silent_mask;
-    return ((mask >> receiver) | (kind == EV_REQUEST ? mask >> sender : 0)) & 1;
+    if (((mask >> receiver) | (kind == EV_REQUEST ? mask >> sender : 0)) & 1) return true;
+    return down_at(receiver, clock) || (kind == EV_REQUEST && down_at(sender, clock));
   }
   // The plan's window count and length, read when init() draws the plan.  A set never has more windows than the layout;
   // init() leaves the layout's windows past the set's count empty ([0, 0): never open), so partitioned() and the send path stay
@@ -850,6 +867,29 @@ struct Core {
     return __ldg(table);
 #else
     return *table;
+#endif
+  }
+  // The outages of an outage sweep (bind_outages): whether node n is down at clock t, by its set's window.  down_mask() is the
+  // launch-uniform union of the nodes with a window in any set (a constant-bank read of SweepParams::down_mask on the device; on
+  // the host, where a harness may bind a bare Params, read only when bind_outages set bit 4), so a node without one costs one
+  // test.  As with the links, nothing is held through the loop: the set's schedule offset and the window are loaded where a
+  // pop is tested (sweep_silent_drop); push_timer tests the node's bit alone.
+  LBFT_HD void bind_outages(bool outage_sweep) { records = (records & ~16u) | (outage_sweep ? 16u : 0u); }
+  LBFT_HD uint64_t down_mask() const {
+#if defined(__CUDA_ARCH__)
+    return reinterpret_cast<const SweepParams*>(&P)->down_mask;
+#else
+    return (records & 16) ? reinterpret_cast<const SweepParams*>(&P)->down_mask : 0;
+#endif
+  }
+  LBFT_HD bool down_at(uint32_t n, int32_t t) const {
+    if (!((down_mask() >> n) & 1)) return false;
+    const SweepOutage* w = reinterpret_cast<const SweepParams*>(&P)->outages + outage_off_behind(sw) + n;
+#if defined(__CUDA_ARCH__)
+    const int2 v = __ldg(reinterpret_cast<const int2*>(w));
+    return t >= v.x && t < v.y;
+#else
+    return t >= w->from && t < w->until;
 #endif
   }
   // ------------------------------------------------------------------------------------------
@@ -1791,7 +1831,10 @@ struct Core {
   LBFT_HD void push_timer(uint32_t n, NodeRegs& d, int32_t t) {
     // (not while recording round switches: every pop is a DataWriter sampling point, data_writer.rs:34-50, so the
     // duplicate has to be popped where the reference pops it)
-    if (ELIDE && (uint32_t)t == d.f[F_LAST_TIMER]) {
+    // An outage sweep queues the duplicates of a node with a window (SW: its bit of down_mask, a constant-bank test): if the node
+    // is down at t, the reference pops both timers and drops both before the cancellation test, so the duplicate would count as
+    // popped but not cancelled.  Testing the window here instead holds its loads at every push site and spills the sweep kernels.
+    if (ELIDE && (uint32_t)t == d.f[F_LAST_TIMER] && !(SW && ((down_mask() >> n) & 1))) {
       // An UpdateTimerEvent for (n, t) is already pending with a smaller stamp.  The duplicate could
       // only ever be popped right after it (same time) and be cancelled by
       // ignore_scheduled_updates_until (simulator.rs:403-410) with no side effect: account for it
@@ -1910,7 +1953,8 @@ struct Core {
       proc1 += kind == EV_REQUEST;
       proc2 += kind == EV_RESPONSE;
       proc3 += kind == EV_TIMER;
-      // EXTENSION D.2: silent nodes handle nothing and answer no request
+      // EXTENSION D.2: silent nodes handle nothing and answer no request (SW: nor, on an outage sweep, a node while it is down;
+      // it keeps its state and acts again at the first event it handles after its window)
       if (MAY_SILENT && any_silent()) {
         bool drop;
         if constexpr (SW) drop = sweep_silent_drop(kind, receiver, sender);

@@ -292,10 +292,17 @@ struct SweepSetRights {
 
 // The link latencies of one parameter set of a links sweep (lbft_create_sweep_links): its N x N matrix of u16 milliseconds
 // starts at SweepParams::links[link_off] (entry [sender * N + receiver], N = Layout::num_nodes); sets with equal matrices share
-// one.
+// one.  On an outage sweep (lbft_create_sweep_outages) its N outage windows start at SweepParams::outages[outage_off] (0 and
+// unread on every other sweep, and link_off unread when SweepParams::links is null); sets with equal schedules share one.
 struct SweepLinks {
   uint32_t link_off;
-  uint32_t pad;
+  uint32_t outage_off;
+};
+// One node's outage window of an outage sweep, clamped to [0, max_clock + 1]: down at clock t iff from <= t < until (an empty
+// window is stored as {0, 0}).
+struct SweepOutage {
+  int32_t from;
+  int32_t until;
 };
 // One entry of a links sweep's device table: a rights sweep's entry (a links sweep carries fault and rights records for every
 // set) and its links record behind it (sim_core.cuh Core::link_latency).
@@ -317,7 +324,11 @@ struct SweepParams {
   uint32_t rights;         // bit 0: a rights sweep, whose instances take their voting rights, quorum and leaders from their set's
                            // record; bit 1: a committee sweep (a rights sweep too), whose instances take their committee size from it
   const uint16_t* links;   // a links sweep (a rights sweep too), whose instances add their set's link latencies to every send: the
-                           // sets' matrices (SweepLinks); null on every other sweep
+                           // sets' matrices (SweepLinks); null on every other sweep (and on an outage sweep without matrices)
+  const SweepOutage* outages;  // an outage sweep (a SweepSetLinks table), whose instances drop the events of a node while it is
+                               // down: the sets' schedules of N windows (SweepLinks::outage_off); null on every other sweep
+  uint64_t down_mask;          // an outage sweep: the nodes with a non-empty window in any set, the launch-uniform test in front
+                               // of every window lookup (Core::down_mask); 0 on every other sweep
 };
 
 }  // namespace lbft

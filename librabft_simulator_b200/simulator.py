@@ -571,13 +571,31 @@ class BatchSimulator:
 @dataclass(frozen=True)
 class FaultSet:
     """The fault model of one point of a sweep: the silent (crashed) nodes, by index, and the random partition plan — what
-    ``BatchSimulator``'s ``silent`` / ``partition_windows`` / ``partition_max_len`` give a whole batch."""
+    ``BatchSimulator``'s ``silent`` / ``partition_windows`` / ``partition_max_len`` give a whole batch — and the timed outages:
+    ``((node, down_from, down_until), ...)``, at most one per node, in ms of global clock.  The node is down at clock t iff
+    ``down_from <= t < down_until`` (``down_until`` None: it never recovers).  While down it handles no event and answers no
+    request; it keeps its state and acts again at the first event addressed to it after the window
+    (``lbft_create_sweep_outages``)."""
     silent: tuple = ()
     partition_windows: int = 0
     partition_max_len: int = 0
+    outages: tuple = ()
 
     def __post_init__(self):
         object.__setattr__(self, "silent", tuple(int(n) for n in self.silent))  # (a list or array compares, and hashes, as a tuple)
+        out = []
+        for w in self.outages:
+            node, start, end = w
+            out.append((int(node), int(start), None if end is None else int(end)))
+        nodes = [w[0] for w in out]
+        if len(set(nodes)) != len(nodes):
+            raise ValueError("FaultSet.outages takes at most one window per node")
+        object.__setattr__(self, "outages", tuple(out))
+
+    def has_fault_model(self):
+        """Whether the silent nodes or the partition plan differ from none (what ``lbft_fault_set`` carries; the outages are
+        passed apart)."""
+        return bool(self.silent) or bool(self.partition_windows) or bool(self.partition_max_len)
 
     def to_c(self):
         mask = 0
@@ -644,6 +662,8 @@ class SweepSimulator(BatchSimulator):
     set's delay, node config, faults, voting rights and committee size computes for it.  And the link latencies: when a set
     carries a matrix (``ParamSet.link_latency``, ``lbft_create_sweep_links``), every network message from node a to node b of
     an instance of that set arrives ``link_latency[a][b]`` ms later than its drawn delay says; sets without one get zeros.
+    And the outages: when a set's ``FaultSet`` carries timed outages (``lbft_create_sweep_outages``), each of its nodes with a
+    window handles nothing while it is down; sets without any get none.
     Running, re-seeding (the set assignment stays), streaming and reading results work as on a ``BatchSimulator``."""
 
     def __init__(self, seeds, num_nodes, param_sets, set_of_instance, **shared):
@@ -695,9 +715,9 @@ class SweepSimulator(BatchSimulator):
     def create(self, max_clock):
         """``lbft_create_sweep``, or ``lbft_create_sweep_faults`` when some set has faults, or ``lbft_create_sweep_rights``
         when some set has voting rights, or ``lbft_create_sweep_committees`` when some set has its own committee size, or
-        ``lbft_create_sweep_links`` when some set has link latencies: validate every set, build the per-set host tables,
-        allocate device state."""
-        per_set = any(p.faults != FaultSet() for p in self.param_sets)
+        ``lbft_create_sweep_links`` when some set has link latencies, or ``lbft_create_sweep_outages`` when some set's faults
+        carry outages: validate every set, build the per-set host tables, allocate device state."""
+        per_set = any(p.faults.has_fault_model() for p in self.param_sets)
         if per_set and (self.silent is not None or self.partition_windows or self.partition_max_len):
             raise ValueError("a sweep takes silent nodes and partitions either per set (ParamSet.faults) or shared (silent / "
                              "partition_windows / partition_max_len), not both")
@@ -711,7 +731,15 @@ class SweepSimulator(BatchSimulator):
         so = ctypes.c_void_p(self.set_of_instance.ctypes.data)
         faults = (_lib.LbftFaultSet * len(self.param_sets))(*[p.faults.to_c() for p in self.param_sets]) if per_set else None
         links = self._link_table()
-        if links is not None:
+        outages = self._outage_table()
+        if outages is not None:
+            sizes = np.ascontiguousarray(self._committee_sizes(), dtype=np.uint32) if self._committees() else None
+            _lib.check(self._lib.lbft_create_sweep_outages(
+                ctypes.byref(cfg), sets, faults, None if rights is None else ctypes.c_void_p(rights.ctypes.data),
+                None if sizes is None else ctypes.c_void_p(sizes.ctypes.data),
+                None if links is None else ctypes.c_void_p(links.ctypes.data), outages, len(self.param_sets), so,
+                ctypes.byref(handle)))
+        elif links is not None:
             sizes = np.ascontiguousarray(self._committee_sizes(), dtype=np.uint32) if self._committees() else None
             _lib.check(self._lib.lbft_create_sweep_links(
                 ctypes.byref(cfg), sets, faults, None if rights is None else ctypes.c_void_p(rights.ctypes.data),
@@ -771,6 +799,20 @@ class SweepSimulator(BatchSimulator):
             if (m < 0).any() or (m > 65535).any():
                 raise ValueError("parameter set %d: link_latency entries must be in 0..65535 ms" % s)
             out[s, :n, :n] = m
+        return out
+
+    def _outage_table(self):
+        """The [num_sets * num_nodes] ``lbft_outage`` windows of an outage sweep (empty ones for nodes without a window, and
+        ``down_until`` None as the largest int64), or None when no set carries any."""
+        if all(not p.faults.outages for p in self.param_sets):
+            return None
+        N = self.num_nodes
+        out = (_lib.LbftOutage * (len(self.param_sets) * N))()
+        for s, p in enumerate(self.param_sets):
+            for node, start, end in p.faults.outages:
+                if not 0 <= node < N:
+                    raise ValueError("parameter set %d: outage node %d is not in 0..%d" % (s, node, N - 1))
+                out[s * N + node] = _lib.LbftOutage(start, _lib.INT64_MAX if end is None else end)
         return out
 
     def nodes_of_instance(self):
